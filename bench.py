@@ -38,27 +38,11 @@ def measured_peak():
                     return float(j[k]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
-
-
-def traffic_from_capture(kernel, log2n):
-    """DRAM bytes per launch of `kernel` from the committed ncu capture (profiles/ncu_traffic.json: a list of
-    {kernel, log2n, dram_bytes, source_sha16, capture}); None unless the entry was captured from the current kernel source."""
-    import hashlib
-    try:
-        ent = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-        src = os.path.join(ROOT, "distributedarrays.jl_b200", "csrc", "dab_elementwise.cu")
-        sha = hashlib.sha256(open(src, "rb").read()).hexdigest()[:16]
-        for e in ent:
-            if e.get("kernel") == kernel and int(e.get("log2n", -1)) == int(log2n) and e.get("source_sha16") == sha:
-                return float(e["dram_bytes"])
-    except Exception:
-        pass
-    return None
+    return 3350.0, "datasheet"   # H100 SXM HBM3 data-sheet bandwidth, not a measured rate
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (read-only queries)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -274,6 +258,28 @@ def parity_halo(dab, rt, dst, seed, rows_total, r0, c0):
 
 
 
+DUMP_WINDOWS, DUMP_WINDOW = 512, 4096     # 2^21 Float32 values of y: 8 MiB, well inside the 64 MB budget of a dump
+
+
+def dump_outputs(dab, rt, out_dir, y, s):
+    """What the last timed step handed its caller: ``sum.npy`` (the Float32 s = sum(y)) and a fixed, seeded sample of y = a.*x .+ b,
+    ``y_windows.npy`` (DUMP_WINDOWS x DUMP_WINDOW Float32, windows of this rank's localpart) at ``y_window_offsets.npy`` (Float64 element
+    offsets).  The inputs come from the counter-based generator with a fixed seed, so two builds run with the same arguments can be
+    compared output for output."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    ch = dab.localpart(y)
+    n = ch.size
+    w = min(DUMP_WINDOW, n)
+    rng = np.random.default_rng(SEED + 4242)
+    offs = np.sort(rng.integers(0, n - w + 1, DUMP_WINDOWS))
+    windows = np.stack([_d2h_window(dab, rt, ch, int(o), w) for o in offs]).astype(np.float32)
+    np.save(os.path.join(out_dir, "sum.npy"), np.array([s], dtype=np.float32))
+    np.save(os.path.join(out_dir, "y_windows.npy"), windows)
+    np.save(os.path.join(out_dir, "y_window_offsets.npy"), offs.astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -285,6 +291,7 @@ def main():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-extras", action="store_true")
     ap.add_argument("--no-parity", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last step computed to DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -368,8 +375,10 @@ def main():
     launches = rt.launches() - l0
     ms = max_over_ranks(ms)
     value = 12.0 * N * args.steps / (ms * 1e-3) / 1e9
+    if args.dump_outputs and rank == 0:
+        dump_outputs(dab, rt, args.dump_outputs, y, s)
 
-    # ---- per-kernel timings (same resident data; inputs 4 GiB >> 126 MB L2, so no flush needed)
+    # ---- per-kernel timings (same resident data; inputs 4 GiB >> 50 MB L2, so no flush needed)
     ms_bc, _ = timed(lambda: dab.broadcast_into(y, f, x), args.steps)
     bc_entry = rt.last_kernel  # which C-ABI entry point served the broadcast (dab_affine = the hand-written kernel)
     ms_sum, _ = timed(lambda: dab.sum(y), args.steps)
@@ -476,8 +485,7 @@ def main():
                 ms_h, _ = timed(lambda: sub.copy_to(dst), reps)
                 ms_h = max_over_ranks(ms_h)
                 extras["halo_getindex"] = {"GBs_per_reader": 4.0 * 32768 * 2048 * reps / (ms_h * 1e-3) / 1e9, "slab_bytes": 4 * 32768 * 2048,
-                                           "peak_GBs": 770.0, "what": "every rank pulls a 256 MiB slab of its right neighbour's chunk over NVLink (CUDA-IPC peer loads)"}
-                extras["halo_getindex"]["frac_of_peak"] = extras["halo_getindex"]["GBs_per_reader"] / 770.0
+                                           "what": "every rank pulls a 256 MiB slab of its right neighbour's chunk over NVLink (CUDA-IPC peer loads)"}
                 if not args.no_parity:
                     parity["checks"]["halo_getindex"] = parity_halo(dab, rt, dst, SEED + 1, dimsA[0], I[0][0] - 1, I[1][0] - 1)
                 dst.free()
@@ -493,7 +501,7 @@ def main():
                                        "results PUT into the y owners' exchange arena over NVLink, device-side barriers, one fused beta-scale + ordered add!"}
             xv.close()
             xt.close()
-            # Level-3 widening (K12): C = A*B through the public API (tile products on the tcgen05 3xTF32 kernel, B blocks halo-fetched,
+            # Level-3 widening (K12): C = A*B through the public API (tile products on the wgmma 3xTF32 kernel, B blocks halo-fetched,
             # tile results shipped to the owners of C, ordered add!); useful flops = 2*m*n*k, the tensor core executes 3x that in TF32
             try:
                 nB = 2048
@@ -505,7 +513,7 @@ def main():
                 pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))).get("bf16_tflops") if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else None
                 extras["matmat_A_B"] = {"useful_TFLOPs": tf, "tf32_mma_TFLOPs": 3 * tf, "ms": ms_g / 3, "dims": [dimsA[0], dimsA[1], nB],
                                         "frac_of_tf32_peak": (3 * tf / (world * pk / 2)) if pk else None,
-                                        "what": "A*B (mul!(C, A, B)): dab_gemm tiles = TMA + tcgen05.mma kind::tf32 with TMEM accumulators, 3xTF32 "
+                                        "what": "A*B (mul!(C, A, B)): dab_gemm tiles = TMA + wgmma.mma_async tf32 with register accumulators, 3xTF32 "
                                                 "error-compensated; tf32 peak taken as measured bf16 peak / 2"}
                 if not args.no_parity:
                     Cm = A @ Bm
@@ -577,17 +585,12 @@ def main():
     line = {"metric": "GB/s for map! and sum on Float32 DArray", "value": value, "unit": "GB/s", "n_gpus": world, "steps": args.steps,
             "warmup": warmup, "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "f32", "data": "synthetic",
-            "config": {"workload": workload, "l2": "inputs (4 GiB/GPU) >> 126 MB L2, no flush needed", "grid": list(x.layout.grid),
+            "config": {"workload": workload, "l2": "inputs (4 GiB/GPU) >> 50 MB L2, no flush needed", "grid": list(x.layout.grid),
                        "combine": ("single chunk" if world == 1 else
                                    "fused in the reduce kernel: peer-memory all-gather of the P chunk results over NVLink + ordered left fold"
                                    if rt.fused_combine else "NCCL all-gather of the P chunk results + ordered left fold")},
             "roofline": {"bound": "hbm", "kernel": "ew1_kernel<float, AffineF<float>, 2>", "entry": bc_entry, "achieved": bc_gbs, "peak": peak,
-                         "peak_kind": peak_kind, "unit": "GB/s", "frac": bc_gbs / peak,
-                         # dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed ncu --set full capture of THIS
-                         # kernel source at this size (profiles/ncu_traffic.json, written by tools/ncu_summary.py); null when the
-                         # capture is missing or older than the kernel source's recorded hash
-                         "traffic": traffic_from_capture("ew1_kernel", args.log2n),
-                         "algorithmic_bytes_per_launch": 8 * n_per},
+                         "peak_kind": peak_kind, "unit": "GB/s", "frac": bc_gbs / peak, "algorithmic_bytes_per_launch": 8 * n_per},
             "kernels": {"broadcast_GBs_per_gpu": bc_gbs, "sum_GBs_per_gpu": sum_gbs, "maximum_GBs_per_gpu": max_gbs,
                         "broadcast_frac": bc_gbs / peak, "sum_frac": sum_gbs / peak, "maximum_frac": max_gbs / peak,
                         "ms_broadcast": ms_bc / args.steps, "ms_sum": ms_sum / args.steps},

@@ -1,4 +1,4 @@
-"""distributedarrays.jl_b200 -- B200-native backend for the DArray map!/broadcast + mapreduce hot path.
+"""distributedarrays.jl_b200 -- H100-native backend for the DArray map!/broadcast + mapreduce hot path.
 
 Import it as ``darray_b200`` (the directory name is not a Python identifier; ``darray_b200.py`` at the repo root is a
 loader shim).  The public names mirror DistributedArrays.jl's for this path: ``DArray``, ``distribute``, ``localpart``,
@@ -7,7 +7,7 @@ loader shim).  The public names mirror DistributedArrays.jl's for this path: ``D
 ``maximum``, ``minimum``, ``all``, ``any``, ``count``, ``extrema``, ``Array(d)`` (``to_array``), range ``getindex``.
 
 Everything computes on the GPU through ``csrc/libdab200.so`` (C ABI: ``include/dab200.h``).  There is no CPU fallback:
-importing works anywhere, but the first op without the built extension or without a B200 raises.
+importing works anywhere, but the first op without the built extension or without an H100 raises.
 """
 from . import _lib
 from ._lib import ArgumentError, DabError, DimensionMismatch, UnsupportedError

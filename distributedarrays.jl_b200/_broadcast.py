@@ -1,4 +1,4 @@
-"""Distributed broadcast and map / map!: the reference's ``src/broadcast.jl`` and ``src/mapreduce.jl:3-12`` on B200.
+"""Distributed broadcast and map / map!: the reference's ``src/broadcast.jl`` and ``src/mapreduce.jl:3-12`` on H100.
 
 The reference receives a Julia closure and lets Julia's JIT fuse the whole expression tree into one loop per localpart
 (``copyto!(localpart(dest), lbc)``, src/broadcast.jl:80).  A closure cannot cross a C ABI, so here the Python callable
@@ -8,7 +8,7 @@ the tree is lowered to ONE kernel launch per localpart:
   * ``a*x + b`` (any spelling, e.g. ``2x+1``)        -> ``dab_affine``        (hand-written float4 streaming kernel)
   * a single unary / binary op                        -> ``dab_unary`` / ``dab_binary`` / ``dab_binary_scalar``
   * anything else (nested, N-ary, extruded size-1 dims, mixed element types)
-                                                      -> ``dab_broadcast_expr`` (NVRTC-compiled fused kernel, sm_100a)
+                                                      -> ``dab_broadcast_expr`` (NVRTC-compiled fused kernel, sm_90a)
 
 Semantics kept from the reference: axes check and ``DimensionMismatch`` (src/broadcast.jl:66); plain arrays are
 distributed (``bcdistribute``, :124-137); per destination chunk every argument is cut with ``_bcview`` (:103-120; size-1
@@ -40,7 +40,7 @@ class _TagTypes(dict):
     argument, test/darray.jl:286-294): there are no Int128 arrays, so every place that needs an element type for it refuses."""
 
     def __missing__(self, tag):
-        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"values of type {tag} have no array element type on the B200 backend "
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"values of type {tag} have no array element type on the GPU backend "
                                     "(Int128 is served as the value type of mapreduce(f, op, d) only)")
 
 
@@ -53,7 +53,7 @@ _CT = {"bool": "bool", "i32": "int", "i64": "long long", "i128": "i128", "f32": 
 def tag_of(dtype) -> str:
     dt = np.dtype(dtype)
     if dt not in _TAG:
-        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"element type {dt} not served by the B200 backend")
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"element type {dt} not served by the GPU backend")
     return _TAG[dt]
 
 
@@ -145,7 +145,7 @@ class Expr:
         pe = Expr.wrap(p)
         if promote(self.jt, pe.jt)[0] != "f":
             # Julia's integer ^ is power_by_squaring and throws DomainError for negative exponents: no kernel serves it
-            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "integer ^ integer is not served by the B200 backend")
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "integer ^ integer is not served by the GPU backend")
         return binop("pow", self, pe)
 
     def __bool__(self):

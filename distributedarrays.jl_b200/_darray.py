@@ -1,4 +1,4 @@
-"""DArray on B200: each localpart lives in one GPU's HBM.
+"""DArray on H100: each localpart lives in one GPU's HBM.
 
 Python mirror of the reference's L2 layer (src/darray.jl) for exactly what the hot path needs: the ``DArray`` struct
 (:25-31), constructors ``DArray(init, dims[, procs, dist])`` (:159-174), ``DArray(refs)`` (:183-216),
@@ -33,7 +33,7 @@ _NP = {_lib.F32: np.dtype(np.float32), _lib.F64: np.dtype(np.float64), _lib.I32:
 def dab_dtype(dt) -> int:
     dt = np.dtype(dt)
     if dt not in _DT:
-        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"element type {dt} is not served by the B200 backend (no host fallback)")
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"element type {dt} is not served by the GPU backend (no host fallback)")
     return _DT[dt]
 
 
@@ -235,7 +235,7 @@ class DArray:
 
     def share(self):
         """Collective: exchange CUDA IPC handles of all chunks so that any rank can read any chunk over NVLink
-        (the B200 counterpart of every worker being able to ``remotecall_fetch`` any chunk, src/darray.jl:458)."""
+        (the GPU counterpart of every worker being able to ``remotecall_fetch`` any chunk, src/darray.jl:458)."""
         if self.rt.world == 1:
             self._handles = {}
             return self
@@ -288,7 +288,7 @@ class DArray:
                 idx.append(v)
                 drop.append(False)
             else:
-                raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"index type {type(k).__name__} is not served by the B200 backend")
+                raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"index type {type(k).__name__} is not served by the GPU backend")
         return SubDArray(self, tuple(J), tuple(drop), tuple(idx) if builtins_any(i is not None for i in idx) else None)
 
     def __array__(self, dtype=None, copy=None):

@@ -134,7 +134,7 @@ def lib() -> C.CDLL:
     if _lib is None:
         if not os.path.exists(SO_PATH):
             raise RuntimeError(
-                f"{SO_PATH} is missing: the sm_100a CUDA extension has not been built "
+                f"{SO_PATH} is missing: the sm_90a CUDA extension has not been built "
                 "(run `python -c 'import __graft_entry__ as g; g.build()'` or `make -C distributedarrays.jl_b200/csrc`). "
                 "There is no CPU fallback for the DArray hot path.")
         L = C.CDLL(SO_PATH, mode=C.RTLD_GLOBAL)

@@ -9,7 +9,7 @@ Mirrors the reference's ``src/linalg.jl``:
 * ``lmul!(D::Diagonal, DA)`` / ``rmul!(DA, D::Diagonal)`` (:169-187)                      -> fused broadcast with extrusion
 
 * ``mul!(C::DMatrix, A::DMatrix, B::AbstractMatrix, a, b)`` and the Adjoint/Transpose forms, ``A*B``, ``A'*B`` (:189-311)
-                                                                                          -> K12 ``dab_gemm`` (tcgen05 3xTF32 tile
+                                                                                          -> K12 ``dab_gemm`` (wgmma 3xTF32 tile
   products for Float32, SIMT tiles for Float64 / Int32 / Int64) + the same exchange of the tile results to the owners of C
 """
 from __future__ import annotations

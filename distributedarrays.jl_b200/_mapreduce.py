@@ -1,4 +1,4 @@
-"""Distributed reductions: the reference's ``src/mapreduce.jl:17-131`` on B200.
+"""Distributed reductions: the reference's ``src/mapreduce.jl:17-131`` on H100.
 
   * ``reduce`` / ``mapreduce`` / ``sum`` / ``prod`` / ``maximum`` / ``minimum``  -- ``Base._mapreduce(f, op, ::IndexCartesian,
     d::DArray)`` (reference src/mapreduce.jl:29-35): ONE streaming kernel per localpart, the P chunk results are gathered on

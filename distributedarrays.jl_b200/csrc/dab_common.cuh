@@ -1,4 +1,4 @@
-// dab_common.cuh -- shared internals of libdab200.so (sm_100a only).
+// dab_common.cuh -- shared internals of libdab200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 

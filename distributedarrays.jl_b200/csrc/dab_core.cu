@@ -121,9 +121,9 @@ int32_t dab_init(int32_t device, dab_ctx** out) {
     INIT_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     INIT_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10) {
+    if (prop.major != 9 || prop.minor != 0) {   // sm_90a code (wgmma, TMA) runs on compute capability 9.0 only
         delete ctx;
-        return dab_fail(nullptr, DAB_ERR_UNSUPPORTED, "device %d is sm_%d%d; libdab200 is built for sm_100a only", device,
+        return dab_fail(nullptr, DAB_ERR_UNSUPPORTED, "device %d is sm_%d%d; libdab200 is built for sm_90a only", device,
                         prop.major, prop.minor);
     }
     ctx->sm_count = prop.multiProcessorCount;

@@ -1,4 +1,4 @@
-// dab_elementwise.cu -- K1-K3: the fused per-localpart broadcast / map! loop, as streaming sm_100a kernels.
+// dab_elementwise.cu -- K1-K3: the fused per-localpart broadcast / map! loop, as streaming sm_90a kernels.
 //
 // Replaces Base.Broadcast.copyto!(localpart(dest), lbc) (reference src/broadcast.jl:80), copy(lbc) (:96) and
 // map!(f, localpart(dest), makelocal(src, ...)) (src/mapreduce.jl:8).
@@ -17,9 +17,8 @@ namespace {
 constexpr int EW_THREADS = 256;
 
 // One CTA per 256*UNROLL-vector tile ("flat" grid): the hardware block scheduler hands tiles out in address order as CTAs
-// retire, so the set of concurrently open DRAM pages stays a compact sliding window.  Measured on B200 (tools/sweep_stream.cu,
-// profiles/sweep_r1.txt): 6.94 TB/s for y = a*x+b at 2^30 and 2^31 floats, vs 5.95 TB/s for a persistent grid-stride loop whose
-// CTAs drift apart, 6.65 TB/s for a TMA (cp.async.bulk + mbarrier) ring and 6.6 TB/s for cudaMemcpy D2D.
+// retire, so the set of concurrently open DRAM pages stays a compact sliding window; a persistent grid-stride loop lets its CTAs
+// drift apart and was slower when the kernel was designed, as was a TMA (cp.async.bulk + mbarrier) ring.
 // The extra last CTA handles the remainder vectors and the unaligned head / tail elements.
 template <typename T, typename F, int UNROLL>
 __global__ void __launch_bounds__(EW_THREADS) ew1_kernel(T* y, const T* x, size_t n, size_t head, F f) {
@@ -107,8 +106,8 @@ __global__ void __launch_bounds__(EW_THREADS) ew2_scalar_kernel(T* z, const T* x
 // The north-star design sketch asks for "TMA-staged tiles into shared memory"; this is that kernel: one elected thread streams
 // 32 KiB tiles global -> shared with cp.async.bulk (SASS UBLKCP.S.G) completing on an mbarrier ring (3 stages), all threads apply f
 // in place in shared memory, then the elected thread streams the tile shared -> global (UBLKCP.G.S, bulk async-group).  Persistent,
-// one CTA per SM.  Measured on B200 (tools/sweep_stream.cu, profiles/sweep_r1*.txt): 6.65-6.68 TB/s vs 6.95 TB/s for the flat LDG
-// kernel above -- every element is touched once, so staging buys no reuse and only adds a hop; it is therefore NOT the default.
+// one CTA per SM.  Every element is touched once, so staging buys no reuse over the flat LDG kernel above and only adds a hop; it is
+// therefore NOT the default (bench.py times both: extras.broadcast_tma_variant).
 // Bit-identical results (tests/test_gpu_hotpath.py::test_affine_tma_variant).
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {

@@ -5,19 +5,17 @@
 // :218-226).  Column-major (Julia) operands:  R[m x n] = op(A) * B,  op(A) = A (m x k) or A^T (A stored k x m),  B is k x n.
 // The caller combines the tile results exactly as the reference does (scale C by beta, add!(localpart(C), R, alpha) per tile).
 //
-// Float32 -> gemm_tf32x3_kernel, hand-written for sm_100a:
-//   * operands arrive by TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B tensor maps; SASS UTMALDG) into a 3-stage shared-memory ring,
-//     completion on mbarriers; out-of-range rows / columns / k are zero-filled by the TMA unit, so ragged edges need no special code
-//   * four converter warps split every fp32 tile into tf32 "hi" (round-to-nearest) and "lo" (the rounded remainder) in place
-//   * ONE thread issues tcgen05.mma.kind::tf32 (SASS UTCHMMA... ) with the accumulators in TENSOR MEMORY: per 8-deep k-step the three
-//     products a_lo*b_hi + a_hi*b_lo + a_hi*b_hi ("3xTF32": the dropped a_lo*b_lo term is 2^-22 relative), M = N = 128
-//   * two-level accumulation, because the tensor core TRUNCATES its fp32 accumulator on every tcgen05.mma (measured: ~2^-25 relative
-//     bias per accumulating instruction, linear in their number -- 3e-6 after k = 256 on same-sign data): a TMEM accumulator only sums
-//     KC consecutive k (default 64 = 8 instructions), the two correction products go to a SEPARATE accumulator (their truncation is
-//     2^-11 smaller), and eight drain warps pull each finished pair of partial tiles out of TMEM (tcgen05.ld, SASS LDTM) and add them to
-//     fp32 registers with round-to-nearest while the tensor core already works on the other accumulator set (all 512 TMEM columns)
-//   * epilogue: the drain warps hold one output row per thread (TMEM lane == row), so consecutive lanes store consecutive rows of a
-//     column-major C: coalesced 128-byte stores
+// Float32 -> gemm_tf32x3_kernel, hand-written for sm_90a (Hopper):
+//   * operands arrive by TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B tensor maps) into a 6-stage shared-memory ring, completion on
+//     mbarriers; out-of-range rows / columns / k are zero-filled by the TMA unit, so ragged edges need no special code.  One producer warp.
+//   * "3xTF32": per 8-deep k-step the three products a_lo*b_hi + a_hi*b_lo + a_hi*b_hi (the dropped a_lo*b_lo term is 2^-22 relative).
+//     The B tile (K-major in shared memory, as wgmma needs for tf32) is split into tf32 "hi" (round-to-nearest, in place) and "lo" (the
+//     rounded remainder) by the consumer threads.  A goes to the tensor core from REGISTERS: an untransposed column-major A is MN-major,
+//     which wgmma does not accept for tf32 from shared memory, so every thread loads its fragment from the swizzled tile and splits it there.
+//   * two consumer warpgroups issue wgmma.mma_async m64n128k8 (a_hi x [b_hi | b_lo]) and m64n64k8 (a_lo x b_hi); CTA tile 128 x 64
+//   * two-level accumulation, because the tensor core does not round its fp32 accumulator to nearest (the error grows with the number of
+//     accumulating instructions): the register accumulators only sum KC consecutive k (default 64), then each finished partial tile is
+//     added to fp32 registers with round-to-nearest
 // Everything else (Float64, Int32, Int64; Float32 operands whose base / leading dimension are not 16-byte aligned, which TMA cannot
 // address) -> gemm_simt_kernel: shared-memory tiled FMA kernel, fp64 with DFMA, integers wrap like Julia's.
 #include <cuda.h>
@@ -111,15 +109,16 @@ int32_t launch_simt(dab_ctx* ctx, int transA, size_t m, size_t n, size_t k, cons
     return DAB_OK;
 }
 
-// ======================================================================= tcgen05 3xTF32 kernel =======================================
-constexpr int TG_M = 128, TG_N = 128, TG_K = 32, TG_STAGES = 3;
-constexpr int TG_TILE_BYTES = TG_M * TG_K * 4;                   // 16 KiB: one operand tile (128 x 32 fp32)
-constexpr int TG_STAGE_BYTES = 4 * TG_TILE_BYTES;                // A_hi, A_lo, B_hi, B_lo
-constexpr int TG_THREADS = 448;                                  // warp 0 TMA, warp 1 MMA, warps 2-5 convert, warps 6-13 drain/epilogue
-constexpr int TG_DRAIN_THREADS = 256;                            // two warps per TMEM lane quarter, 64 accumulator columns each
+// ======================================================================= wgmma 3xTF32 kernel ==========================================
+constexpr int TG_M = 128, TG_N = 64, TG_K = 32, TG_STAGES = 6;
+constexpr int TG_A_BYTES = TG_M * TG_K * 4;                      // 16 KiB: one A tile (128 x 32 fp32)
+constexpr int TG_B_BYTES = TG_N * TG_K * 4;                      // 8 KiB: one B tile (32 x 64 fp32), K-major rows of 128 bytes
+constexpr int TG_STAGE_BYTES = TG_A_BYTES + 2 * TG_B_BYTES;      // A, B_hi, B_lo (B_lo right behind B_hi: [B_hi | B_lo] is one N = 128 operand)
+constexpr int TG_CONSUMERS = 256;                                // two warpgroups, 64 rows of the tile each
+constexpr int TG_THREADS = TG_CONSUMERS + 32;                    // + one TMA producer warp
 constexpr int TG_BAR_OFFSET = TG_STAGES * TG_STAGE_BYTES;
-constexpr int TG_SMEM_BYTES = TG_BAR_OFFSET + 256 + 1024;        // + barriers + slack for the 1024-byte alignment of the swizzle atoms
-constexpr int TG_TMEM_COLS = 512;                                // two sets of {main, correction} 128-column fp32 accumulators
+constexpr int TG_SMEM_BYTES = TG_BAR_OFFSET + 128 + 1024;        // + barriers + slack for the 1024-byte alignment of the swizzle atoms
+static_assert(TG_SMEM_BYTES <= 227 * 1024, "shared memory of one CTA");
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -147,65 +146,87 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
                  ::"r"(dst), "l"((uint64_t)map), "r"(bar), "r"(c0), "r"(c1)
                  : "memory");
 }
-// UMMA shared-memory matrix descriptor (sm_100 layout: start address, leading / stride byte offsets in 16-byte units, version 1,
-// layout type 2 = SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout_type = 2u) {
+// wgmma shared-memory matrix descriptor of a K-major operand in the 128-byte swizzle (the layout TMA's SWIZZLE_128B writes): start
+// address, leading byte offset (unused by swizzled K-major operands), stride byte offset = 1024 (8-row atoms of 128-byte rows), layout 1
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;   // descriptor version (Blackwell)
-    d |= (uint64_t)layout_type << 61;   // 2 = SWIZZLE_128B (16-byte atoms), 1 = SWIZZLE_128B with 32-byte atoms
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(1024 >> 4) << 32;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D (64 x N fp32, registers) (+)= A (64 x 8 tf32, registers: rows g / g+8, k t / t+4 of the warp's 16-row slice) x B (8 x N tf32, shared)
+__device__ __forceinline__ void wgmma_n128(float* d, const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "setp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {   // 32 lanes x 16 consecutive fp32 columns (SASS LDTM.x16)
+__device__ __forceinline__ void wgmma_n64(float* d, const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]),
-          "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr));
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
 }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit_wait() {
+    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+}
+// keeps the compiler from moving reads / writes of an accumulator register across the asynchronous wgmma that owns it
+__device__ __forceinline__ void fence_operand(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+
 // fp32 -> (tf32 hi, tf32 lo) with INTEGER arithmetic: round-to-nearest (ties away, the semantics of cvt.rna.tf32.f32) is "add half an ulp of
-// the 13 dropped bits, clear them".  cvt.rna.tf32.f32 issues at a fraction of the ALU rate on sm_100a and made the four converter warps the
-// limiter of the whole kernel (2 conversions per element); IADD / LOP3 / FSUB run at full rate.  The tensor core ignores the low 13 bits of
-// a tf32 operand, so "lo" only needs the rounding add, not the mask.
-__device__ __forceinline__ float tf32_rn_hi(float v) { return __uint_as_float((__float_as_uint(v) + 0x1000u) & 0xffffe000u); }
-__device__ __forceinline__ float tf32_rn_lo(float r) { return __uint_as_float(__float_as_uint(r) + 0x1000u); }
+// the 13 dropped bits, clear them"; IADD / LOP3 / FSUB run at full rate, cvt.rna.tf32.f32 does not.  Both halves have their low 13 bits
+// cleared, so the products do not depend on how the tensor core treats the bits a tf32 operand drops.
+__device__ __forceinline__ float tf32_rn(float v) { return __uint_as_float((__float_as_uint(v) + 0x1000u) & 0xffffe000u); }
+__device__ __forceinline__ float tf32_trunc(float v) { return __uint_as_float(__float_as_uint(v) & 0xffffe000u); }
 __device__ __forceinline__ float4 split_tf32(float4& v) {   // v <- hi (tf32, round to nearest), returns lo = tf32_rn(v - hi)
     float4 lo;
-    const float hx = tf32_rn_hi(v.x), hy = tf32_rn_hi(v.y), hz = tf32_rn_hi(v.z), hw = tf32_rn_hi(v.w);
-    lo.x = tf32_rn_lo(__fsub_rn(v.x, hx));
-    lo.y = tf32_rn_lo(__fsub_rn(v.y, hy));
-    lo.z = tf32_rn_lo(__fsub_rn(v.z, hz));
-    lo.w = tf32_rn_lo(__fsub_rn(v.w, hw));
+    const float hx = tf32_rn(v.x), hy = tf32_rn(v.y), hz = tf32_rn(v.z), hw = tf32_rn(v.w);
+    lo.x = tf32_rn(__fsub_rn(v.x, hx));
+    lo.y = tf32_rn(__fsub_rn(v.y, hy));
+    lo.z = tf32_rn(__fsub_rn(v.z, hz));
+    lo.w = tf32_rn(__fsub_rn(v.w, hw));
     v = make_float4(hx, hy, hz, hw);
     return lo;
 }
 
-// RAWHI (opt-in, dab_set_option "gemm_rawhi"): the tensor core reads an fp32 word as tf32 by IGNORING its low 13 mantissa bits (verified on
-// B200: results identical to an explicit truncation), so the raw tile can serve as the "hi" operand as it is; the converters then only write
-// "lo" = tf32_rn(v - trunc_tf32(v)) and the shared-memory traffic of the conversion drops from 3 to 2 tile passes per operand (the kernel is
-// shared-memory-bandwidth bound: tensor-core operand reads + conversion = ~190 KiB per 32-deep k-block against 128 B/clk).  Measured at
-// 8192^3: +2-5 % speed, but the always-positive remainder of a truncation makes the dropped a_lo*b_lo term a bias: max error 1.02e-6 instead of
-// 0.93e-6 at k = 8192 on same-sign data.  The default keeps the round-to-nearest split (hi rewritten in place), which stays inside 1e-6.
+// RAWHI (opt-in, dab_set_option "gemm_rawhi"): the B tile stays in shared memory as it arrived and serves as the "hi" operand (the tensor
+// core reads an fp32 word as tf32 by ignoring its low 13 mantissa bits), so the converters only write "lo" = tf32_rn(v - trunc_tf32(v)) and
+// the shared-memory traffic of the conversion drops from 3 to 2 tile passes.  A is split in registers: hi = trunc_tf32(v), same remainder.
+// The always-positive remainder of a truncation makes the dropped a_lo*b_lo term a bias; the default keeps the round-to-nearest split.
 __device__ __forceinline__ float4 lo_of_trunc(const float4& v) {   // tf32_rn(v - trunc_tf32(v)), the remainder of the hardware's truncation
     float4 lo;
-    lo.x = tf32_rn_lo(__fsub_rn(v.x, __uint_as_float(__float_as_uint(v.x) & 0xffffe000u)));
-    lo.y = tf32_rn_lo(__fsub_rn(v.y, __uint_as_float(__float_as_uint(v.y) & 0xffffe000u)));
-    lo.z = tf32_rn_lo(__fsub_rn(v.z, __uint_as_float(__float_as_uint(v.z) & 0xffffe000u)));
-    lo.w = tf32_rn_lo(__fsub_rn(v.w, __uint_as_float(__float_as_uint(v.w) & 0xffffe000u)));
+    lo.x = tf32_rn(__fsub_rn(v.x, tf32_trunc(v.x)));
+    lo.y = tf32_rn(__fsub_rn(v.y, tf32_trunc(v.y)));
+    lo.z = tf32_rn(__fsub_rn(v.z, tf32_trunc(v.z)));
+    lo.w = tf32_rn(__fsub_rn(v.w, tf32_trunc(v.w)));
     return lo;
 }
 
@@ -214,167 +235,128 @@ __global__ void __launch_bounds__(TG_THREADS, 1) gemm_tf32x3_kernel(const __grid
                                                                     float* __restrict__ C, size_t ldc, uint32_t m, uint32_t n, uint32_t k, uint32_t kc_blocks) {
     extern __shared__ unsigned char tg_raw[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(tg_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + TG_BAR_OFFSET);
-    // barrier indices: full[s] = s, conv[s] = 3 + s, empty[s] = 6 + s, acc_full[a] = 9 + a, acc_empty[a] = 11 + a
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 16);
-    const uint32_t bar0 = smem_u32(bars);
+    const uint32_t sbase = smem_u32(smem);
+    const uint32_t bar0 = sbase + TG_BAR_OFFSET;   // full[s] = bar0 + 8 s, empty[s] = bar0 + 8 (TG_STAGES + s)
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t m0 = blockIdx.x * TG_M, n0 = blockIdx.y * TG_N;
     const uint32_t nkb = (k + TG_K - 1) / TG_K;
     if (threadIdx.x == 0) {
         for (int s = 0; s < TG_STAGES; ++s) {
             mbar_init(bar0 + 8 * s, 1);
-            mbar_init(bar0 + 8 * (3 + s), 128);
-            mbar_init(bar0 + 8 * (6 + s), 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(bar0 + 8 * (9 + a), 1);
-            mbar_init(bar0 + 8 * (11 + a), TG_DRAIN_THREADS);
+            mbar_init(bar0 + 8 * (TG_STAGES + s), 2);   // one arrival per consumer warpgroup
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {   // one warp allocates the tensor memory (and frees it at the end)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)TG_TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t sbase = smem_u32(smem);
 
-    if (warp == 0) {
+    if (warp == TG_CONSUMERS / 32) {
         // ===== TMA producer =====
         if (lane == 0) {
             for (uint32_t kb = 0; kb < nkb; ++kb) {
                 const uint32_t s = kb % TG_STAGES, ph = (kb / TG_STAGES) & 1u;
-                mbar_wait(bar0 + 8 * (6 + s), ph ^ 1u);
+                mbar_wait(bar0 + 8 * (TG_STAGES + s), ph ^ 1u);
                 const uint32_t full = bar0 + 8 * s;
-                mbar_expect_tx(full, 2 * TG_TILE_BYTES);
-                const uint32_t a_dst = sbase + s * TG_STAGE_BYTES, b_dst = a_dst + 2 * TG_TILE_BYTES;
+                mbar_expect_tx(full, TG_A_BYTES + TG_B_BYTES);
+                const uint32_t a_dst = sbase + s * TG_STAGE_BYTES, b_dst = a_dst + TG_A_BYTES;
                 const int32_t k0 = (int32_t)(kb * TG_K);
                 if (TA) {
                     tma_load_2d(a_dst, &mapA, full, k0, (int32_t)m0);                       // box {32 k, 128 m}: K-major rows of 128 bytes
                 } else {
 #pragma unroll
-                    for (int a = 0; a < 4; ++a)                                             // box {32 m, 32 k}: four M-atoms of 32 rows x 128 bytes
+                    for (int a = 0; a < 4; ++a)                                             // box {32 m, 32 k}: four M-blocks of 32 k-rows x 128 bytes
                         tma_load_2d(a_dst + a * 4096, &mapA, full, (int32_t)(m0 + 32 * a), k0);
                 }
-                tma_load_2d(b_dst, &mapB, full, k0, (int32_t)n0);                           // box {32 k, 128 n}
+                tma_load_2d(b_dst, &mapB, full, k0, (int32_t)n0);                           // box {32 k, 64 n}
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer: one thread, accumulators in tensor memory =====
-        if (lane == 0) {
-            // instruction descriptor: D = F32, A = B = TF32, A major (1 = MN-major, the untransposed column-major A), B K-major, N, M
-            const uint32_t idesc_base = (1u << 4) | (2u << 7) | (2u << 10) | ((TA ? 0u : 1u) << 15) | (0u << 16) | ((uint32_t)(TG_M >> 4) << 24);
-            const uint32_t idesc = idesc_base | ((uint32_t)(TG_N >> 3) << 17);            // N = 128
-            const uint32_t idesc2 = idesc_base | ((uint32_t)((2 * TG_N) >> 3) << 17);     // N = 256: B = [b_hi | b_lo], adjacent tiles of the stage
-            for (uint32_t kb = 0; kb < nkb; ++kb) {
-                const uint32_t s = kb % TG_STAGES, ph = (kb / TG_STAGES) & 1u;
-                const uint32_t chunk = kb / kc_blocks, acc = chunk & 1u, use = chunk >> 1;
-                const bool chunk_start = (kb % kc_blocks) == 0;
-                if (chunk_start) {
-                    mbar_wait(bar0 + 8 * (11 + acc), (use & 1u) ^ 1u);                      // the drain warps have emptied this accumulator
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                }
-                mbar_wait(bar0 + 8 * (3 + s), ph);                                          // converted tiles are in place
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t a_hi = sbase + s * TG_STAGE_BYTES, a_lo = a_hi + TG_TILE_BYTES, b_hi = a_hi + 2 * TG_TILE_BYTES;   // b_lo follows b_hi
-                const uint32_t d = tmem_base + acc * (2 * TG_N), ds = d + TG_N;            // main (hi*hi) and correction accumulators of this set
+        return;
+    }
+
+    // ===== two consumer warpgroups: warpgroup wg owns tile rows 64 wg .. 64 wg + 63 =====
+    const int tid = threadIdx.x, wg = warp >> 2, g = lane >> 2, t = lane & 3;
+    const uint32_t r0 = 64u * wg + 16u * (warp & 3) + g;   // the thread's tile rows: r0 and r0 + 8
+    // acc[0, 32): partial hi*hi product of the current k chunk; acc[32, 64) and acc2: the correction products a_hi*b_lo and a_lo*b_hi (kept
+    // apart so that the two wgmmas of a k-step do not write the same registers, which would serialize them).  The tensor
+    // core does not round its fp32 accumulator to nearest, and that error grows with the number of accumulating instructions: a partial only
+    // sums gemm_kc consecutive k before it is added to `sum` with round-to-nearest.
+    float acc[64], acc2[32], sum[32];
 #pragma unroll
-                for (int j = 0; j < TG_K / 8; ++j) {
-                    // A untransposed = "MN-major" (m contiguous).  For 32-bit operands the tensor core only takes MN-major tiles in the 128-byte
-                    // swizzle with 32-BYTE atoms (UMMA layout type 1; TMA SWIZZLE_128B_ATOM_32B): rows are k (128 B = 32 m each), K-atoms of 4 rows
-                    // are 512 B apart (SBO), the four 32-m M-atoms 4096 B (LBO); k-step j (8 k) starts 1024 B further.
-                    // A transposed and B = K-major, plain 128-byte swizzle (layout type 2): rows are m / n (128 B = 32 k each), 8-row atoms
-                    // 1024 B apart (SBO); k-step j starts 32 B further inside the swizzled row.
-                    const uint32_t aoff = TA ? (uint32_t)j * 32u : (uint32_t)j * 1024u;
-                    const uint32_t albo = TA ? 16u : 4096u, asbo = TA ? 1024u : 512u, alay = TA ? 2u : 1u;
-                    const uint64_t dah = umma_desc(a_hi + aoff, albo, asbo, alay), dal = umma_desc(a_lo + aoff, albo, asbo, alay);
-                    const uint64_t dbh = umma_desc(b_hi + j * 32u, 16u, 1024u);
-                    const uint32_t first = (chunk_start && j == 0) ? 0u : 1u;
-                    // a_hi x [b_hi | b_lo] as ONE N = 256 instruction: columns 0-127 of the accumulator set take the main product, columns
-                    // 128-255 the correction a_hi*b_lo (b_lo sits right behind b_hi in the stage, same 1024-byte atom stride) -- a_hi is
-                    // read from shared memory once instead of twice; then the other correction a_lo x b_hi onto columns 128-255
-                    umma_tf32(d, dah, dbh, idesc2, first);
-                    umma_tf32(ds, dal, dbh, idesc, 1u);
-                }
-                umma_commit(bar0 + 8 * (6 + s));                                            // frees the smem stage when these MMAs have read it
-                if ((kb + 1) % kc_blocks == 0 || kb + 1 == nkb) umma_commit(bar0 + 8 * (9 + acc));   // partial tile complete
+    for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) sum[i] = acc2[i] = 0.0f;
+    uint32_t chunks_done = 0;
+    for (uint32_t kb = 0; kb < nkb; ++kb) {
+        const uint32_t s = kb % TG_STAGES, ph = (kb / TG_STAGES) & 1u;
+        mbar_wait(bar0 + 8 * s, ph);
+        unsigned char* st = smem + s * TG_STAGE_BYTES;
+        // converters: B -> (tf32 hi in place, tf32 lo behind it), elementwise, so the swizzled layout is irrelevant
+        float4* bh = reinterpret_cast<float4*>(st + TG_A_BYTES);
+        float4* bl = bh + TG_B_BYTES / 16;
+#pragma unroll
+        for (int q = 0; q < TG_B_BYTES / 16 / TG_CONSUMERS; ++q) {
+            const int i = tid + q * TG_CONSUMERS;
+            float4 v = bh[i];
+            if (RAWHI) {
+                bl[i] = lo_of_trunc(v);
+            } else {
+                const float4 lo = split_tf32(v);
+                bh[i] = v;
+                bl[i] = lo;
             }
         }
-    } else if (warp < 6) {
-        // ===== converters: fp32 -> (tf32 hi, tf32 lo), elementwise, so the swizzled layout is irrelevant =====
-        const int c = threadIdx.x - 64;
-        for (uint32_t kb = 0; kb < nkb; ++kb) {
-            const uint32_t s = kb % TG_STAGES, ph = (kb / TG_STAGES) & 1u;
-            mbar_wait(bar0 + 8 * s, ph);
-            float4* a_hi = reinterpret_cast<float4*>(smem + s * TG_STAGE_BYTES);
-            float4* a_lo = a_hi + TG_TILE_BYTES / 16;
-            float4* b_hi = a_hi + 2 * (TG_TILE_BYTES / 16);
-            float4* b_lo = a_hi + 3 * (TG_TILE_BYTES / 16);
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");                       // generic-proxy stores -> visible to wgmma
+        asm volatile("bar.sync 1, %0;" ::"n"(TG_CONSUMERS) : "memory");
+        const bool chunk_start = (kb % kc_blocks) == 0;
+        const uint32_t b_hi = sbase + s * TG_STAGE_BYTES + TG_A_BYTES;
+        const float* As = reinterpret_cast<const float*>(st);
 #pragma unroll
-            for (int q = 0; q < TG_TILE_BYTES / 16 / 128; ++q) {
-                const int i = c + q * 128;
-                float4 va = a_hi[i], vb = b_hi[i];
-                if (RAWHI) {
-                    a_lo[i] = lo_of_trunc(va);
-                    b_lo[i] = lo_of_trunc(vb);
-                } else {
-                    const float4 la = split_tf32(va), lb = split_tf32(vb);
-                    a_hi[i] = va;
-                    a_lo[i] = la;
-                    b_hi[i] = vb;
-                    b_lo[i] = lb;
-                }
+        for (int i = 0; i < 64; ++i) fence_operand(acc[i]);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) fence_operand(acc2[i]);
+        wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            // A fragment of k-step j, split into hi / lo in registers
+            uint32_t ah[4], al[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const uint32_t r = r0 + 8u * (e & 1), kk = 8u * j + t + 4u * (e >> 1);
+                // TA: row r holds 32 k (128 B), 16-byte chunk kk/4 stored at chunk (kk/4) ^ (r%8).  Otherwise: four 4 KiB blocks of 32 rows;
+                // k-row kk of block r/32 holds 32 m, 16-byte chunk (r%32)/4 stored at chunk ((r%32)/4) ^ (kk%8)
+                const uint32_t off = TA ? r * 32u + ((((kk >> 2) ^ (r & 7u))) << 2) + (kk & 3u)
+                                        : (r >> 5) * 1024u + kk * 32u + (((((r & 31u) >> 2) ^ (kk & 7u))) << 2) + (r & 3u);
+                const float v = As[off];
+                const float hi = RAWHI ? tf32_trunc(v) : tf32_rn(v);
+                ah[e] = __float_as_uint(hi);
+                al[e] = __float_as_uint(tf32_rn(__fsub_rn(v, hi)));
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");                   // generic-proxy stores -> visible to the tensor core's async proxy
-            mbar_arrive(bar0 + 8 * (3 + s));
+            // a_hi x [b_hi | b_lo] as ONE N = 128 instruction (b_lo sits right behind b_hi, same 1024-byte atom stride): columns 0-63 take
+            // the main product, 64-127 the correction a_hi*b_lo; then a_lo x b_hi into acc2.  k-step j starts 32 B further inside the
+            // swizzled 128-byte rows.
+            const uint64_t dbh = gmma_desc(b_hi + 32u * j);
+            wgmma_n128(acc, ah, dbh, (chunk_start && j == 0) ? 0u : 1u);
+            wgmma_n64(acc2, al, dbh, (chunk_start && j == 0) ? 0u : 1u);
         }
-    } else {
-        // ===== drain + epilogue: warp w may touch TMEM lanes 32*(w%4) .. +31; lane == output row; two warps share a lane quarter and take
-        // 64 of the 128 accumulator columns each (keeps the running fp32 sums in registers) =====
-        const uint32_t quarter = (uint32_t)(warp & 3);
-        const uint32_t half = (uint32_t)(warp - 6) >> 2;
-        const uint32_t row = m0 + quarter * 32 + lane;
-        constexpr int NC = TG_N / 2;
-        float acc[NC];
-        const uint32_t nchunks = (nkb + kc_blocks - 1) / kc_blocks;
-        for (uint32_t ch = 0; ch < nchunks; ++ch) {
-            const uint32_t a = ch & 1u, use = ch >> 1;
-            mbar_wait(bar0 + 8 * (9 + a), use & 1u);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+        wgmma_commit_wait();
 #pragma unroll
-            for (int c4 = 0; c4 < NC / 16; ++c4) {
-                uint32_t v[16], w[16];
-                const uint32_t taddr = tmem_base + a * (2 * TG_N) + half * NC + c4 * 16 + ((quarter * 32u) << 16);
-                tmem_ld16(taddr, v);                  // main partial (hi*hi)
-                tmem_ld16(taddr + TG_N, w);           // correction partial (lo*hi + hi*lo)
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        for (int i = 0; i < 64; ++i) fence_operand(acc[i]);
 #pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    const float p = __fadd_rn(__uint_as_float(v[i]), __uint_as_float(w[i]));
-                    acc[c4 * 16 + i] = ch == 0 ? p : __fadd_rn(acc[c4 * 16 + i], p);
-                }
+        for (int i = 0; i < 32; ++i) fence_operand(acc2[i]);
+        if ((warp & 3) == 0 && lane == 0) mbar_arrive(bar0 + 8 * (TG_STAGES + s));            // this warpgroup is done with the stage
+        if ((kb + 1) % kc_blocks == 0 || kb + 1 == nkb) {                                      // partial tile complete
+#pragma unroll
+            for (int i = 0; i < 32; ++i) {
+                const float p = __fadd_rn(acc[i], __fadd_rn(acc[32 + i], acc2[i]));
+                sum[i] = chunks_done == 0 ? p : __fadd_rn(sum[i], p);
             }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            mbar_arrive(bar0 + 8 * (11 + a));
-        }
-        if (row < m) {
-            float* crow = C + row;
-#pragma unroll
-            for (int j = 0; j < NC; ++j) {
-                const uint32_t col = n0 + half * NC + j;
-                if (col < n) crow[(size_t)col * ldc] = nkb ? acc[j] : 0.0f;
-            }
+            ++chunks_done;
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)TG_TMEM_COLS) : "memory");
+    // epilogue: accumulator element i of the thread is row r0 + 8 ((i / 2) % 2), column 8 (i / 4) + 2 t + i % 2
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+        const uint32_t row = m0 + r0 + 8u * ((i >> 1) & 1), col = n0 + 8u * (i >> 2) + 2u * t + (i & 1);
+        if (row < m && col < n) C[row + (size_t)col * ldc] = sum[i];
     }
 }
 
@@ -395,15 +377,14 @@ EncodeTiledFn encode_tiled() {
 }
 
 // 2-D fp32 tensor map over a column-major matrix: dim 0 = the contiguous direction (extent d0), dim 1 = columns (extent d1, ld elements apart)
-int32_t make_map(dab_ctx* ctx, CUtensorMap* map, const float* base, size_t d0, size_t d1, size_t ld, uint32_t box0, uint32_t box1,
-                 CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B) {
+int32_t make_map(dab_ctx* ctx, CUtensorMap* map, const float* base, size_t d0, size_t d1, size_t ld, uint32_t box0, uint32_t box1) {
     EncodeTiledFn enc = encode_tiled();
     if (!enc) return dab_fail(ctx, DAB_ERR_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
     cuuint64_t dims[2] = {(cuuint64_t)d0, (cuuint64_t)d1};
     cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
     cuuint32_t box[2] = {box0, box1};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
+    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return dab_fail(ctx, DAB_ERR_CUDA, "cuTensorMapEncodeTiled failed with %d (dims %zu x %zu, ld %zu)", (int)r, d0, d1, ld);
     return DAB_OK;
@@ -413,11 +394,11 @@ bool tma_ok(const void* p, size_t ld) { return (reinterpret_cast<uintptr_t>(p) &
 
 int32_t launch_tf32x3(dab_ctx* ctx, int transA, size_t m, size_t n, size_t k, const float* A, size_t lda, const float* B, size_t ldb, float* C, size_t ldc) {
     CUtensorMap mapA, mapB;
-    // untransposed column-major A is "MN-major" for the tensor core; for 32-bit (tf32) operands that needs the 128-byte swizzle with
-    // 32-BYTE atoms (TMA SWIZZLE_128B_ATOM_32B, UMMA layout type 1) -- the 16-byte-atom swizzle is only defined for K-major tf32
-    int32_t st = transA ? make_map(ctx, &mapA, A, k, m, lda, 32, 128) : make_map(ctx, &mapA, A, m, k, lda, 32, 32, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B);
+    // transposed A and B are K-major tiles (rows of 32 k); an untransposed A arrives as four blocks of 32 k-rows x 32 m, which the consumer
+    // threads read back into wgmma's register fragments
+    int32_t st = transA ? make_map(ctx, &mapA, A, k, m, lda, 32, 128) : make_map(ctx, &mapA, A, m, k, lda, 32, 32);
     if (st != DAB_OK) return st;
-    st = make_map(ctx, &mapB, B, k, n, ldb, 32, 128);
+    st = make_map(ctx, &mapB, B, k, n, ldb, 32, TG_N);
     if (st != DAB_OK) return st;
     const size_t gx = (m + TG_M - 1) / TG_M, gy = (n + TG_N - 1) / TG_N;
     if (gx > 0x7fffffffull || gy > 65535ull) return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_gemm: tile grid %zu x %zu too large", gx, gy);

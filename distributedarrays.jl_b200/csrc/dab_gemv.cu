@@ -522,9 +522,9 @@ int32_t launch_n_cfg(dab_ctx* ctx, const T* A, size_t m, size_t n, const T* x, T
     return DAB_OK;
 }
 
-// loads in flight per thread: U = 4 columns x R = 1 row group.  Measured on B200 for the unit-wise variant (leading dimension not a multiple
-// of 16 bytes): (U, R) = (4, 1) gives a steady 4.1-4.2 TB/s; more loads in flight -- (8, 1), (16, 1), (4, 2), (2, 4), (4, 4) -- range
-// from 2.2 to 5.6 TB/s depending on the column stride, so the steady shape is kept (profiles/r2_gemv_unaligned_sweep.txt).
+// loads in flight per thread: U = 4 columns x R = 1 row group.  For the unit-wise variant (leading dimension not a multiple of 16 bytes)
+// (U, R) = (4, 1) gave a steady rate in the design sweep; more loads in flight -- (8, 1), (16, 1), (4, 2), (2, 4), (4, 4) -- swung
+// widely with the column stride, so the steady shape is kept.
 template <typename T, int VEC>
 int32_t launch_n(dab_ctx* ctx, const T* A, size_t m, size_t n, const T* x, T* y) {
     return launch_n_cfg<T, VEC, 4, 1>(ctx, A, m, n, x, y);
@@ -542,7 +542,7 @@ int32_t launch_n_phase(dab_ctx* ctx, const T* A, size_t m, size_t n, const T* x,
     const size_t gx = (rvecs + RT - 1) / RT;
     const size_t slots = (size_t)ctx->sm_count * (size_t)dab_resident_ctas((const void*)gemv_n_phase_kernel<T, VEC, U>, GV_THREADS);
     // four waves of CTAs rather than one: the CTAs holding a masked warp run a little longer and a single wave would wait for them
-    // (measured: tools/sweep_gemv.cu, profiles/r2_sweep_gemv.txt); the partial vectors stay below 1/32 of the matrix bytes
+    // (tools/sweep_gemv.cu sweeps it); the partial vectors stay below 1/32 of the matrix bytes
     size_t want = 4 * slots / (gx * VEC);
     if (want > n / (32 * VEC * (sizeof(Acc) / sizeof(T)))) want = n / (32 * VEC * (sizeof(Acc) / sizeof(T)));
     if (want < 1) want = 1;
@@ -674,8 +674,8 @@ int32_t gemv_t(dab_ctx* ctx, int32_t trans, const T* A, size_t m, size_t n, cons
     const bool vec = ((uintptr_t)A % 16 == 0) && (m % VEC == 0) && (!trans || (uintptr_t)x % 16 == 0);
     if (!trans) {
         // The phase-class kernel is the default for every chunk big enough to matter: 16-byte loads whatever the alignment of the
-        // columns, and four waves of CTAs (6.7-6.8 TB/s on B200 against 6.4 for the single-wave kernel on aligned chunks and 4.2 for
-        // unit-wise loads on misaligned ones; profiles/r2_gemv_phase.txt).  dab_set_option("gemv_phase", 0) restores the round-1 pair.
+        // columns, and four waves of CTAs (faster than the single-wave kernel on aligned chunks and than unit-wise loads on misaligned
+        // ones when it was designed).  dab_set_option("gemv_phase", 0) restores the round-1 pair.
         // Where it pays: the VEC class partials cost 2*VEC*m carriers of traffic (16/n of the Float32 matrix bytes) and a short column
         // leaves row lanes idle -- an aligned chunk switches kernels only when that is below 2 % (measured 4194304 x 128: 5.8 vs 6.4
         // TB/s, 128 x 4194304: 3.0 vs 5.4), a misaligned one as soon as it beats the unit-wise loads' -35 %.
@@ -684,8 +684,8 @@ int32_t gemv_t(dab_ctx* ctx, int32_t trans, const T* A, size_t m, size_t n, cons
         if (vec) return launch_n<T, VEC>(ctx, A, m, n, x, y);
         return launch_n<T, 1>(ctx, A, m, n, x, y);
     }
-    // columns a thread carries (x is loaded once per COLS column elements): 8 with 16-byte loads (Float32 32768 x 16384: 6.47 TB/s
-    // against 5.91 with 4; profiles/r2_gemv_phase.txt), dab_set_option("gemv_t_cols", 4) for the A/B measurement
+    // columns a thread carries (x is loaded once per COLS column elements): 8 with 16-byte loads (faster than 4 on a large Float32
+    // chunk when it was designed), dab_set_option("gemv_t_cols", 4) for the A/B measurement
     if (ctx->opt_gemv_t_cols == 8 && vec && n >= 64) return launch_t<T, VEC, 8>(ctx, A, m, n, x, y);
     // misaligned columns: the phase-class kernel keeps the 16-byte loads (gemv_phase = 0: unit-wise loads, the round-1 kernel)
     if (!vec && ctx->opt_gemv_phase && (uintptr_t)A % sizeof(T) == 0 && (uintptr_t)x % sizeof(T) == 0 && m >= 256 && n >= 64)

@@ -4,7 +4,7 @@
 // copy(lbc) (:96): the whole tree  f.(args...)  is fused into a single pass over the chunk -- N-ary, nested, with size-1
 // ("extruded", src/broadcast.jl:112-113) dims and mixed element types.  The host runtime (distributedarrays.jl_b200/
 // _broadcast.py) traces the user's function into C source for ONE element (Julia promotion already applied); this file
-// wraps it into two sm_100a kernels with NVRTC (-fmad=false: no FMA contraction, Julia semantics):
+// wraps it into two sm_90a kernels with NVRTC (-fmad=false: no FMA contraction, Julia semantics):
 //   dab_bc_linear  : every array argument is dense and has the destination's shape -> 4 consecutive elements per thread,
 //                    16/32-byte vector loads and stores, grid-stride (HBM roofline: sum of element sizes per element);
 //   dab_bc_general : per-argument strides (0 = extruded dim), coalesced along dim 0.
@@ -304,8 +304,8 @@ std::string build_source(const char* expr, int32_t out_dt, int nargs, const int3
     s += "#define DAB_EXPR (";
     s += expr;
     s += ")\n";
-    // ---- linear kernel: flat grid, one CTA per 2 x 256 vectors of 4 elements (same shape as ew1_kernel: measured 6.9 vs 6.6 TB/s
-    // for the persistent grid-stride form); the extra last CTA takes the remainder vectors and the scalar tail
+    // ---- linear kernel: flat grid, one CTA per 2 x 256 vectors of 4 elements (same shape as ew1_kernel, which beat
+    // the persistent grid-stride form); the extra last CTA takes the remainder vectors and the scalar tail
     s += "extern \"C\" __global__ void __launch_bounds__(256) dab_bc_linear(BcParams p) {\n"
          "  const u64 n = p.shape[0] * p.shape[1] * p.shape[2] * p.shape[3];\n"
          "  const u64 nv = n / 4;\n"
@@ -435,7 +435,7 @@ int32_t compile_cubin(dab_ctx* ctx, const std::string& src, std::vector<char>* c
     nvrtcProgram prog;
     nvrtcResult r = rt.CreateProgram(&prog, src.c_str(), "dab_broadcast.cu", 0, nullptr, nullptr);
     if (r != NVRTC_SUCCESS) return dab_fail(ctx, DAB_ERR_NVRTC, "nvrtcCreateProgram: %s", rt.GetErrorString(r));
-    const char* opts[] = {"--gpu-architecture=sm_100a", "-fmad=false", "--std=c++17", "-lineinfo", "-default-device", "--device-int128"};
+    const char* opts[] = {"--gpu-architecture=sm_90a", "-fmad=false", "--std=c++17", "-lineinfo", "-default-device", "--device-int128"};
     r = rt.CompileProgram(prog, int128 ? 6 : 5, opts);
     if (r != NVRTC_SUCCESS) {
         size_t ls = 0;
@@ -692,7 +692,7 @@ std::unordered_map<std::string, CompiledMr> g_mr_cache;
 extern "C" {
 
 // Diagnostic (no GPU needed): run the same source generation + NVRTC compilation as dab_broadcast_expr and report the size
-// of the sm_100a cubin.  Lets the host-side tests validate the tracer's code generation on a CPU-only machine.
+// of the sm_90a cubin.  Lets the host-side tests validate the tracer's code generation on a CPU-only machine.
 int32_t dab_jit_compile_check(const char* expr, int32_t out_dtype, int32_t nargs, const int32_t* arg_dtypes,
                               const int32_t* arg_is_array, size_t* cubin_bytes) {
     if (!expr || !ctype_of(out_dtype) || nargs < 0 || nargs > 8 || (nargs && (!arg_dtypes || !arg_is_array)))

@@ -1,4 +1,4 @@
-// dab_reduce.cu -- K4 / K7: whole-chunk mapreduce(f, op, localpart(d)) as one streaming sm_100a kernel.
+// dab_reduce.cu -- K4 / K7: whole-chunk mapreduce(f, op, localpart(d)) as one streaming sm_90a kernel.
 //
 // Replaces the per-worker Base.mapreduce / reduce / all / any / count at reference src/mapreduce.jl:23,31,100,109,118
 // and the caller-side left fold reduce(op, results) at src/mapreduce.jl:26,34 (dab_combine_ordered).
@@ -39,8 +39,8 @@ __global__ void __launch_bounds__(RD_THREADS, 8) reduce_kernel(const T* __restri
     const size_t ntiles = nvec / TILE;
     A acc = R::identity();
     // "flat" grid: CTA b owns the tiles_per_cta consecutive tiles starting at b*tiles_per_cta (fixed mapping -> deterministic
-    // result); the block scheduler issues CTAs in address order, keeping the open DRAM pages a compact window.  Measured on
-    // B200 (profiles/sweep_r1.txt): 7.55 TB/s vs 7.2 TB/s for a persistent grid-stride loop.
+    // result); the block scheduler issues CTAs in address order, keeping the open DRAM pages a compact window (faster than a
+    // persistent grid-stride loop when the kernel was designed).
     size_t t_end = ((size_t)blockIdx.x + 1) * (size_t)tiles_per_cta;
     if (t_end > ntiles) t_end = ntiles;
 #pragma unroll 1

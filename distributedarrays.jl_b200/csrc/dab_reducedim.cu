@@ -1,4 +1,4 @@
-// dab_reducedim.cu -- K5 / K6: mapreduce(f, op, localpart(A), dims=region) as streaming sm_100a kernels.
+// dab_reducedim.cu -- K5 / K6: mapreduce(f, op, localpart(A), dims=region) as streaming sm_90a kernels.
 //
 // Replaces the per-worker Base.mapreducedim! at reference src/mapreduce.jl:64 (phase 1, mapreducedim_within) and :77
 // (phase 2, accumulation of the gathered partials onto localpart(R) in mapreducedim_between!).
@@ -8,7 +8,7 @@
 //   * inner == 1  ("leading dims", e.g. sum(A, dims=1)): every output is a CONTIGUOUS run of `reduce` elements.
 //       - long runs : one CTA per (run, split); 16-byte evict-first loads, 4 in flight per thread, per-run head/tail peel
 //         (run starts are not 16-byte aligned when reduce % (16/sizeof T) != 0); runs are split across CTAs when there are too
-//         few of them to fill 148 SMs, and a tiny second kernel folds the splits in order (deterministic, no atomics).
+//         few of them to fill the SMs, and a tiny second kernel folds the splits in order (deterministic, no atomics).
 //       - short / medium runs: a sub-warp group of G lanes per run (G = #16-byte vectors in the run, <= 32), so a warp streams
 //         32/G consecutive runs with 512 contiguous bytes per load instruction; flat grid.
 //   * inner  > 1  (reduce over a non-leading dim): threads map along i (coalesced), each walks r with 8 independent loads in

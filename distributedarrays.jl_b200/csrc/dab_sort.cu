@@ -4,7 +4,7 @@
 // Keys only, ascending in Julia's `isless` order: integers by value; floats with -0.0 < +0.0 and every NaN after +Inf (bit
 // patterns preserved; the reference keeps NaNs in their original relative order, here they are ordered by payload).
 //
-// Algorithm: least-significant-digit radix sort, 8-bit digits, hand-written for sm_100a, "onesweep" structure.  HBM-bound integer work:
+// Algorithm: least-significant-digit radix sort, 8-bit digits, hand-written for sm_90a, "onesweep" structure.  HBM-bound integer work:
 //   sort_hist_kernel      one read of the keys -> the 256-bin histogram of EVERY digit position
 //   sort_plan_kernel      (1 CTA) bucket bases per digit, which passes run (a digit that is constant over the chunk is skipped: Int64 data
 //                         in a small range needs 2-3 of 8 passes), buffer ping-pong -- on the DEVICE: dab_sort never synchronises the stream
@@ -26,7 +26,7 @@ constexpr int ST_THREADS = 256;
 constexpr int ST_KPT = 8;                        // keys per thread (16 left the scatter at 111 registers = 2 CTAs per SM, latency-bound)
 constexpr int ST_TILE = ST_THREADS * ST_KPT;     // 2048 keys per CTA
 
-// Lanes of the warp whose 8-bit digit equals mine (dg = 256 marks "no key"; those lanes group together): 9 ballots.  On sm_100a
+// Lanes of the warp whose 8-bit digit equals mine (dg = 256 marks "no key"; those lanes group together): 9 ballots.  On sm_90a
 // __match_any_sync costs one round per DISTINCT value in the warp (measured ~45 clk per warp-step on random digits); the bitwise
 // form is flat.
 template <int B>
@@ -577,7 +577,7 @@ int32_t sort_t(dab_ctx* ctx, const void* in_v, void* out_v, void* tmp_v, size_t 
     DAB_REQUIRE(ctx, tmp != nullptr && tmp != out && tmp != in, DAB_ERR_ARG, "dab_sort: tmp must be a distinct buffer of n elements");
     DAB_REQUIRE(ctx, n < 0xFFFFF000ull, DAB_ERR_UNSUPPORTED, "dab_sort: chunks of 2^32 or more elements are not served");
     // tile shape: 32 KiB of keys per CTA in shared memory -> ~128-byte bucket runs per tile on random digits
-    // tile shape (measured on B200, profiles/r2_sort_vs_cub.txt: larger tiles and 3 resident CTAs per SM win over smaller tiles at 4 CTAs
+    // tile shape (tools/sort_vs_cub.cu sweeps it: larger tiles and 3 resident CTAs per SM won over smaller tiles at 4 CTAs
     // and over 128-register CTAs at 2): 256 threads x 16 keys (64-bit) / x 32 keys (32-bit) = 32 KiB of keys per tile, twice in shared memory
     if constexpr (sizeof(U) == 8) return sort_passes<T, 256, 16, 3>(ctx, in, out, tmp, n);
     else return sort_passes<T, 256, 32, 3>(ctx, in, out, tmp, n);

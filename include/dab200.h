@@ -1,5 +1,5 @@
 /*
- * dab200.h -- C ABI of libdab200.so: the B200 (sm_100a) backend for the DArray
+ * dab200.h -- C ABI of libdab200.so: the H100 (sm_90a) backend for the DArray
  *             map!/broadcast + mapreduce hot path of DistributedArrays.jl.
  *
  * The reference (DistributedArrays.jl v0.6.9) is pure Julia and has NO FFI / plugin
@@ -170,7 +170,7 @@ int32_t dab_binary(dab_ctx* ctx, int32_t dtype, int32_t op, void* z, const void*
 int32_t dab_binary_scalar(dab_ctx* ctx, int32_t dtype, int32_t op, void* z, const void* x, const void* s,
                           int32_t scalar_left, size_t n);
 /* General fused broadcast  dest .= f.(args...)  for an arbitrary expression tree, compiled at run
- * time with NVRTC for sm_100a (what Julia's JIT does for a Broadcasted, src/broadcast.jl:65-85).
+ * time with NVRTC for sm_90a (what Julia's JIT does for a Broadcasted, src/broadcast.jl:65-85).
  * `expr` is C source for ONE element in terms of a0..a{nargs-1} (already converted to their
  * dtypes) and must yield a value of out_dtype, e.g. "a0 - a1 * sinf(a2)".  Each arg k is either
  * a device array (arg_ptrs[k] != NULL) indexed through arg_strides[k*4 .. k*4+3] (0 for an extruded
@@ -182,7 +182,7 @@ int32_t dab_broadcast_expr(dab_ctx* ctx, const char* expr, int32_t out_dtype, vo
                            const void* const* arg_ptrs, const size_t* arg_strides, const uint64_t* arg_scalars);
 
 /* Diagnostic, needs no GPU: generate + NVRTC-compile the kernels dab_broadcast_expr would use for this expression and
- * report the sm_100a cubin size (arg_is_array[k] != 0: array argument, else by-value scalar). */
+ * report the sm_90a cubin size (arg_is_array[k] != 0: array argument, else by-value scalar). */
 int32_t dab_jit_compile_check(const char* expr, int32_t out_dtype, int32_t nargs, const int32_t* arg_dtypes,
                               const int32_t* arg_is_array, size_t* cubin_bytes);
 
@@ -257,7 +257,7 @@ int32_t dab_gemv(dab_ctx* ctx, int32_t dtype, int32_t trans, const void* A, size
  * R[m x n] (ldc) = op(A) * B on column-major operands of ONE worker: transA = 0 -> A is m x k (lda); transA = 1 -> op(A) = A^T with A
  * stored k x m (lda); B is k x n (ldb).  Replaces  localpart(A) * convert(localtype(B), Bjk)  and the transpose / adjoint forms of
  * _matmatmul! (src/linalg.jl:218-226); the caller scales C by beta and adds alpha * R per tile exactly as the reference (:232-252).
- * Float32 with 16-byte aligned bases and leading dimensions: TMA-fed tcgen05 (3xTF32 error-compensated, TMEM accumulators drained
+ * Float32 with 16-byte aligned bases and leading dimensions: TMA-fed wgmma (3xTF32 error-compensated, register partials drained
  * every "gemm_kc" k for fp32 round-to-nearest accumulation); otherwise and for Float64 / Int32 / Int64: shared-memory tiled FMA kernel
  * (integers wrap like Julia's).  n == 1 with a dense A (lda == its row count) IS a matrix-vector product and is served by K9
  * (dab_gemv: one read of A at the HBM roofline).  R is overwritten. */

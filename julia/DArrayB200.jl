@@ -284,7 +284,7 @@ end
 # keyword arguments do not take part in dispatch: ONE method serves both spellings
 Base.sort(a::B200Array{T,1}; by = identity, kw...) where {T} = by === identity ? sort_keys(a) : sort_by(a, by.(a))
 
-# localpart(A) * Bjk, transpose(localpart(A)) * Bjk inside _matmatmul!  (src/linalg.jl:218-226): K12, tcgen05 3xTF32 for Float32
+# localpart(A) * Bjk, transpose(localpart(A)) * Bjk inside _matmatmul!  (src/linalg.jl:218-226): K12, wgmma 3xTF32 for Float32
 function gemm(transA::Bool, A::B200Array{T,2}, B::B200Array{T,2}) where {T}
     m, k = transA ? reverse(size(A)) : size(A)
     size(B, 1) == k || throw(DimensionMismatch("matrix A has dimensions ($m, $k), matrix B has dimensions $(size(B))"))

@@ -165,7 +165,7 @@ class HostMemABI:
         return 0
 
     def dab_device_info(self, ctx, sm, cc, free_b, total_b):
-        sm._obj.value, cc._obj.value, free_b._obj.value, total_b._obj.value = 148, 100, 1 << 30, 1 << 30
+        sm._obj.value, cc._obj.value, free_b._obj.value, total_b._obj.value = 132, 90, 1 << 30, 1 << 30
         return 0
 
     def dab_stream(self, ctx, out):

@@ -165,8 +165,8 @@ def test_classify_map_for_reductions():
     assert classify_map(lambda x: 2 * x, np.int64)[0] is None                 # general f -> fused map kernel + identity reduce
 
 
-def test_nvrtc_codegen_compiles_for_sm100a(dab):
-    """The exact source dab_broadcast_expr would JIT, compiled with NVRTC for sm_100a on this CPU-only box."""
+def test_nvrtc_codegen_compiles_for_sm90a(dab):
+    """The exact source dab_broadcast_expr would JIT, compiled with NVRTC for sm_90a on a CPU-only machine."""
     from darray_b200 import _lib, abs2, ifelse, jl_max, mod, sin, sqrt
     from darray_b200._broadcast import codegen, convert, trace
 
@@ -343,7 +343,7 @@ def test_last_session_gpu_tests_dry_run_on_the_host_memory_abi(hostmem, dab):
     """The GPU tests of tests/test_gpu_zz_last_session.py that the host-memory ABI emulation can carry (all but the dab_gemm dispatch) are
     executed here, on CPU, exactly as written (same functions, a runtime on the emulation in place of the rt fixtures): the host runtime
     above the ABI -- tracer, run_local's routing and stride tables, collapse_dims, layouts, halo plans, the sort / Int128 / copy / norm
-    flows -- runs for real, only the kernels are NumPy.  Whatever fails on the B200 later is then in a kernel or a binding, not in a typo,
+    flows -- runs for real, only the kernels are NumPy.  Whatever fails on the GPU later is then in a kernel or a binding, not in a typo,
     a shape or a wrong NumPy twin of the TEST, nor in the host logic."""
     import test_gpu_zz_last_session as z
     rt = dab.init(workers_per_rank=8, use_dist=False)
@@ -409,7 +409,7 @@ def test_bench_host_logic_against_the_host_memory_abi():
 
 
 def test_smoke_host_logic_against_the_host_memory_abi():
-    """``__graft_entry__.smoke()`` (what the driver runs on the B200 before the bench) with the C ABI emulated over host memory: its host side
+    """``__graft_entry__.smoke()`` (the end-to-end check run on the GPU before the bench) with the C ABI emulated over host memory: its host side
     -- layouts vs the oracle, map!, broadcast, sum / maximum, sum(dims=1), the halo read, A*B, the strided view, sort -- runs through."""
     import subprocess
     r = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "run_on_hostmem.py"), "__graft_entry__.py", "smoke"], cwd=ROOT,

@@ -1,4 +1,4 @@
-"""CPU-only: the source generated for the fused map+reduce kernels (dab_mapreduce_expr) compiles with NVRTC for sm_100a for every
+"""CPU-only: the source generated for the fused map+reduce kernels (dab_mapreduce_expr) compiles with NVRTC for sm_90a for every
 (op, value type) combination the host runtime can request, and unsupported combinations are refused, not silently served."""
 import ctypes as C
 
@@ -121,7 +121,7 @@ _EXT_NAMES = ["acos", "acosh", "acot", "acoth", "acsc", "acsch", "asec", "asech"
 
 
 def test_extended_unary_functions_trace_and_compile():
-    """Every added unary function traces with Julia's result type and its broadcast kernel compiles for sm_100a (Float64 argument here; the
+    """Every added unary function traces with Julia's result type and its broadcast kernel compiles for sm_90a (Float64 argument here; the
     Float32 / Int64 variants were compiled once when the functions were added).  Functions Julia defines by composition are composed the
     same way (sec = inv(cos), asec = acos(inv), deg2rad = x * (pi / 180) in the argument's type)."""
     import darray_b200 as dab
@@ -152,7 +152,7 @@ def test_extended_unary_functions_trace_and_compile():
 
 def test_shift_operators_trace_and_compile():
     """``a .<< 2``, ``2 .<< a``, ``a .<< a`` and ``>>`` (test/darray.jl:863-867): the result has the type of the LEFT operand, the count is
-    an Int64, floats are a MethodError; the kernels compile for sm_100a; the emulator's model follows Julia (negative counts, counts past
+    an Int64, floats are a MethodError; the kernels compile for sm_90a; the emulator's model follows Julia (negative counts, counts past
     the width)."""
     import darray_b200 as dab  # noqa: F401
     import hostmem_abi as hm

@@ -1,6 +1,6 @@
 """GPU parity tests for K12 (dab_gemm): the tile product of the matrix-matrix mul! (reference src/linalg.jl:189-257).
 
-Float32 goes through the tcgen05 3xTF32 kernel (TMA operands, TMEM accumulators) when bases / leading dimensions are 16-byte aligned and
+Float32 goes through the wgmma 3xTF32 kernel (TMA operands, register accumulators) when bases / leading dimensions are 16-byte aligned and
 through the SIMT tile kernel otherwise; Float64 / Int32 / Int64 through the SIMT kernel.  Integers are exact (wrap-around like Julia);
 floats are compared with an fp64 product: |R - R64| <= tol * (|A| @ |B|) elementwise (the forward-error form of every GEMM bound),
 tol = 2e-6 for Float32 (BLAS sgemm itself only guarantees k * eps), 1e-14 * k for Float64."""
@@ -78,7 +78,7 @@ def test_gemm_f32(dab, rt1, m, n, k, transA):
 
 def test_gemm_f32_relative_1e6_on_positive_data(dab, rt1):
     """Uniform [0,1) data (the bench's distribution): every entry of the tensor-core product within 1e-6 RELATIVE of the fp64 product,
-    for a long contraction, thanks to the two-level accumulation (TMEM partials of gemm_kc k, fp32 round-to-nearest between them)."""
+    for a long contraction, thanks to the two-level accumulation (register partials of gemm_kc k, fp32 round-to-nearest between them)."""
     rng = np.random.default_rng(5)
     m, n, k = 256, 256, 8192
     A, B = rng.random((m, k)).astype(F32), rng.random((k, n)).astype(F32)

@@ -208,7 +208,7 @@ def test_matvec_errors_and_reference_dot_test(dab, rt8):
 def test_matmatmul(dab, rt8, dtype, grid):
     """``A*B``, ``A'*B``, ``transpose(A)*B`` and ``mul!(C, A, B, alpha, beta)`` (reference src/linalg.jl:189-311; reference tests
     test/darray.jl:915-931, 996-1012): layout of the result (owners, grid, cuts) equals the oracle's, integer results exactly, float
-    results within the forward-error bound of the tile products (K12: tcgen05 3xTF32 for aligned Float32 tiles, SIMT otherwise)."""
+    results within the forward-error bound of the tile products (K12: wgmma 3xTF32 for aligned Float32 tiles, SIMT otherwise)."""
     rng = np.random.default_rng(47)
     m, kdim, n = 96, 130, 72                               # 130 / 8 -> 17,17,16,... column blocks: unaligned leading dimensions too
     mk = (lambda *s: rng.integers(-9, 9, s).astype(dtype)) if np.dtype(dtype).kind != "f" else (lambda *s: rng.standard_normal(s).astype(dtype))
@@ -268,7 +268,7 @@ def test_matmatmul_reference_tests_and_errors(dab, rt8):
 
 
 def test_matmatmul_float32_tensor_core_tiles(dab, rt2):
-    """Chunks big and aligned enough for the tcgen05 path (2 workers -> 512 x 256 column blocks): 1e-6 relative on positive data."""
+    """Chunks big and aligned enough for the wgmma path (2 workers -> 512 x 256 column blocks): 1e-6 relative on positive data."""
     rng = np.random.default_rng(59)
     A, B = rng.random((512, 512)).astype(np.float32), rng.random((512, 384)).astype(np.float32)
     DA, DB = dab.distribute(A), dab.distribute(B)

@@ -16,8 +16,8 @@
 STATUS: these tests have NOT been executed on hardware yet.  What is verified on CPU: the sort-by-key composition (key|position words,
 two rounds for 64-bit keys, gather) step by step in ``tests/hostmem_abi.py`` against a stable ``isless`` argsort, the whole host flow
 of ``_sort.py`` against the oracle (``tests/test_cpu_sort.py``), and that the collapsed box of ``collapse_dims`` addresses exactly the
-elements NumPy's broadcasting reads (``tests/test_cpu_host.py``), that the Int128 reduce kernels compile with NVRTC for sm_100a and
-that the host side (slot decoding, wrap-around fold) is exact (``tests/test_cpu_jit_reduce.py``).  What only a B200 can verify: the two small sort-by-key kernels,
+elements NumPy's broadcasting reads (``tests/test_cpu_host.py``), that the Int128 reduce kernels compile with NVRTC for sm_90a and
+that the host side (slot decoding, wrap-around fold) is exact (``tests/test_cpu_jit_reduce.py``).  What only a GPU can verify: the two small sort-by-key kernels,
 their ctypes bindings, and the N-d broadcast through the real NVRTC kernel.  The module therefore runs LAST (file name) and is marked
 ``xfail(strict=False)``: a pass is reported as XPASS, a failure cannot hide a regression elsewhere or turn the tier red for code that
 was never claimed as measured.  Order inside the module: host-side compositions of GPU-tested kernels first, new NVRTC device code

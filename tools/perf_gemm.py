@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""K12 timing: dab_gemm (tcgen05 3xTF32) on square and chunk-shaped Float32 problems, the SIMT kernel beside it; error vs fp64 on a slice."""
+"""K12 timing: dab_gemm (wgmma 3xTF32) on square and chunk-shaped Float32 problems, the SIMT kernel beside it; error vs fp64 on a slice."""
 import ctypes as C
 import json
 import os
@@ -55,7 +55,7 @@ def main():
                 _lib.call("dab_d2h", rt.ctx, C.c_void_p(host.ctypes.data), C.c_void_p(Cc.ptr + 4 * j * m), 4 * rows)
                 rt.sync()
                 worst = max(worst, float(np.abs(host - want[:, j]).max() / np.abs(want[:, j]).min()))
-            print(json.dumps({"kernel": {0: "tcgen05_3xtf32", 1: "simt", 2: "tcgen05_3xtf32_rawhi"}[simt], "m": m, "n": n, "k": k, "ms": round(ms, 4), "useful_TFLOPs": round(tf, 1),
+            print(json.dumps({"kernel": {0: "wgmma_3xtf32", 1: "simt", 2: "wgmma_3xtf32_rawhi"}[simt], "m": m, "n": n, "k": k, "ms": round(ms, 4), "useful_TFLOPs": round(tf, 1),
                               "tf32_mma_TFLOPs": round(3 * tf, 1) if simt != 1 else None, "frac_of_bf16_peak_div2_div3": round(tf / (peak / 2 / 3), 3) if simt != 1 else None,
                               "max_rel_err_vs_fp64": worst}), flush=True)
         rt.set_option("gemm_simt", 0)

@@ -1,6 +1,6 @@
 // tools/sort_vs_cub.cu -- K11 (dab_sort, through the C ABI of libdab200.so) against cub::DeviceRadixSort::SortKeys, the library
 // yardstick.  Self-checking: every dab_sort result is compared element by element with CUB's on the device.  Not part of the product.
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -I include -o tools/sort_vs_cub tools/sort_vs_cub.cu \
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -I include -o tools/sort_vs_cub tools/sort_vs_cub.cu \
 //        -L distributedarrays.jl_b200/csrc -ldab200 -Xlinker -rpath -Xlinker '$ORIGIN/../distributedarrays.jl_b200/csrc'
 //   tools/sort_vs_cub [log2n_64bit=27] [log2n_32bit=28] [reps=5] [variants=3] [test mask=0xff]
 #include <cuda_runtime.h>

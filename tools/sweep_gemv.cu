@@ -3,7 +3,7 @@
 //   * gemv_n_kernel<float,4,4,1> (aligned, consecutive columns) on m = 2^15, 32800 (multiple of 128 B), 32772 (multiple of 16 B only)
 //   * gemv_n_phase_kernel<float,4,4> (4 phase classes, column stride 4) on the same aligned m's and on odd / even misaligned m's
 // each over the number of column splits (CTAs in flight) and the CTAs resident per SM (limited through dynamic shared memory).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -fmad=false --expt-relaxed-constexpr -o tools/sweep_gemv \
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -fmad=false --expt-relaxed-constexpr -o tools/sweep_gemv \
 //        tools/sweep_gemv.cu -Ldistributedarrays.jl_b200/csrc -ldab200 -Xlinker -rpath='$ORIGIN/../distributedarrays.jl_b200/csrc'
 #include "../distributedarrays.jl_b200/csrc/dab_gemv.cu"
 

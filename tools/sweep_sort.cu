@@ -8,7 +8,7 @@
 //   V1  keys staged global->shared with cp.async (all copies in flight by construction), ranking / scatter read shared memory
 //   V2  V1 + the tile is reordered by digit in shared memory, then written in runs (consecutive threads -> consecutive addresses)
 // each at KPT = 8 and 16 keys per thread, for 64-bit and 32-bit keys.
-// Build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -lineinfo -o sweep_sort sweep_sort.cu ; run: ./sweep_sort [log2n]
+// Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -o sweep_sort sweep_sort.cu ; run: ./sweep_sort [log2n]
 #include <cuda_pipeline.h>
 #include <cuda_runtime.h>
 

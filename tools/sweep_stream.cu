@@ -1,9 +1,9 @@
-// tools/sweep_stream.cu -- design-space sweep for the two streaming kernels of the hot path on a real B200:
+// tools/sweep_stream.cu -- design-space sweep for the two streaming kernels of the hot path on a real GPU:
 //   (1) y = a*x + b   (read 4 B + write 4 B per element)   and   (2) sum(x)   (read 4 B per element),
 // over: vector loads in flight per thread (UNROLL), resident CTAs per SM, CTA size, tile interleaving vs contiguous per-CTA
 // ranges, cache policy of the loads/stores, and a TMA (cp.async.bulk + mbarrier ring, in-place in shared memory) variant.
 // Not part of the product: it only tells us which variant libdab200.so should ship.  Build: nvcc -O3 -gencode
-// arch=compute_100a,code=sm_100a -fmad=false -o sweep_stream sweep_stream.cu ; run: ./sweep_stream [log2n]
+// arch=compute_90a,code=sm_90a -fmad=false -o sweep_stream sweep_stream.cu ; run: ./sweep_stream [log2n]
 #include <cuda_runtime.h>
 
 #include <cstdint>
@@ -49,11 +49,16 @@ __device__ __forceinline__ float4 aff(float4 v, float a, float b) {
     return v;
 }
 
-// ------------------------------------------------------------------ 32-byte (256-bit) accesses: sm_100 ld/st .v8.b32
+// ------------------------------------------------------------------ 32-byte (256-bit) accesses: ld/st .v8.b32 from sm_100 on,
+// two 16-byte accesses before (sm_90 has no 256-bit global access)
 struct __align__(32) f8 { float v[8]; };
 template <int POL>
 __device__ __forceinline__ f8 ld32(const f8* p) {
     f8 r;
+#if __CUDA_ARCH__ < 1000
+    reinterpret_cast<float4*>(r.v)[0] = ld16<POL == 0 ? 0 : POL == 1 ? 1 : 3>(reinterpret_cast<const float4*>(p));
+    reinterpret_cast<float4*>(r.v)[1] = ld16<POL == 0 ? 0 : POL == 1 ? 1 : 3>(reinterpret_cast<const float4*>(p) + 1);
+#else
     unsigned* u = reinterpret_cast<unsigned*>(r.v);
     if (POL == 0)
         asm volatile("ld.global.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];" : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]) : "l"(p));
@@ -61,15 +66,21 @@ __device__ __forceinline__ f8 ld32(const f8* p) {
         asm volatile("ld.global.L1::no_allocate.L2::evict_first.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];" : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]) : "l"(p));
     else
         asm volatile("ld.global.nc.L1::no_allocate.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];" : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]) : "l"(p));
+#endif
     return r;
 }
 template <int POL>
 __device__ __forceinline__ void st32(f8* p, const f8& r) {
+#if __CUDA_ARCH__ < 1000
+    st16<POL == 0 ? 0 : 1>(reinterpret_cast<float4*>(p), reinterpret_cast<const float4*>(r.v)[0]);
+    st16<POL == 0 ? 0 : 1>(reinterpret_cast<float4*>(p) + 1, reinterpret_cast<const float4*>(r.v)[1]);
+#else
     const unsigned* u = reinterpret_cast<const unsigned*>(r.v);
     if (POL == 0)
         asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(u[0]), "r"(u[1]), "r"(u[2]), "r"(u[3]), "r"(u[4]), "r"(u[5]), "r"(u[6]), "r"(u[7]));
     else
         asm volatile("st.global.L1::no_allocate.L2::evict_first.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(u[0]), "r"(u[1]), "r"(u[2]), "r"(u[3]), "r"(u[4]), "r"(u[5]), "r"(u[6]), "r"(u[7]));
+#endif
 }
 template <int THREADS, int UNROLL, int LP, int SP>
 __global__ void __launch_bounds__(THREADS) affine_tiles32(f8* __restrict__ y, const f8* __restrict__ x, size_t nvec, float a, float b) {
