@@ -167,12 +167,13 @@ int32_t dab_comm_destroy(dab_ctx* ctx) {
     if (!ctx || !ctx->comm) return DAB_OK;
     NcclApi& api = nccl();
     cudaSetDevice(ctx->device);
+    const int32_t st = dab_flush_pending(ctx);  // no DAB_ENTER here: queue a deferred dab_affine before tearing down
     cudaStreamSynchronize(ctx->stream);
     if (api.ok) api.CommDestroy((ncclComm_t)ctx->comm);
     ctx->comm = nullptr;
     ctx->rank = 0;
     ctx->nranks = 1;
-    return DAB_OK;
+    return st;
 }
 
 int32_t dab_allgather(dab_ctx* ctx, const void* send_dev, void* recv_dev, size_t nbytes_per_rank) {
@@ -239,11 +240,14 @@ int32_t dab_recv(dab_ctx* ctx, void* recv_dev, size_t nbytes, int32_t peer) {
 //   reduce(op, results)                                                                        -> ordered left fold
 int32_t dab_mapreduce_all(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, const void* map_param, const void* x, size_t n,
                           void* out_host) {
-    DAB_ENTER(ctx);
-    DAB_REQUIRE(ctx, out_host, DAB_ERR_ARG, "dab_mapreduce_all: null out");
+    DAB_ENTER_NOFLUSH(ctx);  // dab_reduce below consumes or flushes the deferred dab_affine
     int32_t rdt;
-    if (op == DAB_EXTREMA) return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_mapreduce_all: extrema combines through dab_reduce + dab_allgather");
-    if (dab_reduce_result_dtype(dtype, op, map, &rdt) != DAB_OK) return dab_fail(ctx, DAB_ERR_ARG, "bad dtype/op");
+    if (!out_host || op == DAB_EXTREMA || dab_reduce_result_dtype(dtype, op, map, &rdt) != DAB_OK) {
+        DAB_FLUSH(ctx);
+        DAB_REQUIRE(ctx, out_host, DAB_ERR_ARG, "dab_mapreduce_all: null out");
+        if (op == DAB_EXTREMA) return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_mapreduce_all: extrema combines through dab_reduce + dab_allgather");
+        return dab_fail(ctx, DAB_ERR_ARG, "bad dtype/op");
+    }
     if ((ctx->mbox_ranks > 1 || !ctx->comm || ctx->nranks == 1) && n > 0) {
         // fused path: ONE kernel = chunk reduce + peer-memory all-gather + ordered fold + scalar into pinned host memory
         ctx->fuse_op = op;
@@ -320,6 +324,7 @@ int32_t dab_mailbox_attach(dab_ctx* ctx, const void* handles, int32_t rank, int3
 int32_t dab_mailbox_detach(dab_ctx* ctx) {
     if (!ctx) return DAB_OK;
     cudaSetDevice(ctx->device);
+    const int32_t st = dab_flush_pending(ctx);  // no DAB_ENTER here: queue a deferred dab_affine before tearing down
     for (int j = 0; j < ctx->mbox_ranks; ++j)
         if (j != ctx->rank && ctx->peer_mbox_host[j]) cudaIpcCloseMemHandle(ctx->peer_mbox_host[j]);
     if (ctx->peer_mbox_dev) cudaFree(ctx->peer_mbox_dev);
@@ -328,7 +333,7 @@ int32_t dab_mailbox_detach(dab_ctx* ctx) {
     ctx->mailbox = nullptr;
     ctx->mbox_ranks = 0;
     cudaGetLastError();
-    return DAB_OK;
+    return st;
 }
 
 

@@ -12,6 +12,18 @@
 #define DAB_SLOT_BYTES 64
 #define DAB_MAX_RANKS 64
 
+// A dab_affine call whose kernel has not been launched yet (dab_elementwise.cu).  y .= a.*x .+ b is usually followed by a
+// reduction of y (sum(y), map!(f, d, d); sum(d)); the reduce kernel can then compute y itself while it streams x and skip
+// re-reading 4 GiB of y from HBM.  The record holds copies of a and b, not the caller's pointers.
+struct dab_pending_affine {
+    int active;
+    int32_t dtype;
+    void* y;
+    const void* x;
+    size_t n;
+    unsigned char a[8], b[8];
+};
+
 struct dab_ctx {
     int device;
     int sm_count;
@@ -51,6 +63,8 @@ struct dab_ctx {
     int opt_gemv_t_cols;    // dab_set_option("gemv_t_cols"): columns one thread of the A'*x kernel carries (4 or 8)
     int opt_gemv_t_waves;   // dab_set_option("gemv_t_waves"): waves of CTAs the A'*x kernel is split into
     int opt_ew_tma;         // dab_set_option("ew_tma"): route aligned unary elementwise launches through the TMA-staged kernel
+    dab_pending_affine pending;  // at most one deferred dab_affine; launched by the next entry or consumed by dab_reduce
+    int defer_off;          // set by dab_stream: foreign work on the raw stream expects every call to be queued already
     char err[512];
 };
 
@@ -70,7 +84,28 @@ int32_t dab_fail_cuda(dab_ctx* ctx, cudaError_t e, const char* what, const char*
         if (!(cond)) return dab_fail((ctx), (status), __VA_ARGS__);  \
     } while (0)
 
+// Launches the deferred dab_affine kernel, if any (dab_elementwise.cu).  The slot is cleared first; a launch error is
+// returned with text naming dab_affine.
+int32_t dab_flush_pending(dab_ctx* ctx);
+
+#define DAB_FLUSH(ctx)                                    \
+    do {                                                  \
+        if ((ctx)->pending.active) {                      \
+            int32_t st__ = dab_flush_pending(ctx);        \
+            if (st__ != DAB_OK) return st__;              \
+        }                                                 \
+    } while (0)
+
+// Every entry point starts with DAB_ENTER, which first queues a deferred dab_affine: work is issued in call order.
 #define DAB_ENTER(ctx)                                                      \
+    do {                                                                    \
+        if ((ctx) == nullptr) return dab_fail(nullptr, DAB_ERR_ARG, "null ctx"); \
+        DAB_CUDA((ctx), cudaSetDevice((ctx)->device));                      \
+        DAB_FLUSH(ctx);                                                     \
+    } while (0)
+
+// dab_reduce, dab_reduce_host and dab_mapreduce_all only: dab_reduce either consumes the deferred dab_affine or flushes it.
+#define DAB_ENTER_NOFLUSH(ctx)                                              \
     do {                                                                    \
         if ((ctx) == nullptr) return dab_fail(nullptr, DAB_ERR_ARG, "null ctx"); \
         DAB_CUDA((ctx), cudaSetDevice((ctx)->device));                      \

@@ -153,6 +153,7 @@ int32_t dab_mailbox_detach(dab_ctx* ctx);
 int32_t dab_shutdown(dab_ctx* ctx) {
     if (!ctx) return DAB_OK;
     cudaSetDevice(ctx->device);
+    const int32_t st = dab_flush_pending(ctx);  // no DAB_ENTER here: a deferred dab_affine still runs before the teardown
     cudaStreamSynchronize(ctx->stream);
     if (ctx->comm) dab_comm_destroy(ctx);
     cudaFree(ctx->block_partials);
@@ -176,7 +177,7 @@ int32_t dab_shutdown(dab_ctx* ctx) {
     cudaFreeHost(ctx->host_slot);
     cudaStreamDestroy(ctx->stream);
     delete ctx;
-    return DAB_OK;
+    return st;
 }
 
 int32_t dab_sync(dab_ctx* ctx) {
@@ -201,9 +202,12 @@ int32_t dab_device_info(dab_ctx* ctx, int32_t* device, int32_t* sm_count, size_t
     return DAB_OK;
 }
 
+// Whoever holds the raw stream may queue work on it directly, and that work expects every earlier call of this ctx to be
+// queued already: DAB_ENTER flushes, and dab_affine stops deferring for the rest of the ctx's life.
 int32_t dab_stream(dab_ctx* ctx, void** stream) {
     DAB_ENTER(ctx);
     DAB_REQUIRE(ctx, stream, DAB_ERR_ARG, "null stream out-pointer");
+    ctx->defer_off = 1;
     *stream = (void*)ctx->stream;
     return DAB_OK;
 }
@@ -212,6 +216,10 @@ int32_t dab_stream(dab_ctx* ctx, void** stream) {
 // TMA-staged shared-memory ring instead of the default flat LDG/STG kernel (same results; measured slower, see dab_elementwise.cu).
 int32_t dab_set_option(dab_ctx* ctx, const char* key, int64_t value) {
     if (!ctx || !key) return dab_fail(ctx, DAB_ERR_ARG, "null argument");
+    if (ctx->pending.active) {  // no DAB_ENTER here: a deferred dab_affine launches as it was called, before the switch changes
+        DAB_CUDA(ctx, cudaSetDevice(ctx->device));
+        DAB_FLUSH(ctx);
+    }
     if (strcmp(key, "ew_tma") == 0) {
         ctx->opt_ew_tma = value != 0;
         return DAB_OK;
@@ -252,6 +260,10 @@ int32_t dab_set_option(dab_ctx* ctx, const char* key, int64_t value) {
 
 int32_t dab_launch_count(dab_ctx* ctx, uint64_t* launches) {
     if (!ctx || !launches) return dab_fail(ctx, DAB_ERR_ARG, "null argument");
+    if (ctx->pending.active) {  // no DAB_ENTER here: count a deferred dab_affine as launched -- it is, from here on
+        DAB_CUDA(ctx, cudaSetDevice(ctx->device));
+        DAB_FLUSH(ctx);
+    }
     *launches = ctx->launches;
     return DAB_OK;
 }

@@ -258,12 +258,6 @@ int32_t launch_ew2(dab_ctx* ctx, T* z, const T* x, const T* y, size_t n, F f) {
 }
 
 // ---- functors --------------------------------------------------------------------------------
-template <typename T>
-struct AffineF {  // a*x + b, two roundings (Julia never contracts; src/broadcast.jl:80 runs Base's loop)
-    T a, b;
-    __device__ __forceinline__ T operator()(T x) const { return jl::add(jl::mul(a, x), b); }
-};
-
 template <typename T, int FN>
 struct UnaryF {
     __device__ __forceinline__ T operator()(T x) const {
@@ -373,7 +367,64 @@ int32_t binary_t(dab_ctx* ctx, int32_t op, T* z, const T* x, const T* y, const T
     }
 }
 
+// A dab_affine call is deferred exactly when launch_ew1 would run ew1_kernel on it: x and y share their 16-byte misalignment,
+// and the TMA variant is off.  x and y are the same array (map!(f, d, d)) or do not overlap, so a consumer that reads x and
+// writes y element by element (dab_reduce.cu) computes the same y.
+template <typename T>
+bool affine_deferrable(const dab_ctx* ctx, const T* y, const T* x, size_t n) {
+    if (n == 0 || ctx->opt_ew_tma || ctx->defer_off) return false;
+    const uintptr_t ux = (uintptr_t)x, uy = (uintptr_t)y;
+    if ((ux & 15) != (uy & 15) || ux % sizeof(T) != 0) return false;
+    const size_t bytes = n * sizeof(T);
+    return ux == uy || ux + bytes <= uy || uy + bytes <= ux;
+}
+
+template <typename T>
+int32_t affine_t(dab_ctx* ctx, int32_t dtype, T* y, const T* x, const void* a, const void* b, size_t n) {
+    const AffineF<T> f{*(const T*)a, *(const T*)b};
+    if (affine_deferrable(ctx, y, x, n)) {
+        dab_pending_affine& p = ctx->pending;
+        p.dtype = dtype;
+        p.y = y;
+        p.x = x;
+        p.n = n;
+        memcpy(p.a, &f.a, sizeof(T));
+        memcpy(p.b, &f.b, sizeof(T));
+        p.active = 1;
+        return DAB_OK;
+    }
+    return launch_ew1(ctx, y, x, n, f);
+}
+
+template <typename T>
+int32_t launch_pending(dab_ctx* ctx, const dab_pending_affine& p) {
+    AffineF<T> f;
+    memcpy(&f.a, p.a, sizeof(T));
+    memcpy(&f.b, p.b, sizeof(T));
+    return launch_ew1(ctx, (T*)p.y, (const T*)p.x, p.n, f);
+}
+
 }  // namespace
+
+int32_t dab_flush_pending(dab_ctx* ctx) {
+    const dab_pending_affine p = ctx->pending;
+    ctx->pending.active = 0;  // before the launch: nothing below may flush again
+    if (!p.active) return DAB_OK;
+    int32_t st;
+    switch (p.dtype) {
+        case DAB_F32: st = launch_pending<float>(ctx, p); break;
+        case DAB_F64: st = launch_pending<double>(ctx, p); break;
+        case DAB_I32: st = launch_pending<int32_t>(ctx, p); break;
+        default: st = launch_pending<long long>(ctx, p); break;  // DAB_I64: dab_affine defers no other dtype
+    }
+    if (st != DAB_OK) {
+        char why[sizeof(ctx->err)];
+        memcpy(why, ctx->err, sizeof(why));
+        why[sizeof(why) - 1] = 0;
+        return dab_fail(ctx, st, "dab_affine (deferred launch): %s", why);
+    }
+    return DAB_OK;
+}
 
 extern "C" {
 
@@ -381,11 +432,10 @@ int32_t dab_affine(dab_ctx* ctx, int32_t dtype, void* y, const void* x, const vo
     DAB_ENTER(ctx);
     DAB_REQUIRE(ctx, ((x && y) || n == 0) && a && b, DAB_ERR_ARG, "dab_affine: null pointer");
     switch (dtype) {
-        case DAB_F32: return launch_ew1(ctx, (float*)y, (const float*)x, n, AffineF<float>{*(const float*)a, *(const float*)b});
-        case DAB_F64: return launch_ew1(ctx, (double*)y, (const double*)x, n, AffineF<double>{*(const double*)a, *(const double*)b});
-        case DAB_I32: return launch_ew1(ctx, (int32_t*)y, (const int32_t*)x, n, AffineF<int32_t>{*(const int32_t*)a, *(const int32_t*)b});
-        case DAB_I64:
-            return launch_ew1(ctx, (long long*)y, (const long long*)x, n, AffineF<long long>{*(const long long*)a, *(const long long*)b});
+        case DAB_F32: return affine_t(ctx, dtype, (float*)y, (const float*)x, a, b, n);
+        case DAB_F64: return affine_t(ctx, dtype, (double*)y, (const double*)x, a, b, n);
+        case DAB_I32: return affine_t(ctx, dtype, (int32_t*)y, (const int32_t*)x, a, b, n);
+        case DAB_I64: return affine_t(ctx, dtype, (long long*)y, (const long long*)x, a, b, n);
         default: return dab_fail(ctx, DAB_ERR_ARG, "dab_affine: bad dtype %d", dtype);
     }
 }

@@ -10,6 +10,10 @@
 // FP64 pipe is idle >90 % of the time and the result is far inside the 1e-6 tolerance.  Warp shuffle -> shared-memory
 // tree -> one partial per CTA -> the LAST CTA to finish (ticket counter) folds the CTA partials in a fixed order, so the
 // result is deterministic for a given (n, grid).  No atomics on data, no second launch.
+//
+// Fused map-store-reduce: when the reduced array is the y of a deferred dab_affine (y .= a.*x .+ b; dab_elementwise.cu) the
+// same kernel reads x instead, stores y and reduces it -- 8 B/element of Float32 instead of 8 (broadcast) + 4 (reduce), and
+// bit-identical to reducing the finished y (AffineStore below).
 #include <type_traits>
 
 #include <cmath>
@@ -20,13 +24,40 @@ namespace {
 
 constexpr int RD_UNROLL = 4;
 
+// What the reduce kernel does with each loaded value before the map.  NoStore: nothing (plain reduction of x).
+struct NoStore {
+    template <typename T>
+    __device__ __forceinline__ void vec(Pack<T>&, size_t) const {}
+    template <typename T>
+    __device__ __forceinline__ T scalar(T v, size_t) const { return v; }
+};
+// AffineStore: the kernel consumes a deferred dab_affine -- x is the affine's input, each value becomes y = a*x + b, is stored
+// to y (same index, same thread, so x == y in place is safe) and is then reduced.  The reduction sees exactly the values a
+// plain reduce of the finished y would load, in the same order.
+template <typename T>
+struct AffineStore {
+    AffineF<T> f;
+    T* y;      // y[i] pairs with x[i]
+    int4* yv;  // y + head as 16-byte vectors (x and y share their misalignment)
+    __device__ __forceinline__ void vec(Pack<T>& p, size_t i) const {
+#pragma unroll
+        for (int k = 0; k < Pack<T>::N; ++k) p.v[k] = f(p.v[k]);
+        st_stream(yv + i, as_int4(p));
+    }
+    __device__ __forceinline__ T scalar(T v, size_t i) const {
+        v = f(v);
+        y[i] = v;
+        return v;
+    }
+};
+
 // Result slot layout (16 bytes at `out`): [0..8) the result in its result dtype, [8..16) the wide accumulator (fp64 for
 // float SUM/PROD -- lets the host see the un-rounded carrier; tests use it).
-template <typename T, typename Map, typename R, typename Out>
+template <typename T, typename Map, typename R, typename Out, typename St>
 __global__ void __launch_bounds__(RD_THREADS, 8) reduce_kernel(const T* __restrict__ x, size_t n, size_t head, Map map,
                                                              typename R::A* __restrict__ partials, unsigned int* counter,
                                                              void* out, int finalize_mode, long long n_for_all, int tiles_per_cta,
-                                                             FusedComm fc) {
+                                                             FusedComm fc, St st) {
     using A = typename R::A;
     using V = typename Map::V;
     constexpr int VPT = 16 / sizeof(T);
@@ -53,6 +84,7 @@ __global__ void __launch_bounds__(RD_THREADS, 8) reduce_kernel(const T* __restri
 #pragma unroll
         for (int u = 0; u < RD_UNROLL; ++u) {
             Pack<T> p = as_pack<T>(r[u]);
+            st.vec(p, base + (size_t)u * RD_THREADS);
             V m[VPT];
 #pragma unroll
             for (int k = 0; k < VPT; ++k) m[k] = map(p.v[k]);
@@ -71,13 +103,14 @@ __global__ void __launch_bounds__(RD_THREADS, 8) reduce_kernel(const T* __restri
     if (blockIdx.x == gridDim.x - 1) {  // remainder vectors, unaligned head, tail
         for (size_t i = ntiles * TILE + threadIdx.x; i < nvec; i += RD_THREADS) {
             Pack<T> p = as_pack<T>(ld_stream(xv + i));
+            st.vec(p, i);
             V m = map(p.v[0]);
 #pragma unroll
             for (int k = 1; k < VPT; ++k) m = R::tile(m, map(p.v[k]));
             acc = R::comb(acc, R::lift(m));
         }
-        for (size_t i = threadIdx.x; i < head; i += RD_THREADS) acc = R::comb(acc, R::lift(map(x[i])));
-        for (size_t i = head + nvec * VPT + threadIdx.x; i < n; i += RD_THREADS) acc = R::comb(acc, R::lift(map(x[i])));
+        for (size_t i = threadIdx.x; i < head; i += RD_THREADS) acc = R::comb(acc, R::lift(map(st.scalar(x[i], i))));
+        for (size_t i = head + nvec * VPT + threadIdx.x; i < n; i += RD_THREADS) acc = R::comb(acc, R::lift(map(st.scalar(x[i], i))));
     }
     acc = block_reduce<R>(acc, smem);
     // ---- two-level "last one out" combine: deterministic, no second launch, tail latency of a few microseconds.
@@ -204,11 +237,12 @@ __global__ void __launch_bounds__(RD_THREADS, 8) reduce_kernel(const T* __restri
     }  // arithmetic Out
 }
 
-template <typename T, typename Map, typename R, typename Out>
-int32_t launch_reduce(dab_ctx* ctx, const T* x, size_t n, Map map, void* out, int finalize_mode) {
+template <typename T, typename Map, typename R, typename Out, typename St = NoStore>
+int32_t launch_reduce(dab_ctx* ctx, const T* x, size_t n, Map map, void* out, int finalize_mode, St st = St()) {
     constexpr int VPT = 16 / sizeof(T);
     size_t head = ((16 - ((uintptr_t)x & 15)) & 15) / sizeof(T);
     if (head > n) head = n;
+    if constexpr (!std::is_same<St, NoStore>::value) st.yv = reinterpret_cast<int4*>(st.y + head);
     size_t tiles = (n - head) / ((size_t)VPT * RD_THREADS * RD_UNROLL);
     size_t k = 2;  // 32 KiB of input per CTA
     if ((tiles + k - 1) / k > (size_t)DAB_MAX_REDUCE_BLOCKS) k = (tiles + DAB_MAX_REDUCE_BLOCKS - 1) / DAB_MAX_REDUCE_BLOCKS;
@@ -229,8 +263,8 @@ int32_t launch_reduce(dab_ctx* ctx, const T* x, size_t n, Map map, void* out, in
         fc.nranks = 1;
         fc.op = ctx->fuse_op;
     }
-    reduce_kernel<T, Map, R, Out><<<(unsigned)grid, RD_THREADS, 0, ctx->stream>>>(x, n, head, map, (typename R::A*)ctx->block_partials,
-                                                                                  ctx->counter, out, finalize_mode, (long long)n, (int)k, fc);
+    reduce_kernel<T, Map, R, Out, St><<<(unsigned)grid, RD_THREADS, 0, ctx->stream>>>(x, n, head, map, (typename R::A*)ctx->block_partials,
+                                                                                      ctx->counter, out, finalize_mode, (long long)n, (int)k, fc, st);
     DAB_LAUNCHED(ctx);
     return DAB_OK;
 }
@@ -287,6 +321,31 @@ int32_t reduce_t(dab_ctx* ctx, int32_t op, int32_t map, const void* param, const
 #undef P
         default: return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "map %d not served by a reduce kernel (no host fallback)", map);
     }
+}
+
+// The deferred dab_affine y .= a.*x .+ b and the reduction of y as ONE kernel: reads x, writes y, reduces y (8 B/element of
+// Float32 instead of 8 + 4).  Same CTA geometry, element-to-thread mapping and fold as reduce_arith<T, DAB_MAP_ID> on y.
+template <typename T>
+int32_t reduce_pending_affine(dab_ctx* ctx, int32_t op, const dab_pending_affine& p, void* out) {
+    using M = MapF<T, DAB_MAP_ID>;
+    AffineStore<T> st;
+    memcpy(&st.f.a, p.a, sizeof(T));
+    memcpy(&st.f.b, p.b, sizeof(T));
+    st.y = (T*)p.y;
+    st.yv = nullptr;  // set by launch_reduce from the head
+    const T* x = (const T*)p.x;
+    switch (op) {
+        case DAB_SUM: return launch_reduce<T, M, SumTraits<T>, ResultOfSum<T>>(ctx, x, p.n, M{(T)0}, out, 0, st);
+        case DAB_PROD: return launch_reduce<T, M, ProdTraits<T>, ResultOfSum<T>>(ctx, x, p.n, M{(T)0}, out, 0, st);
+        case DAB_MAX: return launch_reduce<T, M, MaxTraits<T>, T>(ctx, x, p.n, M{(T)0}, out, 0, st);
+        default: return launch_reduce<T, M, MinTraits<T>, T>(ctx, x, p.n, M{(T)0}, out, 0, st);  // DAB_MIN
+    }
+}
+
+bool consumes_pending(const dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, const void* x, size_t n) {
+    const dab_pending_affine& p = ctx->pending;
+    return p.active && x == p.y && n == p.n && dtype == p.dtype && map == DAB_MAP_ID &&
+           (op == DAB_SUM || op == DAB_PROD || op == DAB_MAX || op == DAB_MIN);
 }
 
 int32_t reduce_u8(dab_ctx* ctx, int32_t op, int32_t map, const uint8_t* x, size_t n, void* out) {
@@ -362,7 +421,18 @@ int32_t dab_reduce_result_dtype(int32_t dtype, int32_t op, int32_t map, int32_t*
 // out_dev: 16 bytes (result + wide accumulator)
 int32_t dab_reduce(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, const void* map_param, const void* x, size_t n,
                    void* out_dev) {
-    DAB_ENTER(ctx);
+    DAB_ENTER_NOFLUSH(ctx);
+    if (out_dev && consumes_pending(ctx, dtype, op, map, x, n)) {
+        const dab_pending_affine p = ctx->pending;
+        ctx->pending.active = 0;
+        switch (dtype) {
+            case DAB_F32: return reduce_pending_affine<float>(ctx, op, p, out_dev);
+            case DAB_F64: return reduce_pending_affine<double>(ctx, op, p, out_dev);
+            case DAB_I32: return reduce_pending_affine<int32_t>(ctx, op, p, out_dev);
+            default: return reduce_pending_affine<long long>(ctx, op, p, out_dev);  // DAB_I64
+        }
+    }
+    DAB_FLUSH(ctx);
     DAB_REQUIRE(ctx, out_dev && (x || n == 0), DAB_ERR_ARG, "dab_reduce: null pointer");
     DAB_REQUIRE(ctx, op >= DAB_SUM && op <= DAB_EXTREMA, DAB_ERR_ARG, "dab_reduce: bad op %d", op);
     if (n == 0) return empty_result(ctx, dtype, op, out_dev);
@@ -379,8 +449,11 @@ int32_t dab_reduce(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, const v
 
 int32_t dab_reduce_host(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, const void* map_param, const void* x, size_t n,
                         void* out_host) {
-    DAB_ENTER(ctx);
-    DAB_REQUIRE(ctx, out_host, DAB_ERR_ARG, "dab_reduce_host: null out");
+    DAB_ENTER_NOFLUSH(ctx);  // dab_reduce consumes or flushes the deferred dab_affine
+    if (!out_host) {
+        DAB_FLUSH(ctx);
+        return dab_fail(ctx, DAB_ERR_ARG, "dab_reduce_host: null out");
+    }
     int32_t st = dab_reduce(ctx, dtype, op, map, map_param, x, n, ctx->result_slot);
     if (st != DAB_OK) return st;
     DAB_CUDA(ctx, cudaMemcpyAsync(ctx->host_slot, ctx->result_slot, 16, cudaMemcpyDeviceToHost, ctx->stream));

@@ -103,3 +103,11 @@ __device__ __forceinline__ T sign(T a) {  // Julia sign: keeps +-0 and NaN
 }
 
 }  // namespace jl
+
+// y = a*x + b of dab_affine, two roundings (Julia never contracts; src/broadcast.jl:80 runs Base's loop).  Shared by the
+// elementwise kernel and the reduce kernel that consumes a deferred dab_affine (dab_reduce.cu).
+template <typename T>
+struct AffineF {
+    T a, b;
+    __device__ __forceinline__ T operator()(T x) const { return jl::add(jl::mul(a, x), b); }
+};

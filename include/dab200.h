@@ -22,9 +22,16 @@
  *   - a dab_ctx is bound to ONE device and owns ONE stream.  The reference runs one
  *     single-threaded Julia process per worker (src/mapreduce.jl:6-10): one ctx per
  *     worker process.  All compute entry points are ASYNCHRONOUS on the ctx stream
- *     (== remotecall); dab_sync and the *_host variants are the sync points
+ *     (== remotecall); dab_sync, events and the *_host variants are the sync points
  *     (== remotecall_wait / remotecall_fetch).  A ctx must not be used from two threads
  *     at once; different ctxs are independent.
+ *   - a compute call is queued on the ctx stream no later than the next call on that ctx.
+ *     dab_affine may be held back until then, so that a following dab_reduce /
+ *     dab_reduce_host / dab_mapreduce_all of its output (same pointer, n and dtype, MAP_ID,
+ *     SUM/PROD/MAX/MIN) runs as ONE kernel that stores y and reduces it; results are
+ *     bit-identical either way.  dab_launch_count counts the held-back call as launched.
+ *     dab_stream turns this off for the rest of the ctx's life (work queued directly on
+ *     the raw stream finds every earlier call already queued).
  *   - arrays are column-major (Julia), element counts are size_t (8 GiB chunk = 2^31 floats).
  *   - floating-point elementwise arithmetic is IEEE round-to-nearest per operation and is
  *     NEVER contracted into FMA (Julia semantics, SURVEY Appendix A.4).
@@ -113,7 +120,8 @@ const char* dab_status_string(int32_t status);
 /* remotecall_wait: block until everything queued on the ctx stream is done. */
 int32_t dab_sync(dab_ctx* ctx);
 int32_t dab_device_info(dab_ctx* ctx, int32_t* device, int32_t* sm_count, size_t* free_bytes, size_t* total_bytes);
-/* the ctx's cudaStream_t (as void*), so a host runtime can order its own work after ours. */
+/* the ctx's cudaStream_t (as void*), so a host runtime can order its own work after ours.  Queues a held-back
+ * dab_affine and stops holding any back on this ctx from then on. */
 int32_t dab_stream(dab_ctx* ctx, void** stream);
 /* tuning switches; "combine_timeout_ms" = wall-clock bound of the fused combine's wait for a peer; "ew_tma" = 1 routes aligned unary elementwise launches through the TMA-staged (cp.async.bulk + mbarrier
  * ring) kernel instead of the default flat LDG/STG kernel -- identical results, measured slower (DESIGN.md section 3). */
