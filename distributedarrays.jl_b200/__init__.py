@@ -4,7 +4,8 @@ Import it as ``darray_b200`` (the directory name is not a Python identifier; ``d
 loader shim).  The public names mirror DistributedArrays.jl's for this path: ``DArray``, ``distribute``, ``localpart``,
 ``localindices``, ``locate``, ``makelocal``, ``procs``, ``dzeros/dones/dfill/drand``, ``map`` (``map_``), ``map!``
 (``map_inplace``), broadcast (``broadcast`` / ``broadcast_into``), ``reduce``, ``mapreduce``, ``sum``, ``prod``,
-``maximum``, ``minimum``, ``all``, ``any``, ``count``, ``extrema``, ``Array(d)`` (``to_array``), range ``getindex``.
+``maximum``, ``minimum``, ``all``, ``any``, ``count``, ``extrema``, ``mapslices`` (with ``sort``, ``svdvals``, reductions, elementwise and
+constant slice functions), ``Array(d)`` (``to_array``), range ``getindex``.
 
 Everything computes on the GPU through ``csrc/libdab200.so`` (C ABI: ``include/dab200.h``).  There is no CPU fallback:
 importing works anywhere, but the first op without the built extension or without an H100 raises.
@@ -24,6 +25,7 @@ from ._mapreduce import (all, any, axpy_, count, dot, extrema, isequal, mapreduc
                          prod, reduce, rmul_, sum)
 from ._linalg import Adjoint, Transpose, adjoint, copy_transposed, lmul_diag, matmat, matmul, mul_, mul_mat_, rmul_diag, transpose
 from ._sort import sort, sort_with_boundaries
+from ._slices import mapslices, svdvals
 from .runtime import Runtime, init, myid, nworkers, runtime, workers
 
 __all__ = [n for n in dir() if not n.startswith("_")]

@@ -47,6 +47,7 @@ class _TagTypes(dict):
 _NPT = _TagTypes({"bool": np.dtype(np.bool_), "i32": np.dtype(np.int32), "i64": np.dtype(np.int64), "f32": np.dtype(np.float32),
                   "f64": np.dtype(np.float64)})
 _TAG = {v: k for k, v in _NPT.items()}
+SLICE_TRACING = [0]   # > 0 while mapslices (_slices.py) calls f on the slice tracer
 _CT = {"bool": "bool", "i32": "int", "i64": "long long", "i128": "i128", "f32": "float", "f64": "double"}
 
 
@@ -150,6 +151,16 @@ class Expr:
 
     def __bool__(self):
         raise TypeError("data-dependent Python control flow cannot be traced; use dab.ifelse(cond, a, b)")
+
+    def __array__(self, dtype=None, copy=None):
+        # While mapslices traces f, the expression stands for a whole slice: NumPy must not take it for one element (np.median(x)
+        # would reduce a 0-d object array to x itself).  Otherwise NumPy sees what it saw before: a 0-d object array holding it.
+        if SLICE_TRACING[0]:
+            raise TypeError("a mapslices slice cannot be converted to a NumPy array; served slice functions: sort, svdvals, "
+                            "sum/prod/maximum/minimum of an elementwise expression")
+        a = np.empty((), dtype=object)
+        a[()] = self
+        return a if dtype is None else a.astype(dtype)
 
     def key(self) -> str:
         if self.op == "arg":

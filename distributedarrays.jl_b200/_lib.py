@@ -19,6 +19,8 @@ SUM, PROD, MAX, MIN, ALL, ANY, COUNT, EXTREMA = range(8)
 MAP_ID, MAP_ABS, MAP_ABS2, MAP_NEG, MAP_SQRT, MAP_INV, MAP_FLOOR, MAP_CEIL, MAP_SIGN = range(9)
 MAP_EQ, MAP_NE, MAP_LT, MAP_LE, MAP_GT, MAP_GE, MAP_ISNAN, MAP_NONZERO = range(16, 24)
 ADD, SUB, MUL, DIV, REM, BMAX, BMIN, MOD, IDIV, AND, OR, XOR = range(12)
+SORT_SLICES_SMEM_LEN = 8192                   # longest fibre dab_sort_slices sorts in shared memory
+SVDVALS_MAX_K, SVDVALS_MAX_ELEMS = 32, 4096   # dab_svdvals_batched serves min(m, n) <= 32 and m * n <= 4096
 
 
 class DabError(RuntimeError):
@@ -101,6 +103,8 @@ _SIGS = {
     "dab_sorted_split": (_i32, [_vp, _i32, _vp, _sz, _vp, _i32, C.POINTER(C.c_ulonglong)]),
     "dab_sort_by_key": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _sz, _sz]),
     "dab_sort_by_key_scratch_bytes": (_i32, [_i32, _sz, C.POINTER(_sz)]),
+    "dab_sort_slices": (_i32, [_vp, _i32, _vp, _vp, _sz, _sz, _sz]),
+    "dab_svdvals_batched": (_i32, [_vp, _i32, _vp, _sz, _sz, _sz, _vp, _vp]),
     "dab_comm_unique_id": (_i32, [_vp]),
     "dab_comm_init_rank": (_i32, [_vp, _vp, _i32, _i32]),
     "dab_comm_destroy": (_i32, [_vp]),

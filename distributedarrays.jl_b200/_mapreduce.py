@@ -258,6 +258,10 @@ def mapreduce(f: Optional[Callable], op, d: DArray, *ds, dims=None, init=None, _
     (same-size DArrays / arrays / scalars) ``f`` takes one value per argument: ``mapreduce(*, +, x, y)`` is ``dot(x, y)``.
     A ``SubDArray`` is reduced through ``DArray(d)`` exactly as the reference does (src/mapreduce.jl:36)."""
     from ._darray import SubDArray
+    if isinstance(d, Expr):
+        from . import _slices
+        if _slices.tracing():                                  # f(slice) of mapslices(f, D; dims) is being recognised
+            return _slices.reduce_of_slice(f, op, d, ds, dims, init)
     if isinstance(d, SubDArray):
         tmp = d.to_darray()
         try:

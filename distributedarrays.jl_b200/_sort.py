@@ -187,7 +187,12 @@ def sort(d: DArray, sample=True, by=None, alg=None, **kwargs) -> DArray:  # noqa
     worker balance the parts), False (uniform between min(d) and max(d)), a ``(min, max)`` tuple, or an array used as the sample.
     ``by``: a traceable key function (same closures as broadcast / map); values are ordered stably by ``by(x)``.
     ``alg`` is accepted and ignored: a keys-only sort has one result whatever the algorithm, and the keyed sort is stable like
-    Julia's default."""
+    Julia's default.  Called on the slice of ``mapslices(sort, D; dims)`` it stands for the per-slice sort (``dab_sort_slices``)."""
+    from ._broadcast import Expr
+    if isinstance(d, Expr):
+        from . import _slices
+        if _slices.tracing():
+            return _slices.sort_of_slice(d, by, kwargs)
     return sort_with_boundaries(d, sample, by, alg, **kwargs)[0]
 
 

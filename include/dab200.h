@@ -308,6 +308,27 @@ int32_t dab_sort_by_key_scratch_bytes(int32_t key_dtype, size_t n, size_t* bytes
 int32_t dab_sorted_split(dab_ctx* ctx, int32_t dtype, const void* sorted, size_t n, const void* bounds_host, int32_t nb,
                          unsigned long long* counts_host);
 
+/* ==== slice functions of mapslices(f, D; dims) (src/mapreduce.jl:191-208) =================
+ * The  mapslices(f, localpart(y), dims=z)  run on every worker (:205) for the f that need a kernel of their own. */
+
+/* Longest fibre dab_sort_slices sorts in shared memory; longer fibres go through K11 (dab_sort) one by one. */
+#define DAB_SORT_SLICES_SMEM_LEN 8192
+/* out[fibre] = sort(in[fibre]) for every fibre x[i + inner*(r + len*o)], r < len, of the column-major (inner, len, outer) box, i < inner,
+ * o < outer: mapslices(sort, lp, dims=d) with the chunk collapsed around dimension d.  Julia's isless order (SortKey<T>, as K11); every
+ * output fibre is bit-identical to dab_sort of that fibre (NaNs included: the key encoding is a bijection).  in == out sorts in place;
+ * other overlaps are not allowed.  Scratch of the long-fibre path comes from the ctx block cache.  dtypes: F32 F64 I32 I64. */
+int32_t dab_sort_slices(dab_ctx* ctx, int32_t dtype, const void* in, void* out, size_t inner, size_t len, size_t outer);
+
+/* Limits of dab_svdvals_batched: min(m, n) and m * n. */
+#define DAB_SVDVALS_MAX_K 32
+#define DAB_SVDVALS_MAX_ELEMS 4096
+/* S[b*k .. b*k + k) = svdvals(A_b), descending, k = min(m, n), for the `batch` dense column-major m x n matrices A_b stored one after the
+ * other: mapslices(svdvals, lp, dims=(d1, d2)) once the slices are packed.  One-sided Jacobi in fp64 (Float32 input is rounded once at
+ * the end).  dtypes F32 F64; min(m, n) <= DAB_SVDVALS_MAX_K and m * n <= DAB_SVDVALS_MAX_ELEMS, otherwise DAB_ERR_UNSUPPORTED.  status: a
+ * device int32 set to 0 by the call and to 1 by the kernel when a matrix holds a NaN or Inf (its values are then NaN); Julia's LAPACK
+ * wrapper rejects such input (chkfinite), so the host runtime raises ArgumentError once it has read status. */
+int32_t dab_svdvals_batched(dab_ctx* ctx, int32_t dtype, const void* A, size_t m, size_t n, size_t batch, void* S, int32_t* status);
+
 /* ==== cross-worker combine: NCCL over NVLink (replaces Distributed.remotecall_fetch on
  *      this path only; src/mapreduce.jl:30-34, 72-80; src/darray.jl:809-815) ============== */
 /* 128-byte ncclUniqueId; rank 0 creates it, the host runtime ships it to the other workers. */

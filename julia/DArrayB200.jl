@@ -21,6 +21,7 @@
 #   src/linalg.jl:1-17   transpose!(lp, rp)               LinearAlgebra.transpose! / adjoint!        dab_transpose_box
 #   src/sort.jl:8,22,61  sort(localpart(d)), sort!(lp)    Base.sort / Base.sort!                     dab_sort
 #   src/sort.jl:8,22,61  sort(localpart(d); by = f)       sort_by (keys = f.(a) by broadcast)        dab_sort_by_key
+#   src/mapreduce.jl:205 mapslices(f, localpart(y), dims) mapslices_sort / svdvals_batched       dab_sort_slices / dab_svdvals_batched
 module DArrayB200
 
 using Distributed, DistributedArrays, LinearAlgebra
@@ -283,6 +284,25 @@ function sort_by(a::B200Array{T,1}, keys::B200Array{K,1}) where {T,K}
 end
 # keyword arguments do not take part in dispatch: ONE method serves both spellings
 Base.sort(a::B200Array{T,1}; by = identity, kw...) where {T} = by === identity ? sort_keys(a) : sort_by(a, by.(a))
+
+# mapslices(f, localpart(y), dims=z)  (src/mapreduce.jl:205) for f = sort (one dim) and f = svdvals (two dims, slices already packed as
+# `batch` column-major m x n matrices: the Python runtime packs them with dab_gather_box).  Julia's LAPACK wrapper rejects non-finite
+# input (chkfinite); so does this one, once the status word has been read back.
+function mapslices_sort(a::B200Array{T,N}, d::Int) where {T,N}
+    out = B200Array{T,N}(undef, size(a))
+    inner, len, outer = prod(size(a)[1:d-1]; init = 1), size(a, d), prod(size(a)[d+1:N]; init = 1)
+    check(ccall((:dab_sort_slices, libdab), Int32, (Ptr{Cvoid}, Int32, Ptr{Cvoid}, Ptr{Cvoid}, Csize_t, Csize_t, Csize_t),
+                ctx(), dab_dtype(T), a.ptr, out.ptr, inner, len, outer), ctx())
+    out
+end
+function svdvals_batched(a::B200Array{T,3}) where {T<:Union{Float32,Float64}}
+    m, n, batch = size(a)
+    S = B200Array{T,2}(undef, (min(m, n), batch)); st = B200Array{Int32,1}(undef, (1,))
+    check(ccall((:dab_svdvals_batched, libdab), Int32, (Ptr{Cvoid}, Int32, Ptr{Cvoid}, Csize_t, Csize_t, Csize_t, Ptr{Cvoid}, Ptr{Cvoid}),
+                ctx(), dab_dtype(T), a.ptr, m, n, batch, S.ptr, st.ptr), ctx())
+    Array(st)[1] == 0 || throw(ArgumentError("matrix contains Infs or NaNs"))
+    S
+end
 
 # localpart(A) * Bjk, transpose(localpart(A)) * Bjk inside _matmatmul!  (src/linalg.jl:218-226): K12, wgmma 3xTF32 for Float32
 function gemm(transA::Bool, A::B200Array{T,2}, B::B200Array{T,2}) where {T}
