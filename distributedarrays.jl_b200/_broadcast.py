@@ -128,6 +128,19 @@ class Expr:
     __ne__ = lambda s, o: s._bin("ne", o)  # type: ignore[assignment]
     __hash__ = None  # type: ignore[assignment]
 
+    def __matmul__(self, o):
+        # a matrix product of slices (ppeval(*, A, B)): a marker while a slice function is traced, and no operator otherwise
+        if not SLICE_TRACING[0]:
+            return NotImplemented
+        from ._slices import matmul_of_slices
+        return matmul_of_slices(self, o)
+
+    def __rmatmul__(self, o):
+        if not SLICE_TRACING[0]:
+            return NotImplemented
+        from ._slices import matmul_of_slices
+        return matmul_of_slices(o, self)
+
     def __neg__(self):
         return unop("neg", self)
 

@@ -21,6 +21,7 @@ MAP_EQ, MAP_NE, MAP_LT, MAP_LE, MAP_GT, MAP_GE, MAP_ISNAN, MAP_NONZERO = range(1
 ADD, SUB, MUL, DIV, REM, BMAX, BMIN, MOD, IDIV, AND, OR, XOR = range(12)
 SORT_SLICES_SMEM_LEN = 8192                   # longest fibre dab_sort_slices sorts in shared memory
 SVDVALS_MAX_K, SVDVALS_MAX_ELEMS = 32, 4096   # dab_svdvals_batched serves min(m, n) <= 32 and m * n <= 4096
+EIGVALS_SYM_MAX_N = 64                        # dab_eigvals_sym_batched serves n <= 64
 
 
 class DabError(RuntimeError):
@@ -105,6 +106,8 @@ _SIGS = {
     "dab_sort_by_key_scratch_bytes": (_i32, [_i32, _sz, C.POINTER(_sz)]),
     "dab_sort_slices": (_i32, [_vp, _i32, _vp, _vp, _sz, _sz, _sz]),
     "dab_svdvals_batched": (_i32, [_vp, _i32, _vp, _sz, _sz, _sz, _vp, _vp]),
+    "dab_matmul_batched": (_i32, [_vp, _i32, _sz, _sz, _sz, _vp, _sz, _vp, _sz, _vp, _sz]),
+    "dab_eigvals_sym_batched": (_i32, [_vp, _i32, _vp, _sz, _sz, _vp, _vp]),
     "dab_comm_unique_id": (_i32, [_vp]),
     "dab_comm_init_rank": (_i32, [_vp, _vp, _i32, _i32]),
     "dab_comm_destroy": (_i32, [_vp]),

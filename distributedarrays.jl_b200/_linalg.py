@@ -266,7 +266,12 @@ def mul_(y: DArray, A: Union[DArray, Transpose], x, alpha=1, beta=0) -> DArray:
 
 def matmul(A: Union[DArray, Transpose], x) -> DArray:
     """``A*x`` (reference src/linalg.jl:280-284): y lives on ``procs(A)[:,1]`` with one chunk per grid row; ``A'*x`` /
-    ``transpose(A)*x`` (:293-301, 303-311): on ``procs(A)[1,:]``, one chunk per grid column."""
+    ``transpose(A)*x`` (:293-301, 303-311): on ``procs(A)[1,:]``, one chunk per grid column.  Inside ``ppeval`` (a traced slice
+    function) the product of slices is recorded for ``dab_matmul_batched`` instead."""
+    from ._broadcast import Expr
+    if isinstance(A, Expr) or isinstance(x, Expr):
+        from ._slices import matmul_of_slices
+        return matmul_of_slices(A, x)
     M, trans = _unwrap(A)
     xnd = len(x.dims) if isinstance(x, DArray) else np.ndim(x)
     if xnd == 2:

@@ -15,6 +15,7 @@ and the kernels behind them:
   ``svdvals``, two dimensions                    one ``dab_gather_box`` packs the slices as (m, n, batch), ``dab_svdvals_batched``,
                                                  one ``dab_gather_box`` scatters (k, 1, batch) back; Int32 / Int64 are converted to
                                                  Float64 first, as Julia's ``svdvals`` does
+  ``eigvals``, two dimensions, square slices     the same with ``dab_eigvals_sym_batched`` (real symmetric slices; see ``eigvals``)
   ``sum/prod/maximum/minimum(g(slice))``, g an   the per-chunk dimensional reduction (``reduce_chunk_dims``); with ``dims=()`` there is
   elementwise traced expression (or identity)    nothing to reduce and it is one elementwise launch of g
   an elementwise expression ``g(slice)``         one elementwise launch (the result has the slice's shape)
@@ -39,7 +40,8 @@ _SORT_DTYPES = (np.dtype(np.float32), np.dtype(np.float64), np.dtype(np.int32), 
 
 
 def tracing() -> bool:
-    """True while ``mapslices`` calls ``f`` on the slice tracer: ``sort``, ``svdvals`` and the reductions then return a marker."""
+    """True while ``mapslices`` / ``ppeval`` call ``f`` on slice tracers: ``sort``, ``svdvals``, ``eigvals``, ``@`` and the reductions then
+    return a marker."""
     return SLICE_TRACING[0] > 0
 
 
@@ -49,6 +51,17 @@ class SliceSort:
 
 class SliceSvdvals:
     """``f(slice) = svdvals(slice)``."""
+
+
+class SliceEigvals:
+    """``f(slice) = eigvals(slice)``."""
+
+
+class SliceMatmul:
+    """``f(slices...) = a * b`` (Julia's matrix product, Python's ``@``): each operand a slice tracer or a host array."""
+
+    def __init__(self, a, b):
+        self.a, self.b = a, b
 
 
 class SliceReduce:
@@ -89,6 +102,29 @@ def svdvals(A):
             raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "mapslices: svdvals of an expression of the slice is not served")
         return SliceSvdvals()
     raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "svdvals is served for the slices of a DArray only: mapslices(svdvals, D, dims=(d1, d2))")
+
+
+def eigvals(A, B=None):
+    """``eigvals`` of a real symmetric slice, ascending: ``ppeval(eigvals, D)`` or ``mapslices(eigvals, D, dims=(d1, d2))``.  There is no
+    distributed eigensolver; anywhere else this raises.  Julia takes the symmetric path when ``ishermitian(A)`` holds; a slice that is not
+    exactly symmetric has complex eigenvalues in general and raises ``UnsupportedError`` once the kernel has flagged it.  The generalised
+    problem ``eigvals(A, B)`` is not served."""
+    if isinstance(A, Expr) and tracing():
+        if B is not None:
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "eigvals(A, B): the generalised eigenvalue problem is complex in general and is "
+                                        "not served")
+        if not _is_slice(A):
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "eigvals of an expression of the slice is not served")
+        return SliceEigvals()
+    raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "eigvals is served for the slices of a DArray only: ppeval(eigvals, D) or "
+                                "mapslices(eigvals, D, dims=(d1, d2))")
+
+
+def matmul_of_slices(a, b):
+    """``a @ b`` while a slice function is traced (``Expr.__matmul__``, ``dab.matmul``); anywhere else it raises."""
+    if not tracing():
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "a matrix product of a traced expression is only served inside ppeval")
+    return SliceMatmul(a, b)
 
 
 # ---- the rules of Base.mapslices ----------------------------------------------------------------------------------------------------
@@ -170,6 +206,8 @@ class _Plan:
             return tuple(sl)
         if self.kind == "svdvals":
             return (min(sl),)
+        if self.kind == "eigvals":
+            return (sl[0],)
         if self.kind == "reduce":
             return ()
         return tuple(self.const.shape)
@@ -179,7 +217,6 @@ class _Plan:
 
 
 def _classify(f, D: DArray, dims: Tuple[int, ...]) -> _Plan:
-    from ._mapreduce import _result_dtype, classify_map
     dt = D.dtype
     tag = tag_of(dt)
     x = Expr("arg", (), tag, 0)
@@ -194,6 +231,21 @@ def _classify(f, D: DArray, dims: Tuple[int, ...]) -> _Plan:
                                     "expression of the slice, elementwise expressions, constant results") from None
     finally:
         SLICE_TRACING[0] -= 1
+    return plan_of(r, dims, dt)
+
+
+def plan_of(r, dims: Tuple[int, ...], dt: np.dtype, what: str = "mapslices") -> _Plan:
+    """The plan of a traced slice function whose result is ``r``, for slices over ``dims`` of an array of eltype ``dt``."""
+    from ._mapreduce import _result_dtype, classify_map
+    if isinstance(r, SliceMatmul):
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what}: matrix products of slices are served by ppeval(*, A, B) only")
+    if isinstance(r, SliceEigvals):
+        if len(dims) != 2:
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what}(eigvals) is served for matrix slices (two slice dimensions), got "
+                                        f"dims {dims}")
+        if dt not in _SORT_DTYPES:
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what}(eigvals): eltype {dt} (served: Float32 Float64 Int32 Int64)")
+        return _Plan("eigvals", dims, dt if dt.kind == "f" else np.dtype(np.float64))
     if isinstance(r, SliceSort):
         if len(dims) != 1:
             raise _lib.ArgumentError(_lib.ERR_ARG, f"mapslices(sort): the slice over dims {dims} is not a vector; sort of a multi-dimensional "
@@ -236,14 +288,15 @@ def _sort_chunk(rt, plan: _Plan, ch: B200Array, out: B200Array):
     _lib.call("dab_sort_slices", rt.ctx, dab_dtype(ch.dtype), C.c_void_p(ch.ptr), C.c_void_p(out.ptr), inner, ln, outer)
 
 
-def _svdvals_chunk(rt, plan: _Plan, ch: B200Array, out: B200Array, status_ptr: int, temps: List[B200Array]):
+def _packed_chunk(rt, plan: _Plan, ch: B200Array, out: B200Array, status_ptr: int, temps: List[B200Array]):
+    """svdvals / eigvals: the slices packed as (m, n, batch), one batched kernel, the (k, batch) values scattered into the chunk."""
     d1, d2 = plan.dims
     s = ch.shape
     m, n = s[d1 - 1], s[d2 - 1]
     k = min(m, n)
     wdt = plan.dtype
     src = ch
-    if ch.dtype != wdt:                                            # svdvals(::Matrix{Int}) works on Float64
+    if ch.dtype != wdt:                                            # svdvals / eigvals(::Matrix{Int}) work on Float64
         src = B200Array.empty(rt, s, wdt, temp=True)
         temps.append(src)
         run_local(rt, convert(Expr("arg", (), tag_of(ch.dtype), 0), tag_of(wdt)), src, [LocalArg(ch, None, tag_of(ch.dtype))])
@@ -265,7 +318,10 @@ def _svdvals_chunk(rt, plan: _Plan, ch: B200Array, out: B200Array, status_ptr: i
             bstr *= s[j]
     es = wdt.itemsize
     _gather(rt, es, packed.ptr, pstr, src.ptr, _dense_strides(s), s)                 # slices -> (m, n, batch)
-    _lib.call("dab_svdvals_batched", rt.ctx, dab_dtype(wdt), C.c_void_p(packed.ptr), m, n, batch, C.c_void_p(S.ptr), C.c_void_p(status_ptr))
+    if plan.kind == "svdvals":
+        _lib.call("dab_svdvals_batched", rt.ctx, dab_dtype(wdt), C.c_void_p(packed.ptr), m, n, batch, C.c_void_p(S.ptr), C.c_void_p(status_ptr))
+    else:
+        _lib.call("dab_eigvals_sym_batched", rt.ctx, dab_dtype(wdt), C.c_void_p(packed.ptr), n, batch, C.c_void_p(S.ptr), C.c_void_p(status_ptr))
     _gather(rt, es, out.ptr, _dense_strides(out.shape), S.ptr, sstr, out.shape)      # (k, 1, batch) -> the result chunk
 
 
@@ -294,6 +350,49 @@ def _const_chunk(rt, plan: _Plan, cdev: B200Array, out: B200Array):
         if j < c.ndim:
             src_strides[d - 1] = cstr[j]
     _gather(rt, c.dtype.itemsize, out.ptr, _dense_strides(out.shape), cdev.ptr, src_strides, out.shape)
+
+
+def check_limits(plan: _Plan, shapes, what: str = "mapslices"):
+    """The kernels' limits on the slices of chunks of ``shapes``, checked before anything is launched."""
+    if plan.kind not in ("svdvals", "eigvals"):
+        return
+    d1, d2 = plan.dims
+    for s in shapes:
+        m, n = s[d1 - 1], s[d2 - 1]
+        if plan.kind == "svdvals" and (min(m, n) > _lib.SVDVALS_MAX_K or m * n > _lib.SVDVALS_MAX_ELEMS):
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what}(svdvals): slices of {m}x{n}; served: min(m,n) <= "
+                                        f"{_lib.SVDVALS_MAX_K} and m*n <= {_lib.SVDVALS_MAX_ELEMS}")
+        if plan.kind == "eigvals":
+            if m != n:                                             # LinearAlgebra.checksquare
+                raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, f"matrix is not square: dimensions are ({m}, {n})")
+            if n > _lib.EIGVALS_SYM_MAX_N:
+                raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what}(eigvals): slices of {m}x{n}; served: n <= {_lib.EIGVALS_SYM_MAX_N}")
+
+
+def raise_on_status(rt, flags: int):
+    """The status words of dab_svdvals_batched / dab_eigvals_sym_batched, ORed over this rank's chunks: every rank raises, or none."""
+    if rt.world > 1:                                               # the ranks stay in step
+        for f in rt.allgather_object(flags):
+            flags |= int(f)
+    if flags & 1:
+        raise _lib.ArgumentError(_lib.ERR_ARG, "ArgumentError: matrix contains Infs or NaNs")
+    if flags & 2:
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "eigvals: a slice is not symmetric; its eigenvalues are complex in general and "
+                                    "complex element types are not served")
+
+
+def run_chunk(rt, plan: _Plan, ch: B200Array, out: B200Array, status_ptr: int, cdev, temps: List[B200Array]):
+    """One chunk of a mapslices plan: ``out`` (already of the result shape) from ``ch``."""
+    if plan.kind == "sort":
+        _sort_chunk(rt, plan, ch, out)
+    elif plan.kind in ("svdvals", "eigvals"):
+        _packed_chunk(rt, plan, ch, out, status_ptr, temps)
+    elif plan.kind == "reduce":
+        _reduce_chunk(rt, plan, ch, out, temps)
+    elif plan.kind == "map":
+        run_local(rt, plan.expr, out, [LocalArg(ch, None, tag_of(ch.dtype))])
+    else:
+        _const_chunk(rt, plan, cdev, out)
 
 
 def _redistribute(D: DArray, p) -> DArray:
@@ -333,12 +432,7 @@ def mapslices(f, D: DArray, dims) -> DArray:
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "mapslices over a DArray with an empty localpart is not served")
     in_shapes = [shape_of(I) for I in L.indices]
     out_shapes = [plan.out_shape(s) for s in in_shapes]
-    if plan.kind == "svdvals":
-        for s in in_shapes:
-            m, n = s[dims[0] - 1], s[dims[1] - 1]
-            if min(m, n) > _lib.SVDVALS_MAX_K or m * n > _lib.SVDVALS_MAX_ELEMS:
-                raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"mapslices(svdvals): slices of {m}x{n}; served: min(m,n) <= "
-                                            f"{_lib.SVDVALS_MAX_K} and m*n <= {_lib.SVDVALS_MAX_ELEMS}")
+    check_limits(plan, in_shapes)
     layout = layout_from_chunk_shapes(out_shapes, L.grid, L.pids)
     # ---- launches
     rt = D.rt
@@ -347,7 +441,7 @@ def mapslices(f, D: DArray, dims) -> DArray:
     chunks: Dict[int, B200Array] = {}
     status = cdev = None
     try:
-        if plan.kind == "svdvals":
+        if plan.kind in ("svdvals", "eigvals"):
             status = B200Array.empty(rt, (max(1, len(W.chunks)),), np.int32, temp=True)
         if plan.kind == "const":
             cdev = B200Array.from_numpy(rt, plan.const) if plan.const.size else None
@@ -356,22 +450,9 @@ def mapslices(f, D: DArray, dims) -> DArray:
             chunks[pid] = out
             if out.size == 0:
                 continue
-            if plan.kind == "sort":
-                _sort_chunk(rt, plan, ch, out)
-            elif plan.kind == "svdvals":
-                _svdvals_chunk(rt, plan, ch, out, status.ptr + 4 * slot, temps)
-            elif plan.kind == "reduce":
-                _reduce_chunk(rt, plan, ch, out, temps)
-            elif plan.kind == "map":
-                run_local(rt, plan.expr, out, [LocalArg(ch, None, tag_of(ch.dtype))])
-            else:
-                _const_chunk(rt, plan, cdev, out)
+            run_chunk(rt, plan, ch, out, status.ptr + 4 * slot if status is not None else 0, cdev, temps)
         if status is not None:
-            bad = bool(np.any(status.to_numpy()[:len(W.chunks)] != 0))
-            if rt.world > 1:                                   # every rank raises, or none: the ranks stay in step
-                bad = any(rt.allgather_object(bad))
-            if bad:
-                raise _lib.ArgumentError(_lib.ERR_ARG, "ArgumentError: matrix contains Infs or NaNs")
+            raise_on_status(rt, int(np.bitwise_or.reduce(status.to_numpy()[:len(W.chunks)], initial=0)))
     except BaseException:
         for out in chunks.values():
             out.free()

@@ -81,3 +81,36 @@ constexpr int DAB_SVD_MAX_SWEEPS = 40;
 
 // pair tolerance of a sweep over columns of `rows` entries (LAPACK dgesvj's sqrt(m) * eps)
 __host__ __device__ inline double slices_jacobi_tol(int rows) { return 2.220446049250313e-16 * sqrt((double)rows); }
+
+// ---- batched symmetric eigenvalues: two-sided cyclic Jacobi ---------------------------------------------------------------------------
+// A round takes the round-robin pairs of slices_rr_pair: every rotation is computed from the current 2x2 pivots first, then all rows
+// p, q are rotated (J^T A), then all columns (A J); the pairs of a round are disjoint, so this is J^T A J exactly.  A sweep is np - 1
+// rounds; sweeps stop when no pair needed a rotation, or after DAB_EIG_MAX_SWEEPS.
+constexpr int DAB_EIG_MAX_SWEEPS = 40;
+// relative off-diagonal test: |a_pq| <= eps sqrt(|a_pp| |a_qq|) counts as zero ...
+constexpr double DAB_EIG_TOL = 2.220446049250313e-16;
+// ... and so does |a_pq| <= 2^-80 once the matrix is scaled to max |a| in [0.5, 1): by Weyl's bound that moves no eigenvalue by more than
+// 2^-80 of the largest entry, and it keeps the rounding noise around eigenvalues near 0 (rank-deficient input) from being rotated forever
+constexpr double DAB_EIG_ABS_FLOOR = 8.271806125530277e-25;
+
+// Rotation (c, s) that zeroes a_pq of J^T A J, J = [c s; -s c] in rows / columns (p, q): t = s / c is the smaller root of
+// t^2 + 2 zeta t - 1 = 0, zeta = (a_qq - a_pp) / (2 a_pq) (Golub & Van Loan, sym.schur2).  Returns false when a_pq counts as zero.
+__host__ __device__ inline bool slices_sym_rotation(double app, double aqq, double apq, double* c, double* s) {
+    const double g = fabs(apq);
+    if (!(g > DAB_EIG_TOL * sqrt(fabs(app)) * sqrt(fabs(aqq)) && g > DAB_EIG_ABS_FLOOR)) return false;
+    const double zeta = (aqq - app) / (2.0 * apq);
+    double t;
+    if (fabs(zeta) > 1e150) t = 0.5 / zeta;   // 1 + zeta^2 would overflow; t = 1 / (2 zeta) to working precision
+    else t = (zeta >= 0.0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
+    *c = 1.0 / sqrt(1.0 + t * t);
+    *s = *c * t;
+    return true;
+}
+
+// position of d[i] among d[0 .. n) in ascending order, ties by index (the eigenvalues are written at their rank)
+__host__ __device__ inline int slices_rank_asc(const double* d, int n, int i) {
+    const double v = d[i];
+    int rank = 0;
+    for (int j = 0; j < n; ++j) rank += d[j] < v || (d[j] == v && j < i);
+    return rank;
+}

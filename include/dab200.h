@@ -329,6 +329,26 @@ int32_t dab_sort_slices(dab_ctx* ctx, int32_t dtype, const void* in, void* out, 
  * wrapper rejects such input (chkfinite), so the host runtime raises ArgumentError once it has read status. */
 int32_t dab_svdvals_batched(dab_ctx* ctx, int32_t dtype, const void* A, size_t m, size_t n, size_t batch, void* S, int32_t* status);
 
+/* The slice functions of ppeval(f, D...; dim) (src/mapreduce.jl:210-323) that need a kernel of their own: the  _ppeval(f, localparts...)
+ * run on every worker (:315) once the slices are packed. */
+
+/* C_b = A_b * B_b for b < batch: A_b is m x k at A + b * strideA, B_b is k x n at B + b * strideB, C_b is m x n at C + b * m * n, all dense
+ * column-major; strides in elements, 0 broadcasts that operand to every b.  ppeval(*, A, B) with A_b, B_b the slices.  Float32 products
+ * accumulate in fp64 and are rounded once; Float64 accumulates with one DFMA per k, in k order; Int32 / Int64 wrap as Julia's generic
+ * matmul (Int32 results are Int32).  k == 0 writes zeros.  C must not overlap A or B.  dtypes F32 F64 I32 I64. */
+int32_t dab_matmul_batched(dab_ctx* ctx, int32_t dtype, size_t m, size_t n, size_t k, const void* A, size_t strideA, const void* B,
+                           size_t strideB, void* C, size_t batch);
+
+/* Largest n dab_eigvals_sym_batched serves (one 32 KiB fp64 matrix in shared memory). */
+#define DAB_EIGVALS_SYM_MAX_N 64
+/* W[b*n .. b*n + n) = eigvals(A_b), ascending, for the `batch` dense column-major n x n matrices A_b stored one after the other:
+ * ppeval(eigvals, D) / mapslices(eigvals, lp, dims=(d1, d2)) once the slices are packed.  Two-sided cyclic Jacobi in fp64 (Float32 input
+ * is rounded once at the end).  dtypes F32 F64; n <= DAB_EIGVALS_SYM_MAX_N, otherwise DAB_ERR_UNSUPPORTED.  status: a device int32 set
+ * to 0 by the call; the kernel ORs in 1 when a matrix holds a NaN or Inf and 2 when a finite matrix is not exactly symmetric
+ * (A[i,j] != A[j,i]); that matrix's values are then NaN.  Julia rejects non-finite input (ArgumentError) and takes a non-symmetric
+ * matrix to the general, complex eigenvalue problem, so the host runtime raises on either once it has read status. */
+int32_t dab_eigvals_sym_batched(dab_ctx* ctx, int32_t dtype, const void* A, size_t n, size_t batch, void* W, int32_t* status);
+
 /* ==== cross-worker combine: NCCL over NVLink (replaces Distributed.remotecall_fetch on
  *      this path only; src/mapreduce.jl:30-34, 72-80; src/darray.jl:809-815) ============== */
 /* 128-byte ncclUniqueId; rank 0 creates it, the host runtime ships it to the other workers. */

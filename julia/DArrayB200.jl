@@ -22,6 +22,7 @@
 #   src/sort.jl:8,22,61  sort(localpart(d)), sort!(lp)    Base.sort / Base.sort!                     dab_sort
 #   src/sort.jl:8,22,61  sort(localpart(d); by = f)       sort_by (keys = f.(a) by broadcast)        dab_sort_by_key
 #   src/mapreduce.jl:205 mapslices(f, localpart(y), dims) mapslices_sort / svdvals_batched       dab_sort_slices / dab_svdvals_batched
+#   src/mapreduce.jl:315 _ppeval(f, localparts...; dim)   matmul_batched / eigvals_sym_batched  dab_matmul_batched / dab_eigvals_sym_batched
 module DArrayB200
 
 using Distributed, DistributedArrays, LinearAlgebra
@@ -302,6 +303,28 @@ function svdvals_batched(a::B200Array{T,3}) where {T<:Union{Float32,Float64}}
                 ctx(), dab_dtype(T), a.ptr, m, n, batch, S.ptr, st.ptr), ctx())
     Array(st)[1] == 0 || throw(ArgumentError("matrix contains Infs or NaNs"))
     S
+end
+
+# _ppeval(f, localparts...; dim)  (src/mapreduce.jl:210-255) for f = * (slices already packed one after the other; a broadcast operand is
+# passed with stride 0) and f = eigvals of real symmetric slices (packed as `batch` column-major n x n matrices).  A slice that is not
+# exactly symmetric has complex eigenvalues in general: not served.
+function matmul_batched(A::B200Array{T}, sa::Int, B::B200Array{T}, sb::Int, m::Int, n::Int, k::Int, batch::Int) where {T}
+    C = B200Array{T,3}(undef, (m, n, batch))
+    check(ccall((:dab_matmul_batched, libdab), Int32,
+                (Ptr{Cvoid}, Int32, Csize_t, Csize_t, Csize_t, Ptr{Cvoid}, Csize_t, Ptr{Cvoid}, Csize_t, Ptr{Cvoid}, Csize_t),
+                ctx(), dab_dtype(T), m, n, k, A.ptr, sa, B.ptr, sb, C.ptr, batch), ctx())
+    C
+end
+function eigvals_sym_batched(a::B200Array{T,3}) where {T<:Union{Float32,Float64}}
+    n, n2, batch = size(a)
+    n == n2 || throw(DimensionMismatch("matrix is not square: dimensions are ($n, $n2)"))
+    W = B200Array{T,2}(undef, (n, batch)); st = B200Array{Int32,1}(undef, (1,))
+    check(ccall((:dab_eigvals_sym_batched, libdab), Int32, (Ptr{Cvoid}, Int32, Ptr{Cvoid}, Csize_t, Csize_t, Ptr{Cvoid}, Ptr{Cvoid}),
+                ctx(), dab_dtype(T), a.ptr, n, batch, W.ptr, st.ptr), ctx())
+    flags = Array(st)[1]
+    flags & 1 == 0 || throw(ArgumentError("matrix contains Infs or NaNs"))
+    flags & 2 == 0 || error("eigvals: a slice is not symmetric; complex eigenvalues are not served")
+    W
 end
 
 # localpart(A) * Bjk, transpose(localpart(A)) * Bjk inside _matmatmul!  (src/linalg.jl:218-226): K12, wgmma 3xTF32 for Float32
