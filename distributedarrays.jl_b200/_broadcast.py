@@ -29,7 +29,7 @@ from builtins import any as builtins_any
 from . import _lib
 from ._darray import B200Array, DArray, dab_dtype, darray, makelocal
 from .layout import shape_of
-from .runtime import runtime
+from .runtime import close_remote_reads, open_remote_reads, runtime
 
 # Julia-type tags and the promotion lattice
 _RANK = {"bool": 0, "i32": 1, "i64": 2, "i128": 3, "f32": 4, "f64": 5}
@@ -667,28 +667,25 @@ def _localise(rt, a, I, pid) -> LocalArg:
     return LocalArg(None, e.val, e.jt)
 
 
-def _prepare_remote_reads(dest_layout, rt, args):
-    """Collective: when a DArray argument's layout differs from the destination's, some rank will have to halo-fetch non-owned
-    data (makelocal's non-local branch, reference src/darray.jl:361-366).  Every rank takes the same decision from the layouts
-    alone, shares the CUDA-IPC handles and fences the producers' streams before the one-sided peer reads."""
-    if rt.world == 1:
-        return False
-    need = [a for a in args if isinstance(a, DArray) and not (a.layout.pids == dest_layout.pids and a.layout.indices == dest_layout.indices)]
-    for a in need:
-        if a._handles is None:
-            a.share()
-    if need:
-        rt.barrier()
-    return bool(need)
+def _remote_args(dest_layout, args) -> List[DArray]:
+    """The DArray arguments whose layout differs from the destination's: some rank will halo-fetch non-owned data of them
+    (makelocal's non-local branch, reference src/darray.jl:361-366).  Every rank takes the same decision from the layouts alone."""
+    return [a for a in args if isinstance(a, DArray) and not (a.layout.pids == dest_layout.pids and a.layout.indices == dest_layout.indices)]
 
 
-def _finish_remote_reads(rt, had_remote: bool):
-    """Collective counterpart of ``_prepare_remote_reads``: the owners of the chunks that were read one-sidedly may not overwrite
-    or free them before EVERY reader's copy kernel has finished (freed blocks go straight back to the allocator cache).  The
-    reference's ``remotecall_fetch`` is synchronous for the same reason.  Stream sync + host barrier, as copy_transposed / mul!."""
-    if had_remote:
-        rt.sync()
-        rt.barrier()
+def _broadcast_chunks(dest: DArray, expr: Expr, args) -> DArray:
+    """Every localpart of ``dest`` from ``bclocal`` of each argument (src/broadcast.jl:140-152) and one fused launch."""
+    rt = dest.rt
+    fenced = open_remote_reads(rt, _remote_args(dest.layout, args), "host")
+    for pid, out in dest.chunks.items():
+        I = dest.layout.localindices(pid)
+        largs = [_localise(rt, a, I, pid) for a in args]
+        run_local(rt, expr, out, largs)
+        for la in largs:
+            if la.temp and la.arr is not None:
+                la.arr.free()                                  # stream-ordered: the block is only reused by later launches
+    close_remote_reads(rt, fenced, "host")
+    return dest
 
 
 def _materialise_views(args):
@@ -724,17 +721,7 @@ def _broadcast_into(dest: DArray, f: Callable, *args) -> DArray:
             if s != 1 and s != want:
                 raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, f"destination axes {dest.dims} are not compatible with source axes {tuple(shp)}")
     expr = trace(f, [_arg_tag(a) for a in args])
-    rt = dest.rt
-    remote = _prepare_remote_reads(dest.layout, rt, args)
-    for pid, out in dest.chunks.items():
-        I = dest.layout.localindices(pid)
-        largs = [_localise(rt, a, I, pid) for a in args]
-        run_local(rt, expr, out, largs)
-        for la in largs:
-            if la.temp and la.arr is not None:
-                la.arr.free()                                  # stream-ordered: the block is only reused by later launches
-    _finish_remote_reads(rt, remote)
-    return dest
+    return _broadcast_chunks(dest, expr, args)
 
 
 def broadcast(f: Callable, *args, rt=None) -> DArray:
@@ -755,16 +742,7 @@ def _broadcast(f: Callable, *args, rt=None) -> DArray:
     expr = trace(f, [_arg_tag(a) for a in args])
     out_dt = _NPT[expr.jt]
     dest = darray(lambda I: B200Array.empty(rt, shape_of(I), out_dt), dims, dtype=out_dt, rt=rt)
-    remote = _prepare_remote_reads(dest.layout, rt, args)
-    for pid, out in dest.chunks.items():
-        I = dest.layout.localindices(pid)
-        largs = [_localise(rt, a, I, pid) for a in args]
-        run_local(rt, expr, out, largs)
-        for la in largs:
-            if la.temp and la.arr is not None:
-                la.arr.free()                                  # stream-ordered: the block is only reused by later launches
-    _finish_remote_reads(rt, remote)
-    return dest
+    return _broadcast_chunks(dest, expr, args)
 
 
 def copy(d: DArray) -> DArray:
@@ -805,7 +783,7 @@ def map_inplace(f: Callable, dest: DArray, src: DArray) -> DArray:
     ``map!(f, localpart(dest), makelocal(src, localindices(dest)...))``."""
     expr = trace(f, [tag_of(src.dtype)])
     rt = dest.rt
-    remote = _prepare_remote_reads(dest.layout, rt, [src])
+    fenced = open_remote_reads(rt, _remote_args(dest.layout, [src]), "host")
     for pid, out in dest.chunks.items():
         I = dest.layout.localindices(pid)
         arr = makelocal(src, I, pid)
@@ -813,7 +791,7 @@ def map_inplace(f: Callable, dest: DArray, src: DArray) -> DArray:
         run_local(rt, expr, out, [LocalArg(arr, None, tag_of(src.dtype))])
         if temp:
             arr.free()
-    _finish_remote_reads(rt, remote)
+    close_remote_reads(rt, fenced, "host")
     return dest
 
 
@@ -843,13 +821,4 @@ def map_localparts(f: Callable, A, B=None) -> DArray:
     out_dt = _NPT[expr.jt]
     from ._darray import darray_like
     dest = darray_like(lambda I: B200Array.empty(rt, shape_of(I), out_dt), lead, dtype=out_dt)
-    remote = _prepare_remote_reads(dest.layout, rt, args)
-    for pid, out in dest.chunks.items():
-        I = dest.layout.localindices(pid)
-        largs = [_localise(rt, a, I, pid) for a in args]
-        run_local(rt, expr, out, largs)
-        for la in largs:
-            if la.temp and la.arr is not None:
-                la.arr.free()                                  # stream-ordered: the block is only reused by later launches
-    _finish_remote_reads(rt, remote)
-    return dest
+    return _broadcast_chunks(dest, expr, args)

@@ -22,7 +22,7 @@ import numpy as np
 
 from . import _lib
 from .layout import Layout, Range, default_procs, layout_from_chunk_shapes, make_layout, rlen, shape_of, slab_plan
-from .runtime import Runtime, runtime
+from .runtime import Runtime, close_remote_reads, open_remote_reads, runtime
 
 _DT = {np.dtype(np.float32): _lib.F32, np.dtype(np.float64): _lib.F64, np.dtype(np.int32): _lib.I32,
        np.dtype(np.int64): _lib.I64, np.dtype(np.bool_): _lib.U8}   # UInt8 is NOT Bool: unserved eltypes raise (no silent reinterpretation)
@@ -157,7 +157,8 @@ _REGISTRY: Dict[Tuple[int, int], "weakref.ReferenceType[DArray]"] = {}
 
 def _release_chunks(chunks: Dict[int, "B200Array"], did):
     """``release_localpart`` (src/core.jl:77-82).  Frees are ordered on the ctx stream; every op that let OTHER ranks read these
-    chunks ended with a collective fence (``_finish_remote_reads``), so nobody is still reading when a finalizer runs."""
+    chunks ended with a collective fence (``runtime.close_remote_reads``, or the fence after an exchange's arena puts), so nobody
+    is still reading when a finalizer runs."""
     for ch in list(chunks.values()):
         try:
             ch.free()
@@ -467,11 +468,7 @@ class SubDArray:
         d = self.parent
         rt = d.rt
         shape = self.shape
-        remote = rt.world > 1
-        if remote:
-            if d._handles is None:
-                d.share()
-            rt.device_barrier()
+        fenced = open_remote_reads(rt, [d], "device")
 
         def init(I):
             ch = B200Array.empty(rt, shape_of(I), d.dtype)
@@ -483,8 +480,7 @@ class SubDArray:
         if len(shape) == 0:
             raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "DArray of a zero-dimensional view")
         out = darray(init, shape, procs=list(d.layout.pids), dtype=d.dtype, rt=rt)
-        if remote:
-            rt.device_barrier()
+        close_remote_reads(rt, fenced, "device")
         return out
 
     def to_numpy(self) -> np.ndarray:
@@ -781,11 +777,7 @@ def reshape(A: DArray, dims) -> DArray:
     if int(np.prod(dims, dtype=np.int64)) != A.size:
         raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, "dimensions must be consistent with array size")
     rt = A.rt
-    remote = rt.world > 1
-    if remote:
-        if A._handles is None:
-            A.share()
-        rt.device_barrier()
+    fenced = open_remote_reads(rt, [A], "device")
     strides = np.cumprod((1,) + dims[:-1]).astype(np.int64)
 
     def init(I):
@@ -800,8 +792,7 @@ def reshape(A: DArray, dims) -> DArray:
         return ch
 
     out = darray(init, dims, dtype=A.dtype, rt=rt)
-    if remote:
-        rt.device_barrier()
+    close_remote_reads(rt, fenced, "device")
     return out
 
 

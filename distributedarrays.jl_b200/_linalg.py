@@ -22,7 +22,7 @@ import numpy as np
 from . import _lib
 from ._darray import B200Array, DArray, SubDArray, dab_dtype, darray
 from .layout import make_layout, rlen, shape_of
-from .runtime import Runtime
+from .runtime import Runtime, close_remote_reads, exchange_stacks, fence, grouped_exchange, open_remote_reads
 
 _GEMV_DTYPES = (np.dtype(np.float32), np.dtype(np.float64), np.dtype(np.int32), np.dtype(np.int64))
 
@@ -71,10 +71,7 @@ def copy_transposed(W: Transpose) -> DArray:
     D = W.parent
     rt = D.rt
     R = darray(lambda I: B200Array.empty(rt, shape_of(I), D.dtype), W.dims, procs=list(D.layout.pids), dtype=D.dtype, rt=rt)
-    if rt.world > 1:
-        if D._handles is None:
-            D.share()
-        rt.barrier()
+    fenced = open_remote_reads(rt, [D], "host")
     es = D.dtype.itemsize
     from .layout import slab_plan
     for pid, out in R.chunks.items():
@@ -92,9 +89,7 @@ def copy_transposed(W: Transpose) -> DArray:
             # J-box element (r, c) -> out[c, r]
             dst = out.ptr + ((dc[0] - 1) + (dr[0] - 1) * dst_ld) * es
             _lib.call("dab_transpose_box", rt.ctx, es, C.c_void_p(dst), dst_ld, C.c_void_p(src), sshape[0], rows, cols)
-    if rt.world > 1:
-        rt.sync()
-        rt.barrier()                                       # owners may not free / overwrite D before every reader is done
+    close_remote_reads(rt, fenced, "host")
     return R
 
 
@@ -172,37 +167,15 @@ def mul_(y: DArray, A: Union[DArray, Transpose], x, alpha=1, beta=0) -> DArray:
     cuts_c = L.cuts[cd]
     isz, code = dt.itemsize, dab_dtype(dt)
     ypids = y.layout.pids
-    remote_x = isinstance(x, DArray) and rt.world > 1
-    if remote_x:
-        if x._handles is None:
-            x.share()                                      # once per DVector: the CUDA-IPC handles of its chunks
-        rt.device_barrier()                                # x's producers (on their own streams) are done before anybody reads it
+    remote_x = open_remote_reads(rt, [x] if isinstance(x, DArray) else [], "device")
 
     def tile_pid(i, j):                                    # procs(A)[i,j]  /  procs(A)[j,i]
         return L.pids[(j + i * g0) if trans else (i + j * g0)]
 
-    # ---- where the tile results are combined: per consumer rank, the stacks of its y chunks back to back (gj slots of plen each);
-    # every rank derives the same table, so a producer knows the slot of its tile inside the CONSUMER's arena bank
-    def stack_table(rank):
-        off, tab = 0, {}
-        for i in range(gi):
-            if rt.rank_of(ypids[i]) == rank:
-                tab[i] = off
-                off += (rlen(y.layout.indices[i][0]) * gj * isz + 255) & ~255
-        return tab, off
-
-    tables = {r: stack_table(r) for r in {rt.rank_of(p) for p in ypids}}
-    need = max(t[1] for t in tables.values())
-    use_arena = need <= rt.arena()["bank_bytes"] if rt.world > 1 else False
-    if use_arena:
-        bank = rt.arena_next_bank()
-        peers = rt.arena()["peers"]
-        my_base = peers[rt.rank] + bank
-        my_tab = tables.get(rt.rank, ({}, 0))[0]
-    else:                                                  # one rank (or stacks too large for the arena): private stacks + NCCL send/recv
-        my_tab, my_bytes = stack_table(rt.rank)
-        my_stack = B200Array.empty(rt, (max(my_bytes, 16),), np.uint8, temp=True)
-        my_base = my_stack.ptr
+    # ---- where the tile results are combined: on the owner of y's chunk i, a stack of gj slots of plen each
+    st = exchange_stacks(rt, [rt.rank_of(p) for p in ypids], [rlen(ix[0]) * gj * isz for ix in y.layout.indices])
+    my_tab = st.tables[rt.rank]
+    peers = rt.arena()["peers"] if st.use_arena else None
 
     # ---- R[i,j] = localpart(A) * xj on the tile owners (src/linalg.jl:90-98); a tile whose consumer is this rank is written straight
     # into its slot of the stack
@@ -220,47 +193,40 @@ def mul_(y: DArray, A: Union[DArray, Transpose], x, alpha=1, beta=0) -> DArray:
             plen = ch.shape[rd]
             orank = rt.rank_of(ypids[i])
             if orank == rt.rank:
-                rptr = my_base + my_tab[i] + j * plen * isz
+                rptr = st.base + my_tab[i] + j * plen * isz
             else:
                 r = B200Array.empty(rt, (plen,), dt, temp=True)
                 temps.append(r)
                 rptr = r.ptr
-                if use_arena:
-                    puts.append((peers[orank] + bank + tables[orank][0][i] + j * plen * isz, rptr, plen * isz))
+                if st.use_arena:
+                    puts.append((peers[orank] + st.bank + st.tables[orank][i] + j * plen * isz, rptr, plen * isz))
                 else:
                     sends[(i, j)] = rptr
             _lib.call("dab_gemv", rt.ctx, code, 1 if trans else 0, C.c_void_p(ch.ptr), ch.shape[0], ch.shape[1], C.c_void_p(xblocks[j].ptr),
                       C.c_void_p(rptr))
     # ---- ship the tile results to the owner of y's chunk i (the fetch(rij) of :113-115)
-    if use_arena:
+    if st.use_arena:
         for dst, src, nb in puts:                          # one-sided puts over NVLink into the consumer's arena bank
             if nb:
                 _lib.call("dab_d2d", rt.ctx, C.c_void_p(dst), C.c_void_p(src), nb)
-        rt.device_barrier()                                # every producer's puts have landed; also: every reader of x is done with it
+        fence(rt, "device")                                # every producer's puts have landed; also: every reader of x is done with it
     elif rt.world > 1:
         plan = matvec_exchange_plan(L, y.layout, trans, rt.rank_of, rt.rank)   # same (i, j) order on both sides of every pair
         sends = [(sends[(i, j)], plen * isz, peer) for i, j, plen, peer in plan["sends"] if plen]
-        recvs = [(my_base + my_tab[i] + j * plen * isz, plen * isz, peer) for i, j, plen, peer in plan["recvs"] if plen]
-        if sends or recvs:
-            _lib.call("dab_group_start", rt.ctx)
-            for ptr, nb, peer in sends:
-                _lib.call("dab_send", rt.ctx, C.c_void_p(ptr), nb, peer)
-            for ptr, nb, peer in recvs:
-                _lib.call("dab_recv", rt.ctx, C.c_void_p(ptr), nb, peer)
-            _lib.call("dab_group_end", rt.ctx)
+        recvs = [(st.base + my_tab[i] + j * plen * isz, plen * isz, peer) for i, j, plen, peer in plan["recvs"] if plen]
+        grouped_exchange(rt, sends, recvs)
     # ---- scale y (:101-111), then add!(localpart(y), R[i,j], α) for each j (:114-117; j order) -- one fused launch per y chunk
     a_s, b_s = np.asarray(alpha, dtype=dt), np.asarray(beta, dtype=dt)
     for i, off in my_tab.items():
         ych = y.chunks[ypids[i]]
         if ych.size:
             _lib.call("dab_accumulate_stack", rt.ctx, code, C.c_void_p(ych.ptr), ych.size, C.c_void_p(b_s.ctypes.data), C.c_void_p(a_s.ctypes.data),
-                      C.c_void_p(my_base + off), ych.size, gj)
+                      C.c_void_p(st.base + off), ych.size, gj)
     for t in temps + list(xblocks.values()):
         t.free()
-    if not use_arena:
-        my_stack.free()
-        if remote_x:
-            rt.device_barrier()                            # owners may not overwrite x before every reader's fetch has run
+    if not st.use_arena:                                   # with the arena, the fence after the puts closed the reads of x
+        rt.free_temp(st.temp)
+        close_remote_reads(rt, remote_x, "device")
     return y
 
 
@@ -366,11 +332,7 @@ def mul_mat_(Cd: DArray, A: Union[DArray, Transpose], B, alpha=1, beta=0) -> DAr
     c0, gk = CL.grid
     cuts_c, cuts_k = L.cuts[cd], CL.cuts[1]
     code, isz = dab_dtype(dt), dt.itemsize
-    remote_b = isinstance(B, DArray) and rt.world > 1
-    if remote_b:
-        if B._handles is None:
-            B.share()
-        rt.barrier()
+    remote_b = open_remote_reads(rt, [B] if isinstance(B, DArray) else [], "host")
 
     def tile_pid(i, j):
         return L.pids[(j + i * g0) if trans else (i + j * g0)]
@@ -406,13 +368,7 @@ def mul_mat_(Cd: DArray, A: Union[DArray, Transpose], B, alpha=1, beta=0) -> DAr
             _lib.call("dab_d2d", rt.ctx, C.c_void_p(stacks[(i, k)].ptr + j * rows * cols * isz), C.c_void_p(R[(i, j, k)].ptr), rows * cols * isz)
     sends = [(R[(i, j, k)].ptr, rows * cols * isz, peer) for i, j, k, rows, cols, peer in plan["sends"] if rows * cols]
     recvs = [(stacks[(i, k)].ptr + j * rows * cols * isz, rows * cols * isz, peer) for i, j, k, rows, cols, peer in plan["recvs"] if rows * cols]
-    if sends or recvs:
-        _lib.call("dab_group_start", rt.ctx)
-        for ptr, nb, peer in sends:
-            _lib.call("dab_send", rt.ctx, C.c_void_p(ptr), nb, peer)
-        for ptr, nb, peer in recvs:
-            _lib.call("dab_recv", rt.ctx, C.c_void_p(ptr), nb, peer)
-        _lib.call("dab_group_end", rt.ctx)
+    grouped_exchange(rt, sends, recvs)
     # ---- scale C (:232-240), then add!(localpart(C), R[i,j,k], α) for each j (:243-252; j order)
     a_s, b_s = np.asarray(alpha, dtype=dt), np.asarray(beta, dtype=dt)
     for (i, k), stack in stacks.items():
@@ -433,9 +389,7 @@ def mul_mat_(Cd: DArray, A: Union[DArray, Transpose], B, alpha=1, beta=0) -> DAr
             _lib.call("dab_binary", rt.ctx, code, _lib.ADD, C.c_void_p(cch.ptr), C.c_void_p(cch.ptr), C.c_void_p(rp), nel)
     for t in list(R.values()) + temps + list(stacks.values()):
         t.free()
-    if remote_b:
-        rt.sync()
-        rt.barrier()
+    close_remote_reads(rt, remote_b, "host")
     return Cd
 
 

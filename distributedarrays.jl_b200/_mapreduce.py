@@ -23,6 +23,7 @@ from . import _lib
 from ._broadcast import Expr, broadcast, tag_of, trace, _NPT
 from ._darray import B200Array, DArray, dab_dtype, np_dtype
 from .layout import Layout, collapse_for_region, ravel, shape_of, unravel
+from .runtime import close_remote_reads, exchange_stacks, fence, grouped_exchange, open_remote_reads
 
 _OPS = {"+": _lib.SUM, "add": _lib.SUM, "sum": _lib.SUM, "*": _lib.PROD, "mul": _lib.PROD, "prod": _lib.PROD, "max": _lib.MAX,
         "min": _lib.MIN}
@@ -160,7 +161,7 @@ def _empty_slot(rt, opc: int, rdt: np.dtype, slot_ptr: int):
 def _mapreduce_expr(expr: Expr, opc: int, d: DArray, others: Sequence, return_partials: bool = False):
     """General ``mapreduce(f, op, d, others...)``: f is an arbitrary traced expression over 1..8 arguments.  ONE fused NVRTC
     kernel per localpart (``dab_mapreduce_expr``), no temporary f.(d) array; combine as in ``_mapreduce_all``."""
-    from ._broadcast import _NPT as NPT, _localise, _prepare_remote_reads, codegen
+    from ._broadcast import _NPT as NPT, _localise, _remote_args, codegen
     rt = d.rt
     args = [d] + list(others)
     for a in others:
@@ -185,8 +186,7 @@ def _mapreduce_expr(expr: Expr, opc: int, d: DArray, others: Sequence, return_pa
     else:
         rdt = np.dtype(np.int64) if val_tag in ("bool", "i32", "i64") and opc in (_lib.SUM, _lib.PROD, _lib.ALL, _lib.ANY, _lib.COUNT) else NPT[val_tag]
     src = codegen(expr).encode()
-    from ._broadcast import _finish_remote_reads
-    remote = _prepare_remote_reads(d.layout, rt, [a for a in others if isinstance(a, DArray)])
+    fenced = open_remote_reads(rt, _remote_args(d.layout, others), "host")
     temps = []
 
     def launch(pid, ch, slot_ptr):
@@ -210,7 +210,7 @@ def _mapreduce_expr(expr: Expr, opc: int, d: DArray, others: Sequence, return_pa
     finally:
         for t in temps:
             t.free()
-        _finish_remote_reads(rt, remote)
+        close_remote_reads(rt, fenced, "host")
     if wide:
         vals = [_int128(host[16 * (pid - 1):16 * pid].tobytes()) for pid in d.layout.pids]
         res = fold128(vals, opc)
@@ -546,50 +546,28 @@ def mapreducedim(f: Optional[Callable], op, d: DArray, dims, init=None) -> DArra
         # launch, no host sync); slabs too large for the arena, or DAB_FUSED_COMBINE=0, take the grouped ncclSend/ncclRecv path.
         Rchunks: Dict[int, B200Array] = {}
         isz = rdt.itemsize
-
-        def stack_table(rank):
-            off, tab = 0, {}
-            for rl, members in enumerate(fibres):
-                if rt.rank_of(Rpids[rl]) == rank:
-                    plen = int(np.prod(shape_of(Rindices[rl])))
-                    tab[rl] = (off, plen, len(members))
-                    off += (plen * len(members) * isz + 255) & ~255
-            return tab, off
-
-        tables = {r: stack_table(r) for r in {rt.rank_of(p) for p in Rpids}}
-        use_arena = rt.world > 1 and max(t[1] for t in tables.values()) <= rt.arena()["bank_bytes"]
-        my_tab, my_bytes = tables.get(rt.rank, ({}, 0))
-        priv = None
-        if use_arena:
-            bank = rt.arena_next_bank()
-            peers = rt.arena()["peers"]
-            my_base = peers[rt.rank] + bank
-        else:
-            priv = B200Array.empty(rt, (max(my_bytes, 16),), np.uint8, temp=True)
-            my_base = priv.ptr
+        plens = [int(np.prod(shape_of(ix))) for ix in Rindices]
+        st = exchange_stacks(rt, [rt.rank_of(p) for p in Rpids], [plen * len(members) * isz for plen, members in zip(plens, fibres)])
+        my_tab = st.tables[rt.rank]
         xp = exchange_plan(L, Rlayout, fibres, rt.rank_of, rt.rank)
         for rl, slot, mp in xp["local"]:
-            off, plen, _ = my_tab[rl]
+            plen = plens[rl]
             if plen:
-                _lib.call("dab_d2d", rt.ctx, C.c_void_p(my_base + off + slot * plen * isz), C.c_void_p(partial[mp].ptr), plen * isz)
-        if use_arena:
+                _lib.call("dab_d2d", rt.ctx, C.c_void_p(st.base + my_tab[rl] + slot * plen * isz), C.c_void_p(partial[mp].ptr), plen * isz)
+        if st.use_arena:
+            peers = rt.arena()["peers"]
             for mp, peer, rl in xp["sends"]:
-                off, plen, _ = tables[peer][0][rl]
+                plen = plens[rl]
                 slot = fibres[rl].index(L.pids.index(mp))
                 if plen:
-                    _lib.call("dab_d2d", rt.ctx, C.c_void_p(peers[peer] + bank + off + slot * plen * isz), C.c_void_p(partial[mp].ptr), plen * isz)
-            rt.device_barrier()
+                    _lib.call("dab_d2d", rt.ctx, C.c_void_p(peers[peer] + st.bank + st.tables[peer][rl] + slot * plen * isz), C.c_void_p(partial[mp].ptr),
+                              plen * isz)
+            fence(rt, "device")                                    # every producer's puts have landed
         else:
             sends = [(partial[mp].ptr, partial[mp].size * isz, peer) for mp, peer, _ in xp["sends"]]
-            recvs = [(my_base + my_tab[rl][0] + slot * my_tab[rl][1] * isz, my_tab[rl][1] * isz, peer) for rl, slot, _, peer in xp["recvs"]]
-            if sends or recvs:
-                _lib.call("dab_group_start", rt.ctx)
-                for ptr, nb, peer in sends:
-                    _lib.call("dab_send", rt.ctx, C.c_void_p(ptr), nb, peer)
-                for ptr, nb, peer in recvs:
-                    _lib.call("dab_recv", rt.ctx, C.c_void_p(ptr), nb, peer)
-                _lib.call("dab_group_end", rt.ctx)
-        for rl, (off, plen, nm) in my_tab.items():
+            recvs = [(st.base + my_tab[rl] + slot * plens[rl] * isz, plens[rl] * isz, peer) for rl, slot, _, peer in xp["recvs"]]
+            grouped_exchange(rt, sends, recvs)
+        for rl, off in my_tab.items():
             owner = Rpids[rl]
             Rch = B200Array.empty(rt, shape_of(Rindices[rl]), rdt)
             acc = 0
@@ -598,11 +576,11 @@ def mapreducedim(f: Optional[Callable], op, d: DArray, dims, init=None) -> DArra
                 _lib.call("dab_fill", rt.ctx, dab_dtype(rdt) if rdt != np.dtype(np.int64) else _lib.I64, C.c_void_p(Rch.ptr), Rch.size,
                           C.c_void_p(v.ctypes.data))
                 acc = 1
-            # Base.mapreducedim!(identity, op, localpart(R), Bfull): accumulate the nm partial slabs, in grid order, onto R
-            _lib.call("dab_reducedim", rt.ctx, dab_dtype(rdt), opc, _lib.MAP_ID, C.c_void_p(my_base + off), plen, nm, 1, C.c_void_p(Rch.ptr), acc)
+            # Base.mapreducedim!(identity, op, localpart(R), Bfull): accumulate the partial slabs of the fibre, in grid order, onto R
+            _lib.call("dab_reducedim", rt.ctx, dab_dtype(rdt), opc, _lib.MAP_ID, C.c_void_p(st.base + off), plens[rl], len(fibres[rl]), 1,
+                      C.c_void_p(Rch.ptr), acc)
             Rchunks[owner] = Rch
-        if priv is not None:
-            priv.free()
+        rt.free_temp(st.temp)
         for p in partial.values():
             p.free()
         return DArray(Rlayout, rdt, Rchunks, rt)

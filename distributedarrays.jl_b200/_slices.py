@@ -35,6 +35,7 @@ from . import _lib
 from ._broadcast import _NPT, SLICE_TRACING, Expr, LocalArg, convert, run_local, tag_of
 from ._darray import B200Array, DArray, SubDArray, darray, dab_dtype
 from .layout import Layout, defaultdist, layout_from_chunk_shapes, make_layout, rlen, shape_of
+from .runtime import close_remote_reads, open_remote_reads
 
 _SORT_DTYPES = (np.dtype(np.float32), np.dtype(np.float64), np.dtype(np.int32), np.dtype(np.int64))
 
@@ -398,11 +399,7 @@ def run_chunk(rt, plan: _Plan, ch: B200Array, out: B200Array, status_ptr: int, c
 def _redistribute(D: DArray, p) -> DArray:
     """``DArray(size(D), procs(D), p) do I; D[I...] end`` (src/mapreduce.jl:200-202): every new chunk is one halo read."""
     rt = D.rt
-    remote = rt.world > 1
-    if remote:
-        if D._handles is None:
-            D.share()
-        rt.device_barrier()
+    fenced = open_remote_reads(rt, [D], "device")
 
     def init(I):
         ch = B200Array.empty(rt, shape_of(I), D.dtype)
@@ -411,8 +408,7 @@ def _redistribute(D: DArray, p) -> DArray:
         return ch
 
     DD = darray(init, D.dims, list(D.layout.pids), p, dtype=D.dtype, rt=rt)
-    if remote:
-        rt.device_barrier()
+    close_remote_reads(rt, fenced, "device")
     return DD
 
 

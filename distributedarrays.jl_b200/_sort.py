@@ -30,6 +30,7 @@ import numpy as np
 from . import _lib
 from ._darray import B200Array, DArray, dab_dtype
 from .layout import layout_from_chunk_shapes
+from .runtime import grouped_exchange
 
 _SORT_DTYPES = (np.dtype(np.float32), np.dtype(np.float64), np.dtype(np.int32), np.dtype(np.int64))
 SAMPLE_SIZE_ON_WORKER = 512                                    # src/sort.jl:69
@@ -316,13 +317,7 @@ def sort_with_boundaries(d: DArray, sample=True, by=None, alg=None, **kwargs):
         _lib.call("dab_d2d", rt.ctx, C.c_void_p(recv[j].ptr + off * isz), C.c_void_p(srt[p].ptr + (ends[p][j] - n) * isz), n * isz)
     sends = [(srt[p].ptr + (ends[p][j] - n) * isz, n * isz, peer) for j, p, n, peer in plan["sends"]]
     recvs = [(recv[j].ptr + off * isz, n * isz, peer) for j, p, off, n, peer in plan["recvs"]]
-    if sends or recvs:
-        _lib.call("dab_group_start", rt.ctx)
-        for ptr, nb, peer in sends:
-            _lib.call("dab_send", rt.ctx, C.c_void_p(ptr), nb, peer)
-        for ptr, nb, peer in recvs:
-            _lib.call("dab_recv", rt.ctx, C.c_void_p(ptr), nb, peer)
-        _lib.call("dab_group_end", rt.ctx)
+    grouped_exchange(rt, sends, recvs)
     for s in srt.values():
         s.free()
 

@@ -13,7 +13,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import List, Optional
+from typing import Dict, List, NamedTuple, Optional, Sequence
 
 import numpy as np
 
@@ -279,6 +279,85 @@ class Runtime:
             self.dist = None
         if _RT is self:
             _RT = None
+
+
+# ---- how a rank reads from or ships to its peers ------------------------------------------------------------------------------
+# Every operation with a cross-rank step goes through these helpers.  They take the runtime as an argument, so that a test can
+# drive them with a stand-in.  All of them are collective: every rank calls them in the same order with arguments derived from
+# the layouts alone.  DESIGN.md §5 lists which operations use which fence kind.
+
+
+def fence(rt, kind: str):
+    """``"host"``: ``barrier`` (stream sync + host barrier).  ``"device"``: ``device_barrier`` (stream-ordered, no host sync)."""
+    if kind == "host":
+        rt.barrier()
+    elif kind == "device":
+        rt.device_barrier()
+    else:
+        raise ValueError(f"fence kind {kind!r}: expected 'host' or 'device'")
+
+
+def open_remote_reads(rt, arrays: Sequence, kind: str) -> bool:
+    """Opening half of a one-sided read of other ranks' chunks of the DArrays ``arrays``: shares the CUDA-IPC handles not
+    shared yet and fences the producers, so that every earlier write to those chunks has landed before a peer reads them.
+    Nothing happens on one rank or for an empty list.  Returns whether it fenced; pass that to ``close_remote_reads``."""
+    if rt.world == 1 or not arrays:
+        return False
+    for a in arrays:
+        if a._handles is None:
+            a.share()
+    fence(rt, kind)
+    return True
+
+
+def close_remote_reads(rt, fenced: bool, kind: str):
+    """Closing half of ``open_remote_reads``, with the same fence kind: the owners of the chunks that were read may not
+    overwrite or free them before every reader's copy has run (freed blocks go straight back to the allocator cache).  The
+    reference's ``remotecall_fetch`` is synchronous for the same reason."""
+    if fenced:
+        if kind == "host":
+            rt.sync()
+        fence(rt, kind)
+
+
+def grouped_exchange(rt, sends: Sequence, recvs: Sequence):
+    """One grouped NCCL point-to-point exchange of ``(device pointer, bytes, peer rank)`` transfers: every send in list order,
+    then every receive in list order.  NCCL matches the grouped calls between two ranks in the order they are issued, so both
+    sides must list a pair's transfers in the same order (the exchange plans do).  Two empty lists issue nothing."""
+    if not sends and not recvs:
+        return
+    _lib.call("dab_group_start", rt.ctx)
+    for ptr, nb, peer in sends:
+        _lib.call("dab_send", rt.ctx, C.c_void_p(ptr), nb, peer)
+    for ptr, nb, peer in recvs:
+        _lib.call("dab_recv", rt.ctx, C.c_void_p(ptr), nb, peer)
+    _lib.call("dab_group_end", rt.ctx)
+
+
+class Stacks(NamedTuple):
+    tables: Dict[int, Dict[int, int]]  # rank -> {result chunk: byte offset of its stack}, for every rank
+    use_arena: bool
+    bank: int                          # byte offset of the arena bank of this exchange (0 without the arena)
+    base: int                          # device address of this rank's stacks
+    temp: int                          # the private stack buffer the caller frees with ``free_temp`` (0 with the arena)
+
+
+def exchange_stacks(rt, owners: Sequence[int], nbytes: Sequence[int]) -> Stacks:
+    """Where the consumers of an exchange collect what they receive: one stack per result chunk ``c``, of ``nbytes[c]`` bytes
+    rounded up to 256, on rank ``owners[c]``; each rank's stacks lie back to back in chunk order.  Every rank derives the same
+    tables, so a producer knows the offset of a stack inside its consumer's buffer.  With several ranks, and every rank's
+    stacks fitting one bank, the stacks sit in the exchange arena and producers put into ``arena()["peers"][r] + bank +
+    offset``.  Otherwise they sit in a private temporary and arrive by ``grouped_exchange``."""
+    tables: Dict[int, Dict[int, int]] = {r: {} for r in range(rt.world)}
+    totals = [0] * rt.world
+    for c, (r, nb) in enumerate(zip(owners, nbytes)):
+        tables[r][c] = totals[r]
+        totals[r] += (nb + 255) & ~255
+    if rt.world > 1 and max(totals) <= rt.arena()["bank_bytes"]:
+        bank = rt.arena_next_bank()
+        return Stacks(tables, True, bank, rt.arena()["peers"][rt.rank] + bank, 0)
+    temp = rt.alloc_temp(max(totals[rt.rank], 16))
+    return Stacks(tables, False, 0, temp, temp)
 
 
 def init(workers_per_rank: int = 1, device: Optional[int] = None, use_dist: Optional[bool] = None) -> Runtime:
