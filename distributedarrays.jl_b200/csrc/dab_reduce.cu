@@ -5,7 +5,8 @@
 //
 // Roofline: HBM, 4 B/element read (sizeof(T)), output negligible.
 // Design: flat grid, one CTA of 256 threads per 32 KiB of input; each thread keeps UNROLL independent 16-byte evict-first loads
-// in flight, reduces the 16 values of a tile step with a register tree in the element type, and carries the running
+// in flight, reduces the 16 values of a tile step with a register tree in the element type (Int32 sums and products instead fold
+// each value, widened to Int64, straight into the accumulator), and carries the running
 // value in a wide accumulator (fp64 for float sums/products, int64 for integers) -- one F2D + DADD per 16 elements, so the
 // FP64 pipe is idle >90 % of the time and the result is far inside the 1e-6 tolerance.  Warp shuffle -> shared-memory
 // tree -> one partial per CTA -> the LAST CTA to finish (ticket counter) folds the CTA partials in a fixed order, so the
@@ -59,7 +60,7 @@ __global__ void __launch_bounds__(RD_THREADS, 8) reduce_kernel(const T* __restri
                                                              void* out, int finalize_mode, long long n_for_all, int tiles_per_cta,
                                                              FusedComm fc, St st) {
     using A = typename R::A;
-    using V = typename Map::V;
+    using W = typename R::W;
     constexpr int VPT = 16 / sizeof(T);
     __shared__ A smem[RD_THREADS / 32];
     __shared__ bool is_last;
@@ -80,37 +81,47 @@ __global__ void __launch_bounds__(RD_THREADS, 8) reduce_kernel(const T* __restri
         int4 r[RD_UNROLL];
 #pragma unroll
         for (int u = 0; u < RD_UNROLL; ++u) r[u] = ld_stream(xv + base + (size_t)u * RD_THREADS);
-        V tv[RD_UNROLL];
+        if constexpr (std::is_same<W, typename Map::V>::value) {
+            W tv[RD_UNROLL];
 #pragma unroll
-        for (int u = 0; u < RD_UNROLL; ++u) {
-            Pack<T> p = as_pack<T>(r[u]);
-            st.vec(p, base + (size_t)u * RD_THREADS);
-            V m[VPT];
+            for (int u = 0; u < RD_UNROLL; ++u) {
+                Pack<T> p = as_pack<T>(r[u]);
+                st.vec(p, base + (size_t)u * RD_THREADS);
+                W m[VPT];
 #pragma unroll
-            for (int k = 0; k < VPT; ++k) m[k] = map(p.v[k]);
+                for (int k = 0; k < VPT; ++k) m[k] = map(p.v[k]);
 #pragma unroll
-            for (int w = VPT; w > 1; w >>= 1)  // register tree inside one 16-byte vector
+                for (int w = VPT; w > 1; w >>= 1)  // register tree inside one 16-byte vector
 #pragma unroll
-                for (int k = 0; k < w / 2; ++k) m[k] = R::tile(m[k], m[k + w / 2]);
-            tv[u] = m[0];
+                    for (int k = 0; k < w / 2; ++k) m[k] = R::tile(m[k], m[k + w / 2]);
+                tv[u] = m[0];
+            }
+#pragma unroll
+            for (int w = RD_UNROLL; w > 1; w >>= 1)
+#pragma unroll
+                for (int k = 0; k < w / 2; ++k) tv[k] = R::tile(tv[k], tv[k + w / 2]);
+            acc = R::comb(acc, R::lift(tv[0]));
+        } else {  // widened tile (Int32 sums and products)
+#pragma unroll
+            for (int u = 0; u < RD_UNROLL; ++u) {
+                Pack<T> p = as_pack<T>(r[u]);
+                st.vec(p, base + (size_t)u * RD_THREADS);
+                acc = fold_into<R>(acc, p, map);
+            }
         }
-#pragma unroll
-        for (int w = RD_UNROLL; w > 1; w >>= 1)
-#pragma unroll
-            for (int k = 0; k < w / 2; ++k) tv[k] = R::tile(tv[k], tv[k + w / 2]);
-        acc = R::comb(acc, R::lift(tv[0]));
     }
     if (blockIdx.x == gridDim.x - 1) {  // remainder vectors, unaligned head, tail
         for (size_t i = ntiles * TILE + threadIdx.x; i < nvec; i += RD_THREADS) {
             Pack<T> p = as_pack<T>(ld_stream(xv + i));
             st.vec(p, i);
-            V m = map(p.v[0]);
+            W m = R::pre(map(p.v[0]));
 #pragma unroll
-            for (int k = 1; k < VPT; ++k) m = R::tile(m, map(p.v[k]));
+            for (int k = 1; k < VPT; ++k) m = R::tile(m, R::pre(map(p.v[k])));
             acc = R::comb(acc, R::lift(m));
         }
-        for (size_t i = threadIdx.x; i < head; i += RD_THREADS) acc = R::comb(acc, R::lift(map(st.scalar(x[i], i))));
-        for (size_t i = head + nvec * VPT + threadIdx.x; i < n; i += RD_THREADS) acc = R::comb(acc, R::lift(map(st.scalar(x[i], i))));
+        for (size_t i = threadIdx.x; i < head; i += RD_THREADS) acc = R::comb(acc, R::lift(R::pre(map(st.scalar(x[i], i)))));
+        for (size_t i = head + nvec * VPT + threadIdx.x; i < n; i += RD_THREADS)
+            acc = R::comb(acc, R::lift(R::pre(map(st.scalar(x[i], i)))));
     }
     acc = block_reduce<R>(acc, smem);
     // ---- two-level "last one out" combine: deterministic, no second launch, tail latency of a few microseconds.

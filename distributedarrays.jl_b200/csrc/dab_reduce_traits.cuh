@@ -9,23 +9,33 @@ namespace {
 constexpr int RD_THREADS = 256;
 
 // ---------------------------------------------------------------------------------------------------------------
-// Reduce "traits": V = value type after the map, A = accumulator carried across tiles / threads / CTAs.
-//   lift(V) -> A, comb(A, A) -> A (associative up to rounding), tile(V, V) -> V combine inside a tile step.
+// Reduce "traits": V = value type after the map, W = value type inside a tile step, A = accumulator carried across tiles /
+// threads / CTAs.
+//   pre(V) -> W right after the map, tile(W, W) -> W combine inside a tile step, lift(W) -> A, comb(A, A) -> A (associative up
+//   to rounding).
+// W is V except for Int32 sums and products, which widen to Int64 before the first add or multiply (Base.add_sum /
+// Base.mul_prod): a tile of 16 Int32 values would otherwise wrap at 32 bits before it reaches the Int64 accumulator.
 // ---------------------------------------------------------------------------------------------------------------
+template <typename V>
+using WideInt32 = typename std::conditional<std::is_same<V, int32_t>::value, long long, V>::type;
 template <typename V>
 struct SumTraits {
     using A = typename std::conditional<std::is_floating_point<V>::value, double, long long>::type;
+    using W = WideInt32<V>;
     __device__ static __forceinline__ A identity() { return (A)0; }
-    __device__ static __forceinline__ V tile(V a, V b) { return jl::add(a, b); }
-    __device__ static __forceinline__ A lift(V v) { return (A)v; }
+    __device__ static __forceinline__ W pre(V v) { return (W)v; }
+    __device__ static __forceinline__ W tile(W a, W b) { return jl::add(a, b); }
+    __device__ static __forceinline__ A lift(W v) { return (A)v; }
     __device__ static __forceinline__ A comb(A a, A b) { return jl::add(a, b); }
 };
 template <typename V>
 struct ProdTraits {
     using A = typename std::conditional<std::is_floating_point<V>::value, double, long long>::type;
+    using W = WideInt32<V>;
     __device__ static __forceinline__ A identity() { return (A)1; }
-    __device__ static __forceinline__ V tile(V a, V b) { return jl::mul(a, b); }
-    __device__ static __forceinline__ A lift(V v) { return (A)v; }
+    __device__ static __forceinline__ W pre(V v) { return (W)v; }
+    __device__ static __forceinline__ W tile(W a, W b) { return jl::mul(a, b); }
+    __device__ static __forceinline__ A lift(W v) { return (A)v; }
     __device__ static __forceinline__ A comb(A a, A b) { return jl::mul(a, b); }
 };
 template <typename V>
@@ -47,7 +57,9 @@ __device__ __forceinline__ V highest_of() {
 template <typename V>
 struct MaxTraits {  // Julia max: NaN-propagating, +0.0 > -0.0; -Inf is a true identity under those rules
     using A = V;
+    using W = V;
     __device__ static __forceinline__ A identity() { return lowest_of<V>(); }
+    __device__ static __forceinline__ W pre(V v) { return v; }
     __device__ static __forceinline__ V tile(V a, V b) { return jl::max(a, b); }
     __device__ static __forceinline__ A lift(V v) { return v; }
     __device__ static __forceinline__ A comb(A a, A b) { return jl::max(a, b); }
@@ -55,7 +67,9 @@ struct MaxTraits {  // Julia max: NaN-propagating, +0.0 > -0.0; -Inf is a true i
 template <typename V>
 struct MinTraits {
     using A = V;
+    using W = V;
     __device__ static __forceinline__ A identity() { return highest_of<V>(); }
+    __device__ static __forceinline__ W pre(V v) { return v; }
     __device__ static __forceinline__ V tile(V a, V b) { return jl::min(a, b); }
     __device__ static __forceinline__ A lift(V v) { return v; }
     __device__ static __forceinline__ A comb(A a, A b) { return jl::min(a, b); }
@@ -68,7 +82,9 @@ struct Pair {
 template <typename T>
 struct ExtremaTraits {
     using A = Pair<T>;
+    using W = Pair<T>;
     __device__ static __forceinline__ A identity() { return A{highest_of<T>(), lowest_of<T>()}; }
+    __device__ static __forceinline__ W pre(W v) { return v; }
     __device__ static __forceinline__ A tile(A a, A b) { return A{jl::min(a.lo, b.lo), jl::max(a.hi, b.hi)}; }
     __device__ static __forceinline__ A lift(A v) { return v; }
     __device__ static __forceinline__ A comb(A a, A b) { return tile(a, b); }
@@ -81,13 +97,24 @@ struct ExtMapF {
 };
 struct CountTraits {  // V = int (0/1) ; all / any / count all reduce to "number of trues"
     using A = long long;
+    using W = int;
     __device__ static __forceinline__ A identity() { return 0; }
+    __device__ static __forceinline__ W pre(int v) { return v; }
     __device__ static __forceinline__ int tile(int a, int b) { return a + b; }
     __device__ static __forceinline__ A lift(int v) { return (A)v; }
     __device__ static __forceinline__ A comb(A a, A b) { return a + b; }
 };
 
 // ---- map functors: T -> V -----------------------------------------------------------------------
+// Int32 -x for the reduce kernels: the same bits as jl::neg, written as a 64-bit negate truncated to 32 bits.  Given jl::neg, ptxas
+// (CUDA 12.9, sm_90a) folds the 32-bit negations into the operands of a three-input VIMNMX3 and drops one of them, so that
+// maximum(-, d) of Int32 picked the wrong element; it leaves this form alone.  That is how this ptxas schedules it, not a guarantee:
+// tests/test_gpu_reduce_exact.py runs Int32 max / min with -x through every reduce kernel and catches a toolkit that folds it again.
+__device__ __forceinline__ int32_t neg_for_minmax(int32_t a) {
+    int32_t r;
+    asm("{.reg .s64 t; cvt.s64.s32 t, %1; neg.s64 t, t; cvt.u32.u64 %0, t;}" : "=r"(r) : "r"(a));
+    return r;
+}
 template <typename T, int FN>
 struct MapF {
     using V = T;
@@ -95,6 +122,7 @@ struct MapF {
     __device__ __forceinline__ V operator()(T x) const {
         if constexpr (FN == DAB_MAP_ABS) return jl::abs(x);
         else if constexpr (FN == DAB_MAP_ABS2) return jl::mul(x, x);
+        else if constexpr (FN == DAB_MAP_NEG && std::is_same<T, int32_t>::value) return neg_for_minmax(x);
         else if constexpr (FN == DAB_MAP_NEG) return jl::neg(x);
         else return x;
     }
@@ -114,6 +142,17 @@ struct PredF {
         else return x != (T)0;  // NONZERO / identity on Bool
     }
 };
+
+// ---- one 16-byte vector of mapped values folded into a widened accumulator ----------------------------------------------------
+// The kernels' register tree works in the element type.  When the tile type is wider (Int32 sums and products) they fold each
+// value straight into the Int64 accumulator instead: integer results do not depend on the grouping, and the chain keeps one Int64
+// live instead of one per element.
+template <typename R, typename T, typename Map>
+__device__ __forceinline__ typename R::A fold_into(typename R::A acc, const Pack<T>& p, const Map& map) {
+#pragma unroll
+    for (int k = 0; k < 16 / (int)sizeof(T); ++k) acc = R::comb(acc, R::lift(R::pre(map(p.v[k]))));
+    return acc;
+}
 
 // ---- shuffles for 4- and 8-byte accumulators -------------------------------------------------------
 template <typename A>

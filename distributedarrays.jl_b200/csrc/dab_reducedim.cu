@@ -29,7 +29,7 @@ __global__ void __launch_bounds__(RD_THREADS) rdim_lead_cta_kernel(const T* __re
                                                                     Map map, typename R::A* __restrict__ partials,
                                                                     Out* __restrict__ out, int accumulate) {
     using A = typename R::A;
-    using V = typename Map::V;
+    using W = typename R::W;
     constexpr int VPT = 16 / sizeof(T);
     constexpr int UNROLL = 4;
     __shared__ A smem[RD_THREADS / 32];
@@ -53,34 +53,39 @@ __global__ void __launch_bounds__(RD_THREADS) rdim_lead_cta_kernel(const T* __re
                 int4 r[UNROLL];
 #pragma unroll
                 for (int u = 0; u < UNROLL; ++u) r[u] = ld_stream(pv + i + (size_t)u * RD_THREADS);
-                V tv[UNROLL];
+                if constexpr (std::is_same<W, typename Map::V>::value) {
+                    W tv[UNROLL];
 #pragma unroll
-                for (int u = 0; u < UNROLL; ++u) {
-                    Pack<T> pk = as_pack<T>(r[u]);
-                    V m[VPT];
+                    for (int u = 0; u < UNROLL; ++u) {
+                        Pack<T> pk = as_pack<T>(r[u]);
+                        W m[VPT];
 #pragma unroll
-                    for (int k = 0; k < VPT; ++k) m[k] = map(pk.v[k]);
+                        for (int k = 0; k < VPT; ++k) m[k] = map(pk.v[k]);
 #pragma unroll
-                    for (int ww = VPT; ww > 1; ww >>= 1)
+                        for (int ww = VPT; ww > 1; ww >>= 1)
 #pragma unroll
-                        for (int k = 0; k < ww / 2; ++k) m[k] = R::tile(m[k], m[k + ww / 2]);
-                    tv[u] = m[0];
+                            for (int k = 0; k < ww / 2; ++k) m[k] = R::tile(m[k], m[k + ww / 2]);
+                        tv[u] = m[0];
+                    }
+#pragma unroll
+                    for (int ww = UNROLL; ww > 1; ww >>= 1)
+#pragma unroll
+                        for (int k = 0; k < ww / 2; ++k) tv[k] = R::tile(tv[k], tv[k + ww / 2]);
+                    acc = R::comb(acc, R::lift(tv[0]));
+                } else {  // widened tile (Int32 sums and products)
+#pragma unroll
+                    for (int u = 0; u < UNROLL; ++u) acc = fold_into<R>(acc, as_pack<T>(r[u]), map);
                 }
-#pragma unroll
-                for (int ww = UNROLL; ww > 1; ww >>= 1)
-#pragma unroll
-                    for (int k = 0; k < ww / 2; ++k) tv[k] = R::tile(tv[k], tv[k + ww / 2]);
-                acc = R::comb(acc, R::lift(tv[0]));
             }
             for (; i < nvec; i += RD_THREADS) {
                 Pack<T> pk = as_pack<T>(ld_stream(pv + i));
-                V m = map(pk.v[0]);
+                W m = R::pre(map(pk.v[0]));
 #pragma unroll
-                for (int k = 1; k < VPT; ++k) m = R::tile(m, map(pk.v[k]));
+                for (int k = 1; k < VPT; ++k) m = R::tile(m, R::pre(map(pk.v[k])));
                 acc = R::comb(acc, R::lift(m));
             }
-            for (size_t j = threadIdx.x; j < head; j += RD_THREADS) acc = R::comb(acc, R::lift(map(p[j])));
-            for (size_t j = head + nvec * VPT + threadIdx.x; j < n; j += RD_THREADS) acc = R::comb(acc, R::lift(map(p[j])));
+            for (size_t j = threadIdx.x; j < head; j += RD_THREADS) acc = R::comb(acc, R::lift(R::pre(map(p[j]))));
+            for (size_t j = head + nvec * VPT + threadIdx.x; j < n; j += RD_THREADS) acc = R::comb(acc, R::lift(R::pre(map(p[j]))));
         }
         acc = block_reduce<R>(acc, smem);
         if (threadIdx.x == 0) {
@@ -102,7 +107,7 @@ template <typename T, typename Map, typename R, typename Out, int G, bool VEC>
 __global__ void __launch_bounds__(RD_THREADS) rdim_lead_group_kernel(const T* __restrict__ x, size_t red, size_t outer, Map map,
                                                                       Out* __restrict__ out, int accumulate, int kruns) {
     using A = typename R::A;
-    using V = typename Map::V;
+    using W = typename R::W;
     constexpr int VPT = 16 / sizeof(T);
     constexpr int GROUPS = RD_THREADS / G;
     const int gl = threadIdx.x % G;           // lane inside the group
@@ -125,9 +130,9 @@ __global__ void __launch_bounds__(RD_THREADS) rdim_lead_group_kernel(const T* __
             A acc = R::identity();
             if (act[u]) {
                 Pack<T> pk = as_pack<T>(r[u]);
-                V m = map(pk.v[0]);
+                W m = R::pre(map(pk.v[0]));
 #pragma unroll
-                for (int k = 1; k < VPT; ++k) m = R::tile(m, map(pk.v[k]));
+                for (int k = 1; k < VPT; ++k) m = R::tile(m, R::pre(map(pk.v[k])));
                 acc = R::lift(m);
             }
 #pragma unroll
@@ -156,31 +161,31 @@ __global__ void __launch_bounds__(RD_THREADS) rdim_lead_group_kernel(const T* __
                 int4 r[4];
 #pragma unroll
                 for (int u = 0; u < 4; ++u) r[u] = ld_stream(pv + j + (size_t)u * G);
-                V tv[4];
+                W tv[4];
 #pragma unroll
                 for (int u = 0; u < 4; ++u) {
                     Pack<T> pk = as_pack<T>(r[u]);
-                    V m = map(pk.v[0]);
+                    W m = R::pre(map(pk.v[0]));
 #pragma unroll
-                    for (int k = 1; k < VPT; ++k) m = R::tile(m, map(pk.v[k]));
+                    for (int k = 1; k < VPT; ++k) m = R::tile(m, R::pre(map(pk.v[k])));
                     tv[u] = m;
                 }
                 acc = R::comb(acc, R::lift(R::tile(R::tile(tv[0], tv[1]), R::tile(tv[2], tv[3]))));
             }
             for (; j < nvec; j += G) {
                 Pack<T> pk = as_pack<T>(ld_stream(pv + j));
-                V m = map(pk.v[0]);
+                W m = R::pre(map(pk.v[0]));
 #pragma unroll
-                for (int k = 1; k < VPT; ++k) m = R::tile(m, map(pk.v[k]));
+                for (int k = 1; k < VPT; ++k) m = R::tile(m, R::pre(map(pk.v[k])));
                 acc = R::comb(acc, R::lift(m));
             }
         } else {
             size_t j = gl;
             for (; j + 3 * G < nred; j += 4 * G) {
                 T a0 = p[j], a1 = p[j + G], a2 = p[j + 2 * G], a3 = p[j + 3 * G];
-                acc = R::comb(acc, R::lift(R::tile(R::tile(map(a0), map(a1)), R::tile(map(a2), map(a3)))));
+                acc = R::comb(acc, R::lift(R::tile(R::tile(R::pre(map(a0)), R::pre(map(a1))), R::tile(R::pre(map(a2)), R::pre(map(a3))))));
             }
-            for (; j < nred; j += G) acc = R::comb(acc, R::lift(map(p[j])));
+            for (; j < nred; j += G) acc = R::comb(acc, R::lift(R::pre(map(p[j]))));
         }
 #pragma unroll
         for (int d = G / 2; d > 0; d >>= 1) acc = R::comb(acc, shfl_down<A>(acc, d));  // stays inside the G-lane group
@@ -233,16 +238,16 @@ __global__ void __launch_bounds__(RD_THREADS) rdim_strided_kernel(const T* __res
             T v[UNROLL];
 #pragma unroll
             for (int u = 0; u < UNROLL; ++u) v[u] = __ldcs(p + (r + u) * inner);
-            typename Map::V m[UNROLL];
+            typename R::W m[UNROLL];
 #pragma unroll
-            for (int u = 0; u < UNROLL; ++u) m[u] = map(v[u]);
+            for (int u = 0; u < UNROLL; ++u) m[u] = R::pre(map(v[u]));
 #pragma unroll
             for (int ww = UNROLL; ww > 1; ww >>= 1)
 #pragma unroll
                 for (int q = 0; q < ww / 2; ++q) m[q] = R::tile(m[q], m[q + ww / 2]);
             acc = R::comb(acc, R::lift(m[0]));
         }
-        for (; r < hi; ++r) acc = R::comb(acc, R::lift(map(__ldcs(p + r * inner))));
+        for (; r < hi; ++r) acc = R::comb(acc, R::lift(R::pre(map(__ldcs(p + r * inner)))));
         if (nsplit == 1) {
             if (accumulate) acc = R::comb((A)out[k], acc);
             out[k] = narrow<A, Out>(acc);
@@ -285,12 +290,12 @@ __global__ void __launch_bounds__(RD_THREADS) rdim_strided_vec_kernel(const T* _
             int4 v[UNROLL];
 #pragma unroll
             for (int u = 0; u < UNROLL; ++u) v[u] = ld_stream(p + (r + u) * ivec);
-            typename Map::V m[UNROLL][VPT];
+            typename R::W m[UNROLL][VPT];
 #pragma unroll
             for (int u = 0; u < UNROLL; ++u) {
                 Pack<T> pk = as_pack<T>(v[u]);
 #pragma unroll
-                for (int k = 0; k < VPT; ++k) m[u][k] = map(pk.v[k]);
+                for (int k = 0; k < VPT; ++k) m[u][k] = R::pre(map(pk.v[k]));
             }
 #pragma unroll
             for (int k = 0; k < VPT; ++k) {
@@ -301,7 +306,7 @@ __global__ void __launch_bounds__(RD_THREADS) rdim_strided_vec_kernel(const T* _
         for (; r < hi; ++r) {
             Pack<T> pk = as_pack<T>(ld_stream(p + r * ivec));
 #pragma unroll
-            for (int k = 0; k < VPT; ++k) acc[k] = R::comb(acc[k], R::lift(map(pk.v[k])));
+            for (int k = 0; k < VPT; ++k) acc[k] = R::comb(acc[k], R::lift(R::pre(map(pk.v[k]))));
         }
         const size_t k0 = kv * VPT;
 #pragma unroll

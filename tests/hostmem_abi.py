@@ -269,6 +269,10 @@ class HostMemABI:
     def dab_reducedim(self, ctx, dtype, op, mapc, x, inner, red, outer, out, accumulate):
         op, mapc, inner, red, outer = int(op), int(mapc), int(inner), int(red), int(outer)
         dt = _NP[int(dtype)]
+        if inner * outer == 0 or (red == 0 and int(accumulate)):
+            return 0
+        if red == 0 and op in (2, 3):
+            return 3                                               # DAB_ERR_EMPTY: max / min over an empty dimension
         v = _view(x, inner * red * outer, dt).reshape((inner, red, outer), order="F")
         code = C.c_int32()
         assert self._real().dab_reduce_result_dtype(int(dtype), op, mapc, C.byref(code)) == 0
@@ -276,10 +280,12 @@ class HostMemABI:
         wide = np.float64 if rdt.kind == "f" else np.int64
         with np.errstate(all="ignore"):
             m = {0: lambda: v, 1: lambda: np.abs(v), 2: lambda: v * v, 3: lambda: -v}[mapc]()
-            r = {0: lambda: m.astype(wide).sum(axis=1), 1: lambda: m.astype(wide).prod(axis=1), 2: lambda: m.max(axis=1), 3: lambda: m.min(axis=1)}[op]()
+            r = {0: lambda: m.astype(wide).sum(axis=1), 1: lambda: m.astype(wide).prod(axis=1), 2: lambda: jl_extreme(m, 1, True),
+                 3: lambda: jl_extreme(m, 1, False)}[op]()
             o = _view(out, inner * outer, rdt).reshape((inner, outer), order="F")
             if int(accumulate):
-                r = {0: np.add, 1: np.multiply, 2: np.maximum, 3: np.minimum}[op](o.astype(r.dtype), r)
+                r = {0: np.add, 1: np.multiply, 2: lambda a, b: jl_extreme(np.stack([a, b]), 0, True),
+                     3: lambda a, b: jl_extreme(np.stack([a, b]), 0, False)}[op](o.astype(r.dtype), r)
             o[...] = r.astype(rdt)
         self.launches += 1
         return 0
@@ -431,7 +437,7 @@ class HostMemABI:
         self.launches += 2
         return 0
 
-    # -- whole-chunk reductions: only what sort(d; sample=false) needs, minimum / maximum of a chunk (exact, NaN-propagating like Base);
+    # -- whole-chunk reductions: minimum / maximum of a chunk exact (NaN-propagating, +0.0 > -0.0, like Base);
     #    the host-only entry points (result dtype table, ordered fold) are the REAL library's -- they need no GPU
     def _real(self):
         if getattr(self, "_real_lib", None) is None:
@@ -451,13 +457,13 @@ class HostMemABI:
     def _reduce(self, dtype, op, mapc, param, x, n, out):
         """dab_reduce: op in SUM PROD MAX MIN ALL ANY COUNT (0..6), map in ID ABS ABS2 NEG (0..3) or a predicate (16..23, scalar parameter).
         Sums and products in the wide carrier (order-free stand-in for the kernel's tree: compared at tolerance by the tests that use it),
-        max / min exact (NaN-propagating like Base; signed zeros do not occur in the tests that use it)."""
+        max / min exact (NaN-propagating, +0.0 > -0.0, like Base)."""
         op, mapc = int(op), int(mapc)
         dt = _NP[int(dtype)] if int(dtype) != U8 else np.dtype(np.bool_)
         v = _view(x, int(n), dt)
         if op == 7:                                               # EXTREMA: [min, max] in the element type, one pass
             with np.errstate(all="ignore"):
-                pair = np.asarray([np.min(v), np.max(v)], dtype=dt)
+                pair = np.asarray([jl_extreme(v, 0, False), jl_extreme(v, 0, True)], dtype=dt)
             slot = np.zeros(16, dtype=np.uint8)
             slot[:2 * dt.itemsize] = pair.view(np.uint8)
             C.memmove(_addr(out), slot.ctypes.data, 16)
@@ -477,7 +483,7 @@ class HostMemABI:
             if op in (0, 1):
                 acc = (np.sum if op == 0 else np.prod)(m.astype(wide))
             elif op in (2, 3):
-                acc = (np.max if op == 2 else np.min)(m)
+                acc = jl_extreme(m, 0, op == 2)
             else:
                 acc = {4: lambda: int(np.all(m)), 5: lambda: int(np.any(m)), 6: lambda: int(np.count_nonzero(m))}[op]()
         slot = np.zeros(16, dtype=np.uint8)
@@ -565,6 +571,21 @@ class HostMemABI:
             counts[t] = n if rest_nan else lo
         self.launches += 1
         return 0
+
+
+def jl_extreme(m, axis, is_max):
+    """Base's maximum / minimum along ``axis``: any NaN gives NaN, otherwise the extreme value; a zero result is +0.0 for max when
+    a +0.0 is present and -0.0 for min when a -0.0 is present.  tests/test_gpu_reduce_exact.py keeps its own copy on purpose: that
+    one is the reference the kernels are checked against, this one stands in for the kernels."""
+    m = np.asarray(m)
+    if m.dtype.kind != "f":
+        return (np.max if is_max else np.min)(m, axis=axis)
+    nan = np.isnan(m)
+    r = (np.max if is_max else np.min)(np.where(nan, -np.inf if is_max else np.inf, m), axis=axis)
+    has = ((m == 0) & (np.signbit(m) != is_max)).any(axis=axis)
+    win, lose = (m.dtype.type(0.0), m.dtype.type(-0.0)) if is_max else (m.dtype.type(-0.0), m.dtype.type(0.0))
+    r = np.where(r == 0, np.where(has, win, lose), r)
+    return np.where(nan.any(axis=axis), m.dtype.type(np.nan), r).astype(m.dtype)
 
 
 # ---- NumPy interpreter of a traced expression (stands in for dab_unary / dab_affine / dab_broadcast_expr) ---------------------
