@@ -12,9 +12,11 @@ Everything computes on the GPU through ``csrc/libdab200.so`` (C ABI: ``include/d
 importing works anywhere, but the first op without the built extension or without an H100 raises.
 """
 from . import _lib
-from ._lib import ArgumentError, DabError, DimensionMismatch, UnsupportedError
+from ._lib import ArgumentError, DabError, DimensionMismatch, InexactError, UnsupportedError
 from ._broadcast import (Expr, Int128, abs2, broadcast, broadcast_into, ceil, copy, cos, deepcopy, drandn, exp, floor, ifelse, inv, isnan, jl_max, jl_min,
                         log, map_, map_bang, map_inplace, map_localparts, mod, rem, sign, sin, sqrt, tan, tanh, widen)
+from ._broadcast import angle, cis, conj, imag, iszero, real  # noqa: F401 -- complex values (complex(x[, y]) below)
+from ._broadcast import complex_ as complex  # noqa: A004
 from ._broadcast import (acos, acosh, acot, acoth, acsc, acsch, asec, asech, asin, asinh, atan, atanh, cbrt, cosh, cospi, cot, coth, csc,  # noqa: F401
                         csch, deg2rad, erf, erfc, erfcinv, erfcx, erfinv, exp10, exp2, expm1, gamma, isfinite, isinf, log10, log1p, log2,
                         loggamma, rad2deg, round_, sec, sech, sinh, sinpi, trunc)

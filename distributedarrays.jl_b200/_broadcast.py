@@ -45,10 +45,17 @@ class _TagTypes(dict):
 
 
 _NPT = _TagTypes({"bool": np.dtype(np.bool_), "i32": np.dtype(np.int32), "i64": np.dtype(np.int64), "f32": np.dtype(np.float32),
-                  "f64": np.dtype(np.float64)})
+                  "f64": np.dtype(np.float64), "c64": np.dtype(np.complex64), "c128": np.dtype(np.complex128)})
 _TAG = {v: k for k, v in _NPT.items()}
 SLICE_TRACING = [0]   # > 0 while mapslices (_slices.py) calls f on the slice tracer
-_CT = {"bool": "bool", "i32": "int", "i64": "long long", "i128": "i128", "f32": "float", "f64": "double"}
+_CT = {"bool": "bool", "i32": "int", "i64": "long long", "i128": "i128", "f32": "float", "f64": "double", "c64": "jl_c64", "c128": "jl_c128"}
+# ComplexF32 / ComplexF64 <-> their component type (``real(T)`` / ``Complex{T}``)
+_COMP = {"c64": "f32", "c128": "f64"}
+_CPLX_OF = {"f32": "c64", "f64": "c128"}
+
+
+def is_ctag(t: str) -> bool:
+    return t in _COMP
 
 
 def tag_of(dtype) -> str:
@@ -62,6 +69,11 @@ def promote(a: str, b: str) -> str:
     """``promote_type`` for the supported types (Int32+Float32 -> Float32, Float32+Float64 -> Float64, ...)."""
     if a == b:
         return a
+    if is_ctag(a) or is_ctag(b):
+        # Complex{S} with T -> Complex{promote_type(S, T)}: Float64 + ComplexF32 -> ComplexF64, Int64 / Bool + ComplexF32 -> ComplexF32
+        if "i128" in (a, b):
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "Int128 values mixed with complex values are not served")
+        return _CPLX_OF[promote(_COMP.get(a, a), _COMP.get(b, b))]
     if "f" in a[0] + b[0]:  # any float wins over ints/Bool (Int64 + Float32 -> Float32); Float64 only if one IS Float64
         fl = [t for t in (a, b) if t[0] == "f"]
         return "f64" if "f64" in fl else "f32"
@@ -86,6 +98,10 @@ class Expr:
             return v
         if isinstance(v, (bool, np.bool_)):
             return Expr("const", (), "bool", bool(v))
+        if isinstance(v, np.complex64):
+            return Expr("const", (), "c64", complex(v))
+        if isinstance(v, (complex, np.complexfloating)):
+            return Expr("const", (), "c128", complex(v))  # a Python complex literal is a ComplexF64
         if isinstance(v, (int, np.integer)):
             if isinstance(v, np.int32):
                 return Expr("const", (), "i32", int(v))
@@ -151,6 +167,8 @@ class Expr:
         return unop("abs", self)
 
     def __pow__(self, p):
+        if is_ctag(self.jt) or is_ctag(Expr.wrap(p).jt):
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "^ with a complex operand is not served (complex transcendental functions)")
         if isinstance(p, (int, np.integer)) and not isinstance(p, (bool, np.bool_)) and 1 <= int(p) <= 3:  # Base.literal_pow: x^2 == x*x, x^3 == x*x*x
             r = self
             for _ in range(int(p) - 1):
@@ -191,7 +209,29 @@ _FLOAT_ONLY = {"sqrt", "inv", "sin", "cos", "tan", "exp", "exp2", "log", "log2",
 _CMP = {"lt", "le", "gt", "ge", "eq", "ne"}
 
 
+_CPLX_BIN = {"add", "sub", "mul", "div", "eq", "ne"}
+
+
+def _cbinop(op: str, a: Expr, b: Expr) -> Expr:
+    """A binary operation with a complex operand, with Julia's methods: between complex values after promotion; a real operand keeps
+    the specialised real/complex methods (``x*z = Complex(x*zr, x*zi)``, ``x + z = Complex(x + zr, zi)``, ``z/x = Complex(zr/x, zi/x)``,
+    ...) in the component type instead of being promoted to complex -- they differ from full complex arithmetic at Inf / NaN
+    components.  ``==`` compares componentwise after promotion (``z == x`` is ``imag(z) == 0 && real(z) == x``)."""
+    if op in ("lt", "le", "gt", "ge", "max", "min"):
+        raise TypeError(f"MethodError: no method matching isless(::{a.jt}, ::{b.jt}) -- complex numbers are not ordered")
+    if op not in _CPLX_BIN:
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{op} with a complex operand is not served by the GPU backend")
+    jt = promote(a.jt, b.jt)
+    if op in ("eq", "ne"):
+        return Expr(op, (convert(a, jt), convert(b, jt)), "bool")
+    a = convert(a, jt) if is_ctag(a.jt) else convert(a, _COMP[jt])
+    b = convert(b, jt) if is_ctag(b.jt) else convert(b, _COMP[jt])
+    return Expr(op, (a, b), jt)
+
+
 def binop(op: str, a: Expr, b: Expr) -> Expr:
+    if is_ctag(a.jt) or is_ctag(b.jt):
+        return _cbinop(op, a, b)
     jt = promote(a.jt, b.jt)
     if op == "div" and jt[0] != "f":
         jt = "f64"  # Int / Int -> Float64
@@ -210,6 +250,8 @@ def binop(op: str, a: Expr, b: Expr) -> Expr:
 def shiftop(op: str, a: Expr, n: Expr) -> Expr:
     """``a << n`` / ``a >> n`` (test/darray.jl:863-867).  Unlike the arithmetic operators the operands are NOT promoted to a common
     type: the result has the type of ``a`` (Bool counts as Int) and ``n`` is a bit count (Int64 here)."""
+    if is_ctag(a.jt) or is_ctag(n.jt):
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "shifts of complex values are not served")
     if a.jt[0] == "f" or n.jt[0] == "f":
         raise TypeError(f"MethodError: no method matching {'<<' if op == 'x_shl' else '>>'}(::{a.jt}, ::{n.jt})")
     if a.jt == "i128" or n.jt == "i128":
@@ -219,7 +261,18 @@ def shiftop(op: str, a: Expr, n: Expr) -> Expr:
     return Expr(op, (a, convert(n, "i64")), a.jt)
 
 
+# functions served on a complex value: -z, conj, real, imag, abs (hypot), abs2, angle, inv, isnan / isinf / isfinite
+_CPLX_UN = {"neg", "conj", "real", "imag", "abs", "abs2", "angle", "inv", "isnan", "isinf", "isfinite"}
+
+
 def unop(op: str, a: Expr) -> Expr:
+    if is_ctag(a.jt):
+        if op not in _CPLX_UN:
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{op.removeprefix('x_')} of a complex value is not served by the GPU backend "
+                                        "(complex transcendental functions)")
+        if op in ("isnan", "isinf", "isfinite"):
+            return Expr(op, (a,), "bool")
+        return Expr(op, (a,), _COMP[a.jt] if op in ("real", "imag", "abs", "abs2", "angle") else a.jt)
     if op in _FLOAT_ONLY and a.jt[0] != "f":
         a = convert(a, "f64")  # sqrt(::Int) -> Float64
     if op in ("isnan", "isinf", "isfinite"):
@@ -234,8 +287,17 @@ def unop(op: str, a: Expr) -> Expr:
 def convert(a: Expr, jt: str) -> Expr:
     if a.jt == jt:
         return a
+    if is_ctag(a.jt) and not is_ctag(jt):
+        if a.op == "const" and complex(a.val).imag == 0:
+            return convert(Expr("const", (), _COMP[a.jt], complex(a.val).real), jt)
+        raise _lib.InexactError(_lib.ERR_UNSUPPORTED, f"InexactError: a {a.jt} value cannot be converted to {jt}")
     if a.op == "const":
         v = a.val
+        if is_ctag(jt):
+            z = complex(v)
+            if jt == "c64":
+                z = complex(np.complex64(z))
+            return Expr("const", (), jt, z)
         if jt == "f32":
             v = float(np.float32(v))
         elif jt == "f64":
@@ -265,6 +327,73 @@ def widen(x) -> Expr:
 
 def uses_tag(e: Expr, tag: str) -> bool:
     return e.jt == tag or builtins_any(uses_tag(a, tag) for a in e.args)
+
+
+def real(x) -> Expr:
+    """``real(z)``; ``real(x) = x`` for a real value."""
+    e = _traced(x, "real")
+    return unop("real", e) if is_ctag(e.jt) else e
+
+
+def imag(x) -> Expr:
+    """``imag(z)``; ``imag(x) = zero(x)`` for a real value."""
+    e = _traced(x, "imag")
+    return unop("imag", e) if is_ctag(e.jt) else convert(Expr.wrap(0), e.jt)
+
+
+def conj(x) -> Expr:
+    """``conj(z) = Complex(real(z), -imag(z))``; ``conj(x) = x`` for a real value."""
+    e = _traced(x, "conj")
+    return unop("conj", e) if is_ctag(e.jt) else e
+
+
+def angle(x) -> Expr:
+    """``angle(z) = atan(imag(z), real(z))``; ``angle(x) = atan(zero(x), x)`` for a real value (0 or pi)."""
+    e = _traced(x, "angle")
+    return unop("angle", e) if is_ctag(e.jt) else Expr("angle", (_float_of(e),), _float_of(e).jt)
+
+
+def cis(x) -> Expr:
+    """``cis(x) = Complex(cos(x), sin(x))`` of a real value (an integer becomes Float64 first)."""
+    e = _traced(x, "cis")
+    if is_ctag(e.jt):
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "cis of a complex value is not served (complex transcendental functions)")
+    e = _float_of(e)
+    return Expr("cis", (e,), _CPLX_OF[e.jt])
+
+
+def complex_(x, y=None) -> Expr:
+    """``complex(x)`` / ``complex(x, y)``: a ComplexF32 / ComplexF64 from real Float32 / Float64 parts (promoted to one type).
+    ``Complex{Int}`` and ``Complex{Bool}`` values are not served."""
+    e = _traced(x, "complex")
+    if y is None:
+        if is_ctag(e.jt):
+            return e
+        if e.jt not in _CPLX_OF:
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"complex({e.jt}) would be Complex{{{e.jt}}}: only ComplexF32 / ComplexF64 are served")
+        return convert(e, _CPLX_OF[e.jt])
+    f = Expr.wrap(y)
+    if is_ctag(e.jt) or is_ctag(f.jt):
+        raise TypeError("MethodError: complex(x, y) takes two real parts")
+    jt = promote(e.jt, f.jt)
+    if jt not in _CPLX_OF:
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"complex of {jt} parts would be Complex{{{jt}}}: only ComplexF32 / ComplexF64 are served")
+    return Expr("complex", (convert(e, jt), convert(f, jt)), _CPLX_OF[jt])
+
+
+def iszero(x) -> Expr:
+    """``iszero(x)``: ``x == 0`` (both components for a complex value; -0.0 counts as zero)."""
+    return binop("eq", _traced(x, "iszero"), Expr.wrap(0))
+
+
+def _traced(x, name: str) -> Expr:
+    if isinstance(x, Expr):
+        return x
+    raise TypeError(f"dab.{name} is for use inside broadcast/map kernels")
+
+
+def uses_complex(e: Expr) -> bool:
+    return is_ctag(e.jt) or builtins_any(uses_complex(a) for a in e.args)
 
 
 def ifelse(c, a, b) -> Expr:
@@ -388,6 +517,9 @@ def _lit(jt: str, v) -> str:
         return "__int_as_float((int)0x%08x)" % struct.unpack("<I", struct.pack("<f", float(v)))[0]
     if jt == "f64":
         return "__longlong_as_double((long long)0x%016xULL)" % struct.unpack("<Q", struct.pack("<d", float(v)))[0]
+    if is_ctag(jt):
+        z = complex(v)
+        return "%s(%s, %s)" % (_CT[jt], _lit(_COMP[jt], z.real), _lit(_COMP[jt], z.imag))
     if jt == "i32":
         return "((int)%d)" % int(v)
     if jt == "i64":
@@ -404,7 +536,11 @@ def codegen(e: Expr) -> str:
     if e.op == "const":
         return _lit(e.jt, e.val)
     if e.op == "convert":
+        if is_ctag(e.jt):
+            return f"{_CT[e.jt]}({codegen(e.args[0])})"             # constructor: from a real value or the other complex type
         return f"(({_CT[e.jt]})({codegen(e.args[0])}))"
+    if e.op == "complex":
+        return f"{_CT[e.jt]}({codegen(e.args[0])}, {codegen(e.args[1])})"
     if e.op == "ifelse":
         return f"(({codegen(e.args[0])}) ? ({codegen(e.args[1])}) : ({codegen(e.args[2])}))"
     if e.op in _FN2:
@@ -506,8 +642,10 @@ def run_local(rt, expr: Expr, out: B200Array, largs: List[LocalArg]):
     ctx = rt.ctx
     code = dab_dtype(out.dtype)
     rt.last_kernel = "fixed"
+    # complex trees never take a hand-written real kernel: they all go to the NVRTC kernel
+    cplx = uses_complex(expr) or builtins_any(is_ctag(a.tag) for a in largs)
     # ---- hand-written kernels when the tree is one of the fixed shapes
-    if same and expr.jt == out_tag and out_tag != "bool":
+    if same and not cplx and expr.jt == out_tag and out_tag != "bool":
         x0 = largs[0] if largs and largs[0].arr is not None and largs[0].tag == out_tag else None
         if x0 is not None and all(_only_arg0(expr)):
             ab = match_affine(expr)
@@ -558,10 +696,13 @@ def run_local(rt, expr: Expr, out: B200Array, largs: List[LocalArg]):
     rt.last_kernel = "dab_broadcast_expr"
     if uses_tag(expr, "i128"):
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "Int128 values are served inside mapreduce(f, op, d) only, not in a broadcast")
-    if expr.jt[0] == "f" and out_tag[0] != "f":
+    if expr.jt[0] == "f" and out_tag[0] not in "fc":
         # dest .= f.(...) with an integer/Bool destination and float values: Julia converts exactly or throws InexactError per
         # element; a C cast would silently truncate
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"broadcast of {expr.jt} values into a {out_tag} destination (InexactError semantics) is not served")
+    if is_ctag(expr.jt) and not is_ctag(out_tag):
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"broadcast of {expr.jt} values into a {out_tag} destination (InexactError semantics) is not served")
+    expr, largs = split_c128_scalars(expr, largs)
     src = codegen(convert(expr, out_tag)).encode()
     oshape_nd, ashapes = tuple(out.shape), {k: tuple(a.arr.shape) for k, a in enumerate(largs) if a.arr is not None}
     if len(oshape_nd) > 4 or any(len(sh) > 4 for sh in ashapes.values()):
@@ -595,6 +736,28 @@ def run_local(rt, expr: Expr, out: B200Array, largs: List[LocalArg]):
             scal[k] = struct.unpack("<Q", np.asarray(a.scalar, dtype=_NPT[a.tag]).tobytes().ljust(8, b"\0"))[0]
     _lib.call("dab_broadcast_expr", ctx, src, code, C.c_void_p(out.ptr), _lib.sz4(oshape), _lib.sz4(_dense_strides(oshape)), nargs, dts,
               ptrs, strides, scal)
+
+
+def split_c128_scalars(expr: Expr, largs: List["LocalArg"]):
+    """A ComplexF64 scalar does not fit the kernels' 8-byte scalar slot: it enters as ``complex(re, im)`` of two Float64 scalars, its own
+    slot holding the real part and a new last argument the imaginary part.  The generated source depends on the argument positions
+    only, so one compiled kernel serves every value."""
+    ks = [k for k, a in enumerate(largs) if a.arr is None and a.tag == "c128"]
+    if not ks:
+        return expr, largs
+    largs, sub = list(largs), {}
+    for k in ks:
+        z = complex(largs[k].scalar)
+        largs[k] = LocalArg(None, z.real, "f64")
+        largs.append(LocalArg(None, z.imag, "f64"))
+        sub[k] = Expr("complex", (Expr("arg", (), "f64", k), Expr("arg", (), "f64", len(largs) - 1)), "c128")
+
+    def rw(e: Expr) -> Expr:
+        if e.op == "arg":
+            return sub.get(e.val, e)
+        return Expr(e.op, tuple(rw(a) for a in e.args), e.jt, e.val, e.weak) if e.args else e
+
+    return rw(expr), largs
 
 
 def _squeeze(shape):
@@ -761,8 +924,20 @@ def drandn(dims, procs=None, dist=None, dtype=np.float64, seed: int = 1234, rt=N
     """``drandn(dims, ...)`` (reference src/darray.jl:526-532): standard-normal entries.  Box-Muller over two counter-based uniform streams
     (``drand`` with seeds ``seed`` and ``seed + 1``; layout-independent like ``drand``), fused into one elementwise kernel:
     ``sqrt(-2 log(1 - u1)) * cos(2 pi u2)`` with ``1 - u1`` in (0, 1] so the logarithm is finite."""
-    from ._darray import drand
+    from ._darray import component_dtype, drand
     dt = np.dtype(dtype)
+    if dt.kind == "c":
+        # randn(Complex{T}) = Complex{T}(SQRT_HALF * randn(T), SQRT_HALF * randn(T)) (SQRT_HALF a Float64): two real streams, seeds
+        # (seed, seed + 1) and (seed + 2, seed + 3)
+        ct = component_dtype(dt)
+        re = drandn(dims, procs, dist, dtype=ct, seed=seed, rt=rt)
+        im = drandn(dims, procs, dist, dtype=ct, seed=seed + 2, rt=rt)
+        from ._darray import darray_like
+        out = darray_like(lambda I: B200Array.empty(re.rt, shape_of(I), dt), re, dtype=dt)        # re's layout (procs, dist)
+        _broadcast_into(out, lambda a, b: complex_(0.7071067811865476 * a, 0.7071067811865476 * b), re, im)
+        re.close()
+        im.close()
+        return out
     if dt.kind != "f":
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"drandn of eltype {dt}")
     u1 = drand(dims, procs, dist, dtype=dt, seed=seed, rt=rt)

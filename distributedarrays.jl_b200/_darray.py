@@ -25,9 +25,10 @@ from .layout import Layout, Range, default_procs, layout_from_chunk_shapes, make
 from .runtime import Runtime, close_remote_reads, open_remote_reads, runtime
 
 _DT = {np.dtype(np.float32): _lib.F32, np.dtype(np.float64): _lib.F64, np.dtype(np.int32): _lib.I32,
-       np.dtype(np.int64): _lib.I64, np.dtype(np.bool_): _lib.U8}   # UInt8 is NOT Bool: unserved eltypes raise (no silent reinterpretation)
+       np.dtype(np.int64): _lib.I64, np.dtype(np.bool_): _lib.U8,   # UInt8 is NOT Bool: unserved eltypes raise (no silent reinterpretation)
+       np.dtype(np.complex64): _lib.C64, np.dtype(np.complex128): _lib.C128}   # ComplexF32 / ComplexF64, interleaved (re, im)
 _NP = {_lib.F32: np.dtype(np.float32), _lib.F64: np.dtype(np.float64), _lib.I32: np.dtype(np.int32),
-       _lib.I64: np.dtype(np.int64), _lib.U8: np.dtype(np.bool_)}
+       _lib.I64: np.dtype(np.int64), _lib.U8: np.dtype(np.bool_), _lib.C64: np.dtype(np.complex64), _lib.C128: np.dtype(np.complex128)}
 
 
 def dab_dtype(dt) -> int:
@@ -39,6 +40,16 @@ def dab_dtype(dt) -> int:
 
 def np_dtype(code: int) -> np.dtype:
     return _NP[code]
+
+
+def is_complex(dt) -> bool:
+    return np.dtype(dt).kind == "c"
+
+
+def component_dtype(dt) -> np.dtype:
+    """``real(T)``: the element type of each component of a complex type (the type itself for a real one)."""
+    dt = np.dtype(dt)
+    return {np.dtype(np.complex64): np.dtype(np.float32), np.dtype(np.complex128): np.dtype(np.float64)}.get(dt, dt)
 
 
 _allowscalar = [True]
@@ -646,7 +657,8 @@ def dfill(v, dims, procs=None, dist=None, dtype=None, rt=None) -> DArray:
 
 def drand(dims, procs=None, dist=None, dtype=np.float64, seed: int = 1234, rt=None) -> DArray:
     """``drand`` (src/darray.jl:502-518) with the counter-based generator: element with global column-major linear index
-    g is ``(hash32(seed, g) >> 8) * 2^-24`` -- layout-independent and reproducible on the CPU oracle."""
+    g is ``(hash32(seed, g) >> 8) * 2^-24`` -- layout-independent and reproducible on the CPU oracle.  A complex element g is
+    ``complex(u(2g), u(2g+1))`` of that stream in the component type (Julia's ``rand(Complex{T}) = complex(rand(T), rand(T))``)."""
     rt = rt or runtime()
     dims = tuple(int(d) for d in dims)
     dt = np.dtype(dtype)
@@ -662,7 +674,8 @@ def drand(dims, procs=None, dist=None, dtype=np.float64, seed: int = 1234, rt=No
 def _rand_block(rt, ch: B200Array, dims, I, seed):
     """Fill chunk ``I`` of a global array so that values depend on the GLOBAL linear index only: one launch per
     contiguous run of the chunk (runs = trailing-index combinations of the dims after the first split one)."""
-    code = dab_dtype(ch.dtype)
+    code = dab_dtype(component_dtype(ch.dtype))
+    ncomp = 2 if is_complex(ch.dtype) else 1          # a complex array is filled through its real view of 2n components
     shp = shape_of(I)
     # length of the prefix of dims the chunk spans completely -> contiguous run in global memory
     run, k = 1, 0
@@ -679,7 +692,7 @@ def _rand_block(rt, ch: B200Array, dims, I, seed):
     for tail in itertools.product(*reversed(rest)):
         tail = tuple(reversed(tail))
         g = base0 + sum(int(strides[k + j]) * tail[j] for j in range(len(tail)))
-        _lib.call("dab_rand_u01", rt.ctx, code, C.c_void_p(ch.ptr + off * ch.dtype.itemsize), run, int(seed), int(g))
+        _lib.call("dab_rand_u01", rt.ctx, code, C.c_void_p(ch.ptr + off * ch.dtype.itemsize), ncomp * run, int(seed), ncomp * int(g))
         off += run
 
 

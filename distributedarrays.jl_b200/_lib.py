@@ -14,7 +14,7 @@ SO_PATH = os.path.join(_HERE, "csrc", "libdab200.so")
 
 # ---- enums (include/dab200.h) ----------------------------------------------------------------------------
 OK, ERR_CUDA, ERR_ARG, ERR_EMPTY, ERR_DIM_MISMATCH, ERR_NCCL, ERR_UNSUPPORTED, ERR_NVRTC, ERR_NOMEM = range(9)
-F32, F64, I32, I64, U8, I128 = range(6)     # I128: value type of dab_mapreduce_expr only
+F32, F64, I32, I64, U8, I128, C64, C128 = range(8)     # I128: value type of dab_mapreduce_expr only; C64/C128: ComplexF32/F64
 SUM, PROD, MAX, MIN, ALL, ANY, COUNT, EXTREMA = range(8)
 MAP_ID, MAP_ABS, MAP_ABS2, MAP_NEG, MAP_SQRT, MAP_INV, MAP_FLOOR, MAP_CEIL, MAP_SIGN = range(9)
 MAP_EQ, MAP_NE, MAP_LT, MAP_LE, MAP_GT, MAP_GE, MAP_ISNAN, MAP_NONZERO = range(16, 24)
@@ -38,6 +38,10 @@ class ArgumentError(DabError, ValueError):
 
 class DimensionMismatch(DabError, ValueError):
     """Julia ``DimensionMismatch`` (reference src/broadcast.jl:66, src/darray.jl:564)."""
+
+
+class InexactError(DabError, ValueError):
+    """Julia ``InexactError``: a value that the destination's element type cannot hold (a complex scalar into a real array)."""
 
 
 class UnsupportedError(DabError, NotImplementedError):
@@ -100,6 +104,7 @@ _SIGS = {
     "dab_gemv": (_i32, [_vp, _i32, _i32, _vp, _sz, _sz, _vp, _vp]),
     "dab_gemm": (_i32, [_vp, _i32, _i32, _sz, _sz, _sz, _vp, _sz, _vp, _sz, _vp, _sz]),
     "dab_transpose_box": (_i32, [_vp, _i32, _vp, _sz, _vp, _sz, _sz, _sz]),
+    "dab_adjoint_box": (_i32, [_vp, _i32, _vp, _sz, _vp, _sz, _sz, _sz]),
     "dab_sort": (_i32, [_vp, _i32, _vp, _vp, _vp, _sz]),
     "dab_sorted_split": (_i32, [_vp, _i32, _vp, _sz, _vp, _i32, C.POINTER(C.c_ulonglong)]),
     "dab_sort_by_key": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _sz, _sz]),

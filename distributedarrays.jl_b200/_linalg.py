@@ -49,7 +49,8 @@ class Transpose:
 
 
 class Adjoint(Transpose):
-    """``D'`` / ``adjoint(D)``.  Element types served here are real, so it equals the transpose (reference src/linalg.jl:1-8)."""
+    """``D'`` / ``adjoint(D)`` (reference src/linalg.jl:1-8): the conjugate transpose.  For a real element type it equals the transpose;
+    ``copy`` of the adjoint of a ComplexF32 / ComplexF64 DMatrix conjugates every element on the way (``dab_adjoint_box``)."""
 
     conj = True
 
@@ -60,6 +61,14 @@ def transpose(D: DArray) -> Transpose:
 
 def adjoint(D: DArray) -> Adjoint:
     return Adjoint(D)
+
+
+def _refuse_complex(what: str, *xs):
+    """Complex matrix products (GEMV / GEMM) have no kernel yet: refuse on the host, before any allocation or launch."""
+    for x in xs:
+        dt = x.parent.dtype if isinstance(x, Transpose) else (x.dtype if isinstance(x, (DArray, SubDArray)) else np.asarray(x).dtype)
+        if np.dtype(dt).kind == "c":
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what} with element type {np.dtype(dt)} is not served (no complex GEMV / GEMM kernel)")
 
 
 def copy_transposed(W: Transpose) -> DArray:
@@ -73,6 +82,7 @@ def copy_transposed(W: Transpose) -> DArray:
     R = darray(lambda I: B200Array.empty(rt, shape_of(I), D.dtype), W.dims, procs=list(D.layout.pids), dtype=D.dtype, rt=rt)
     fenced = open_remote_reads(rt, [D], "host")
     es = D.dtype.itemsize
+    conj = W.conj and D.dtype.kind == "c"                 # the adjoint of a real matrix is its transpose
     from .layout import slab_plan
     for pid, out in R.chunks.items():
         I = R.layout.localindices(pid)                    # ranges of the transposed array held here
@@ -88,7 +98,10 @@ def copy_transposed(W: Transpose) -> DArray:
             src = D.peer_ptr(spid) + ((sr[0] - 1) + (sc[0] - 1) * sshape[0]) * es
             # J-box element (r, c) -> out[c, r]
             dst = out.ptr + ((dc[0] - 1) + (dr[0] - 1) * dst_ld) * es
-            _lib.call("dab_transpose_box", rt.ctx, es, C.c_void_p(dst), dst_ld, C.c_void_p(src), sshape[0], rows, cols)
+            if conj:
+                _lib.call("dab_adjoint_box", rt.ctx, dab_dtype(D.dtype), C.c_void_p(dst), dst_ld, C.c_void_p(src), sshape[0], rows, cols)
+            else:
+                _lib.call("dab_transpose_box", rt.ctx, es, C.c_void_p(dst), dst_ld, C.c_void_p(src), sshape[0], rows, cols)
     close_remote_reads(rt, fenced, "host")
     return R
 
@@ -146,6 +159,7 @@ def mul_(y: DArray, A: Union[DArray, Transpose], x, alpha=1, beta=0) -> DArray:
     """``mul!(y::DVector, A::DMatrix, x::AbstractVector, α=1, β=0)`` (reference src/linalg.jl:78-118) and, for a
     ``Transpose``/``Adjoint`` wrapper, :120-167.  Error contract as the reference: DimensionMismatch when the contracted sizes
     differ, ArgumentError when y's cuts do not match the matrix cuts along the kept dim."""
+    _refuse_complex("mul!", y, A, x)
     M, trans = _unwrap(A)
     if isinstance(x, (DArray, np.ndarray)) and len(np.shape(x) if not isinstance(x, DArray) else x.dims) == 2:
         return mul_mat_(y, A, x, alpha, beta)
@@ -238,6 +252,7 @@ def matmul(A: Union[DArray, Transpose], x) -> DArray:
     if isinstance(A, Expr) or isinstance(x, Expr):
         from ._slices import matmul_of_slices
         return matmul_of_slices(A, x)
+    _refuse_complex("A*x", A, x)
     M, trans = _unwrap(A)
     xnd = len(x.dims) if isinstance(x, DArray) else np.ndim(x)
     if xnd == 2:
@@ -310,6 +325,7 @@ def mul_mat_(Cd: DArray, A: Union[DArray, Transpose], B, alpha=1, beta=0) -> DAr
     """``mul!(C::DMatrix, A::DMatrix, B::AbstractMatrix, α=1, β=0)`` and the Adjoint / Transpose forms = ``_matmatmul!`` (reference
     src/linalg.jl:189-261).  Same errors as the reference: DimensionMismatch for the contracted / result sizes, ArgumentError when the
     cuts of C's first dimension differ from A's."""
+    _refuse_complex("mul!", Cd, A, B)
     M, trans = _unwrap(A)
     if M.ndim != 2 or Cd.ndim != 2:
         raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, "mul!: C and A must be DMatrices")
@@ -398,6 +414,7 @@ def matmat(A: Union[DArray, Transpose], B) -> DArray:
     ``A'*B`` / ``transpose(A)*B`` (:302-311): on ``procs(A)[1:min(size(procs(A),1), size(procs(B),2)), :]`` with grid
     ``(size(procs(A),2), that min)``.  The reference asks ``procs(B)`` for its grid, so B is a DMatrix there; a host matrix is accepted
     here as a one-column grid (what ``distribute`` of a matrix no wider than tall gives on these workers)."""
+    _refuse_complex("A*B", A, B)
     M, trans = _unwrap(A)
     if M.ndim != 2:
         raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, "A must be a DMatrix")
@@ -426,6 +443,7 @@ def matmat(A: Union[DArray, Transpose], B) -> DArray:
 def lmul_diag(d, DA: DArray) -> DArray:
     """``lmul!(D::Diagonal, DA::DMatrix)`` with ``d = D.diag`` (reference src/linalg.jl:169-177): DA[i,j] = d[i]*DA[i,j]."""
     from ._broadcast import broadcast_into
+    _refuse_complex("lmul!(Diagonal, A)", d, DA)
     dv = np.asarray(d)
     if DA.ndim != 2 or dv.shape != (DA.dims[0],):
         raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, f"lmul!: diagonal of length {dv.shape} vs matrix {DA.dims}")
@@ -435,6 +453,7 @@ def lmul_diag(d, DA: DArray) -> DArray:
 def rmul_diag(DA: DArray, d) -> DArray:
     """``rmul!(DA::DMatrix, D::Diagonal)`` (reference src/linalg.jl:179-187): DA[i,j] = DA[i,j]*d[j]."""
     from ._broadcast import broadcast_into
+    _refuse_complex("rmul!(A, Diagonal)", DA, d)
     dv = np.asarray(d)
     if DA.ndim != 2 or dv.shape != (DA.dims[1],):
         raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, f"rmul!: diagonal of length {dv.shape} vs matrix {DA.dims}")

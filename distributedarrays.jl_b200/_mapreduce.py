@@ -20,8 +20,8 @@ from typing import Callable, Dict, Optional, Sequence, Tuple
 import numpy as np
 
 from . import _lib
-from ._broadcast import Expr, broadcast, tag_of, trace, _NPT
-from ._darray import B200Array, DArray, dab_dtype, np_dtype
+from ._broadcast import Expr, broadcast, is_ctag, tag_of, trace, _NPT
+from ._darray import B200Array, DArray, component_dtype, dab_dtype, is_complex, np_dtype
 from .layout import Layout, collapse_for_region, ravel, shape_of, unravel
 from .runtime import close_remote_reads, exchange_stacks, fence, grouped_exchange, open_remote_reads
 
@@ -51,6 +51,13 @@ def classify_map(f: Optional[Callable], dtype) -> Tuple[Optional[int], Optional[
     e = trace(f, [tag])
     if e.op == "arg":
         return _lib.MAP_ID, None, e
+    if is_ctag(tag):
+        # complex chunks: the reduce kernels serve abs, abs2, -z and isnan; z*z is a complex product, not abs2
+        if len(e.args) == 1 and e.args[0].op == "arg":
+            code = {"abs": _lib.MAP_ABS, "abs2": _lib.MAP_ABS2, "neg": _lib.MAP_NEG, "isnan": _lib.MAP_ISNAN}.get(e.op)
+            if code is not None:
+                return code, None, e
+        return None, None, e
     if e.jt == tag and len(e.args) == 1 and e.args[0].op == "arg":
         code = {"abs": _lib.MAP_ABS, "abs2": _lib.MAP_ABS2, "neg": _lib.MAP_NEG}.get(e.op)
         if code is not None:
@@ -161,7 +168,7 @@ def _empty_slot(rt, opc: int, rdt: np.dtype, slot_ptr: int):
 def _mapreduce_expr(expr: Expr, opc: int, d: DArray, others: Sequence, return_partials: bool = False):
     """General ``mapreduce(f, op, d, others...)``: f is an arbitrary traced expression over 1..8 arguments.  ONE fused NVRTC
     kernel per localpart (``dab_mapreduce_expr``), no temporary f.(d) array; combine as in ``_mapreduce_all``."""
-    from ._broadcast import _NPT as NPT, _localise, _remote_args, codegen
+    from ._broadcast import _NPT as NPT, _localise, _remote_args, codegen, split_c128_scalars
     rt = d.rt
     args = [d] + list(others)
     for a in others:
@@ -173,6 +180,10 @@ def _mapreduce_expr(expr: Expr, opc: int, d: DArray, others: Sequence, return_pa
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "more than 8 mapreduce arguments are not served")
     _check_nonempty(d, opc)
     val_tag = expr.jt
+    if is_ctag(val_tag) and opc in (_lib.MAX, _lib.MIN):
+        raise TypeError(f"MethodError: no method matching isless(::{val_tag}, ::{val_tag}) -- complex numbers are not ordered")
+    if is_ctag(val_tag) and opc not in (_lib.SUM, _lib.PROD):
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "complex values are reduced with + and * only")
     wide = val_tag == "i128"                     # Int128 VALUES (f widens its argument): the 16-byte slot is the result
     if wide and opc not in (_lib.SUM, _lib.PROD, _lib.MAX, _lib.MIN):
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "Int128 values are reduced with + * max min only")
@@ -185,7 +196,6 @@ def _mapreduce_expr(expr: Expr, opc: int, d: DArray, others: Sequence, return_pa
         rdt = np.dtype((np.void, 16))            # raw slot bytes; decoded to Python ints below
     else:
         rdt = np.dtype(np.int64) if val_tag in ("bool", "i32", "i64") and opc in (_lib.SUM, _lib.PROD, _lib.ALL, _lib.ANY, _lib.COUNT) else NPT[val_tag]
-    src = codegen(expr).encode()
     fenced = open_remote_reads(rt, _remote_args(d.layout, others), "host")
     temps = []
 
@@ -194,6 +204,10 @@ def _mapreduce_expr(expr: Expr, opc: int, d: DArray, others: Sequence, return_pa
             return _empty_slot(rt, opc, np.dtype(np.int64) if wide else rdt, slot_ptr)   # 0 / 1 zero-extended = the Int128 identity
         I = d.layout.localindices(pid)
         largs = [_localise(rt, a, I, pid) for a in args]
+        e, largs = split_c128_scalars(expr, largs)
+        if len(largs) > 8:
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "more than 8 mapreduce arguments (a ComplexF64 scalar counts twice) are not served")
+        src = codegen(e).encode()
         n = len(largs)
         dts = (C.c_int32 * n)(*[dab_dtype(NPT[la.tag]) for la in largs])
         ptrs = (C.c_void_p * n)(*[la.arr.ptr if la.arr is not None else None for la in largs])
@@ -225,6 +239,12 @@ def _mapreduce_all(f, op, d: DArray, return_partials: bool = False, others: Sequ
         expr = trace(f, [tag_of(d.dtype)] + [_arg_tag_of(a) for a in others])
         return _mapreduce_expr(expr, opc, d, others, return_partials)
     mapc, param, expr = classify_map(f, d.dtype)
+    if is_complex(d.dtype) and mapc is not None and not _complex_served(opc, mapc):
+        if mapc == _lib.MAP_ID and opc in (_lib.MAX, _lib.MIN):
+            raise TypeError(f"MethodError: no method matching isless(::{d.dtype}, ::{d.dtype}) -- complex numbers are not ordered")
+        mapc = None                                                 # e.g. prod(abs, z): the fused NVRTC kernel on the mapped values
+        if expr is None:
+            expr = trace(lambda z: z, [tag_of(d.dtype)])
     if mapc is None:
         return _mapreduce_expr(expr, opc, d, (), return_partials)   # general closure: one fused NVRTC kernel per chunk
     _check_nonempty(d, opc)
@@ -241,6 +261,12 @@ def _mapreduce_all(f, op, d: DArray, return_partials: bool = False, others: Sequ
     host = _gather_slots(d, lambda pid, ch, slot: _lib.call("dab_reduce", rt.ctx, code, opc, mapc, pp, C.c_void_p(ch.ptr), ch.size, C.c_void_p(slot)))
     res, vals = _fold(host, d.layout.pids, rdt, opc)
     return (res, vals) if return_partials else res
+
+
+def _complex_served(opc: int, mapc: int) -> bool:
+    """(op, map) pairs the reduce kernels serve on a complex chunk (include/dab200.h, dab_reduce)."""
+    out = C.c_int32()
+    return _lib.lib().dab_reduce_result_dtype(_lib.C64, opc, mapc, C.byref(out)) == _lib.OK
 
 
 def _arg_tag_of(a) -> str:
@@ -390,6 +416,8 @@ def extrema(d: DArray):
             return extrema(tmp)
         finally:
             tmp.close()
+    if is_complex(d.dtype):
+        raise TypeError(f"MethodError: no method matching isless(::{d.dtype}, ::{d.dtype}) -- complex numbers are not ordered")
     if d.dtype == np.dtype(np.bool_):
         return (_mapreduce_all(None, _lib.MIN, d), _mapreduce_all(None, _lib.MAX, d))
     _check_nonempty(d, _lib.MAX)
@@ -511,6 +539,8 @@ def mapreducedim(f: Optional[Callable], op, d: DArray, dims, init=None) -> DArra
             return _count_dims(d, f, dims)[0]                    # sum(pred, d; dims): Bools add up as Int (Base.add_sum)
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "Bool-valued maps with dims are served for + only (count / any / all build on it)")
     src, tmp = d, None
+    if is_complex(d.dtype) and mapc not in (None, _lib.MAP_ID):
+        mapc = None                                              # f.(z) by the NVRTC kernel first, then the plain reduction
     if mapc is None:
         from ._broadcast import LocalArg, run_local
         from ._darray import darray_like
@@ -519,6 +549,10 @@ def mapreducedim(f: Optional[Callable], op, d: DArray, dims, init=None) -> DArra
         for pid, out in tmp.chunks.items():
             run_local(rt, expr, out, [LocalArg(d.chunks[pid], None, tag_of(d.dtype))])
         src, mapc = tmp, _lib.MAP_ID
+    if is_complex(src.dtype) and opc != _lib.SUM:
+        if opc in (_lib.MAX, _lib.MIN):
+            raise TypeError(f"MethodError: no method matching isless(::{src.dtype}, ::{src.dtype}) -- complex numbers are not ordered")
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"reductions of {src.dtype} values with dims are served for + only")
     rdt = _result_dtype(src.dtype, opc, mapc)
     L = src.layout
     try:
@@ -596,6 +630,9 @@ def dot(x: DArray, y: DArray):
     """``dot(x, y)`` (reference src/linalg.jl:34-46): per-chunk dot products, summed over the chunks -- one fused pass, 8 B/element."""
     if x.dims != y.dims:
         raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, f"dot: {x.dims} vs {y.dims}")
+    if is_complex(x.dtype) or is_complex(y.dtype):
+        from ._broadcast import conj
+        return _mapreduce_all(lambda a, b: conj(a) * b, _lib.SUM, x, False, (y,))     # Julia's dot conjugates its first argument
     return _mapreduce_all(lambda a, b: a * b, _lib.SUM, x, False, (y,))
 
 
@@ -605,6 +642,9 @@ def norm(x: DArray, p=2):
     nonzeros) and any other real p as ``(sum(abs(x)^p))^(1/p)`` in one fused pass (LinearAlgebra's ``normp`` additionally rescales by the
     largest magnitude against overflow; not done here)."""
     if p == 2:
+        if is_complex(x.dtype):
+            from ._broadcast import abs2
+            return np.sqrt(_mapreduce_all(abs2, _lib.SUM, x))                 # re*re + im*im, a real sum
         return np.sqrt(_mapreduce_all(abs2_fn, _lib.SUM, x))
     if p == 1:
         return _mapreduce_all(abs, _lib.SUM, x)
@@ -626,19 +666,33 @@ def abs2_fn(v):
     return v * v
 
 
+def _scalar_for(a, dtype):
+    """The scalar of ``axpy!`` / ``rmul!`` for an array of eltype T, in T (real T) or, for a complex T, in T when the scalar is complex and
+    in the component type when it is real -- so that ``z * s`` keeps Julia's Complex * Real method (``Complex(zr*s, zi*s)``, no NaN from
+    ``0 * Inf``).  A complex value with a nonzero imaginary part cannot go into a real array (Julia's ``InexactError``)."""
+    if np.iscomplexobj(a) and not is_complex(dtype):
+        z = complex(np.asarray(a)[()])
+        if z.imag != 0:
+            raise _lib.InexactError(_lib.ERR_ARG, f"InexactError: {z} cannot be converted to {np.dtype(dtype)}")
+        a = z.real
+    if is_complex(dtype) and not np.iscomplexobj(a):
+        dtype = component_dtype(dtype)
+    return np.asarray(a, dtype=dtype)[()]
+
+
 def axpy_(a, x: DArray, y: DArray) -> DArray:
     """``axpy!(a, x, y)``: y .= a .* x .+ y (reference src/linalg.jl:24-32)."""
     from ._broadcast import broadcast_into
     if x.dims != y.dims:
         raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, f"axpy!: {x.dims} vs {y.dims}")
-    s = np.asarray(a, dtype=x.dtype)[()]
+    s = _scalar_for(a, y.dtype if is_complex(y.dtype) else x.dtype)
     return broadcast_into(y, lambda u, v: s * u + v, x, y)
 
 
 def rmul_(x: DArray, a) -> DArray:
     """``rmul!(x, a)``: x .= x .* a (reference src/linalg.jl:169-176)."""
     from ._broadcast import broadcast_into
-    s = np.asarray(a, dtype=x.dtype)[()]
+    s = _scalar_for(a, x.dtype)
     return broadcast_into(x, lambda u: u * s, x)
 
 
@@ -676,6 +730,8 @@ def mean(d: DArray, dims=None, f: Optional[Callable] = None):
     cnt = int(np.prod([d.dims[r - 1] for r in region if r <= d.ndim])) if region else 1
     S = mapreducedim(f, "+", d, dims)
     out_t = np.float64 if S.dtype.kind in "iub" or S.dtype == np.float64 else np.float32
+    if is_complex(S.dtype):
+        out_t = component_dtype(S.dtype).type                                # Complex{T} ./ n: each component divided in T
     c = out_t(cnt)
     R = broadcast(lambda s: s / c, S)
     S.close()

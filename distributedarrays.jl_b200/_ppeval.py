@@ -160,6 +160,8 @@ def ppeval(f, *D, dim=None) -> DArray:
     for i, x in enumerate(D):
         if isinstance(x, SubDArray):
             raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "ppeval of a view: make it a DArray first (DArray(view))")
+        if (x.dtype if isinstance(x, DArray) else np.asarray(x).dtype).kind == "c":
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"ppeval with a complex argument ({i + 1}) is not served (no complex slice kernels)")
         if isinstance(x, DArray):
             if dim[i] <= 0:
                 raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"ppeval: DArray argument {i + 1} with dim {dim[i]} <= 0 is not served "

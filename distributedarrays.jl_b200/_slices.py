@@ -416,6 +416,8 @@ def mapslices(f, D: DArray, dims) -> DArray:
     """``mapslices(f, D; dims)`` (reference src/mapreduce.jl:191-208).  See the module docstring for the served ``f``."""
     if isinstance(D, SubDArray):
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "mapslices of a view: make it a DArray first (DArray(view))")
+    if D.dtype.kind == "c":
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"mapslices of a {D.dtype} DArray is not served (no complex slice kernels)")
     N = D.ndim
     dims = normalise_dims(dims, N)
     if N > 8:

@@ -194,6 +194,8 @@ def sort(d: DArray, sample=True, by=None, alg=None, **kwargs) -> DArray:  # noqa
         from . import _slices
         if _slices.tracing():
             return _slices.sort_of_slice(d, by, kwargs)
+    if isinstance(d, DArray) and d.dtype.kind == "c" and by is None:
+        raise TypeError(f"MethodError: no method matching isless(::{d.dtype}, ::{d.dtype}) -- complex numbers are not ordered")
     return sort_with_boundaries(d, sample, by, alg, **kwargs)[0]
 
 

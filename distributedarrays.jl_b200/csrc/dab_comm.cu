@@ -248,7 +248,8 @@ int32_t dab_mapreduce_all(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, 
         if (op == DAB_EXTREMA) return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_mapreduce_all: extrema combines through dab_reduce + dab_allgather");
         return dab_fail(ctx, DAB_ERR_ARG, "bad dtype/op");
     }
-    if ((ctx->mbox_ranks > 1 || !ctx->comm || ctx->nranks == 1) && n > 0) {
+    const bool cplx = rdt == DAB_C64 || rdt == DAB_C128;  // 8- / 16-byte complex results: ordered fold below, not the mailbox combine
+    if ((ctx->mbox_ranks > 1 || !ctx->comm || ctx->nranks == 1) && n > 0 && !cplx) {
         // fused path: ONE kernel = chunk reduce + peer-memory all-gather + ordered fold + scalar into pinned host memory
         ctx->fuse_op = op;
         int32_t st = dab_reduce(ctx, dtype, op, map, map_param, x, n, ctx->result_slot);
@@ -262,6 +263,11 @@ int32_t dab_mapreduce_all(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, 
         memcpy(out_host, &bits, dab_dtype_size(rdt));
         return DAB_OK;
     }
+    if (cplx && ctx->mbox_ranks > 1 && !ctx->comm) {
+        DAB_FLUSH(ctx);
+        return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_mapreduce_all: a complex result across %d ranks needs the NCCL communicator "
+                        "(the mailbox combine carries 8-byte results)", ctx->mbox_ranks);
+    }
     int32_t st = dab_reduce(ctx, dtype, op, map, map_param, x, n, ctx->result_slot);
     if (st != DAB_OK) return st;
     const int P = ctx->comm ? ctx->nranks : 1;
@@ -274,13 +280,13 @@ int32_t dab_mapreduce_all(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, 
     }
     DAB_CUDA(ctx, cudaMemcpyAsync(ctx->host_slot, src, (size_t)P * 16, cudaMemcpyDeviceToHost, ctx->stream));
     DAB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    unsigned char tmp[DAB_MAX_RANKS * 8];
+    unsigned char tmp[DAB_MAX_RANKS * 16];
     size_t es = dab_dtype_size(rdt);
     for (int i = 0; i < P; ++i) memcpy(tmp + (size_t)i * es, (const char*)ctx->host_slot + (size_t)i * 16, es);
-    unsigned char res[8] = {0};
+    unsigned char res[16] = {0};
     st = dab_combine_ordered(rdt, op, tmp, (size_t)P, res);
     if (st != DAB_OK) return dab_fail(ctx, st, "%s", dab_last_error(nullptr));
-    memset(out_host, 0, 8);
+    memset(out_host, 0, es > 8 ? es : 8);
     memcpy(out_host, res, es);
     return DAB_OK;
 }

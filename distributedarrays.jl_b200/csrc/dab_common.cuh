@@ -125,6 +125,8 @@ static inline size_t dab_dtype_size(int32_t dt) {
         case DAB_I32: return 4;
         case DAB_I64: return 8;
         case DAB_U8: return 1;
+        case DAB_C64: return 8;
+        case DAB_C128: return 16;
         default: return 0;
     }
 }
@@ -155,6 +157,12 @@ template <typename T>
 struct alignas(16) Pack {
     static constexpr int N = 16 / sizeof(T);
     T v[N];
+};
+
+// Complex{T} element: interleaved (re, im), aligned to its size so that one 16-byte vector carries whole elements.
+template <typename T>
+struct alignas(2 * sizeof(T)) Cplx {
+    T re, im;
 };
 
 template <typename T>

@@ -528,6 +528,19 @@ int32_t dab_fill(dab_ctx* ctx, int32_t dtype, void* x, size_t n, const void* val
         case DAB_I32: return launch_generate(ctx, (int32_t*)x, n, FillGen<int32_t>{*(const int32_t*)value});
         case DAB_I64: return launch_generate(ctx, (long long*)x, n, FillGen<long long>{*(const long long*)value});
         case DAB_U8: return launch_generate(ctx, (uint8_t*)x, n, FillGen<uint8_t>{*(const uint8_t*)value});
+        case DAB_C64:
+        case DAB_C128: {  // interleaved (re, im): one element is 8 / 16 bytes, stored with the same 16-byte vectors
+            const size_t es = dab_dtype_size(dtype);
+            DAB_REQUIRE(ctx, (uintptr_t)x % es == 0, DAB_ERR_ARG, "dab_fill: complex dtype %d needs %d-byte aligned data", dtype, (int)es);
+            if (dtype == DAB_C64) {
+                FillGen<Cplx<float>> g;
+                memcpy(&g.v, value, 8);
+                return launch_generate(ctx, (Cplx<float>*)x, n, g);
+            }
+            FillGen<Cplx<double>> g;
+            memcpy(&g.v, value, 16);
+            return launch_generate(ctx, (Cplx<double>*)x, n, g);
+        }
         default: return dab_fail(ctx, DAB_ERR_ARG, "dab_fill: bad dtype %d", dtype);
     }
 }

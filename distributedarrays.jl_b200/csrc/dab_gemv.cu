@@ -796,7 +796,63 @@ int32_t launch_transpose(dab_ctx* ctx, void* dst, size_t dst_ld, const void* src
     return DAB_OK;
 }
 
+// conj(transpose) of one box of Complex{T}: transpose_box_kernel's tile walk with 8- / 16-byte elements, the imaginary component negated
+// (its sign bit flipped, as Julia's conj) between the shared-memory tile and the store.
+template <typename T, int TR_TILE>
+__global__ void __launch_bounds__(256) adjoint_box_kernel(Cplx<T>* __restrict__ dst, size_t dst_ld, const Cplx<T>* __restrict__ src,
+                                                          size_t src_ld, size_t rows, size_t cols, unsigned tiles_r) {
+    __shared__ Cplx<T> tile[TR_TILE][TR_TILE + 1];
+    const size_t tr = blockIdx.x % tiles_r, tc = blockIdx.x / tiles_r;
+    const size_t r0 = tr * TR_TILE, c0 = tc * TR_TILE;
+    constexpr int TY = 256 / TR_TILE;
+    constexpr int NK = TR_TILE / TY;
+    const int tx = threadIdx.x & (TR_TILE - 1), ty = threadIdx.x / TR_TILE;
+    Cplx<T> v[NK];
+#pragma unroll
+    for (int q = 0; q < NK; ++q) {
+        const size_t r = r0 + tx, c = c0 + ty + q * TY;
+        v[q] = (r < rows && c < cols) ? src[r + c * src_ld] : Cplx<T>{};
+    }
+#pragma unroll
+    for (int q = 0; q < NK; ++q) tile[ty + q * TY][tx] = v[q];
+    __syncthreads();
+#pragma unroll 4
+    for (int k = ty; k < TR_TILE; k += TY) {
+        const size_t c = c0 + tx, r = r0 + k;
+        if (r < rows && c < cols) {
+            Cplx<T> z = tile[tx][k];
+            z.im = -z.im;
+            dst[c + r * dst_ld] = z;
+        }
+    }
+}
+
+template <typename T>
+int32_t launch_adjoint(dab_ctx* ctx, void* dst, size_t dst_ld, const void* src, size_t src_ld, size_t rows, size_t cols) {
+    constexpr int TR_TILE = 32;  // as dab_transpose_box for 8- and 16-byte units
+    DAB_REQUIRE(ctx, (uintptr_t)dst % sizeof(Cplx<T>) == 0 && (uintptr_t)src % sizeof(Cplx<T>) == 0, DAB_ERR_ARG,
+                "dab_adjoint_box: data must be aligned to the element size");
+    const size_t tiles_r = (rows + TR_TILE - 1) / TR_TILE, tiles_c = (cols + TR_TILE - 1) / TR_TILE;
+    DAB_REQUIRE(ctx, tiles_r * tiles_c <= 0x7fffffffull && tiles_r <= 0xffffffffull, DAB_ERR_ARG, "dab_adjoint_box: too many tiles");
+    adjoint_box_kernel<T, TR_TILE><<<(unsigned)(tiles_r * tiles_c), 256, 0, ctx->stream>>>((Cplx<T>*)dst, dst_ld, (const Cplx<T>*)src, src_ld, rows,
+                                                                                         cols, (unsigned)tiles_r);
+    DAB_LAUNCHED(ctx);
+    return DAB_OK;
+}
+
 }  // namespace
+
+extern "C" int32_t dab_adjoint_box(dab_ctx* ctx, int32_t dtype, void* dst, size_t dst_ld, const void* src, size_t src_ld, size_t rows,
+                                   size_t cols) {
+    DAB_ENTER(ctx);
+    DAB_REQUIRE(ctx, dtype == DAB_C64 || dtype == DAB_C128, DAB_ERR_UNSUPPORTED,
+                "dab_adjoint_box: dtype %d is not complex (the adjoint of a real matrix is dab_transpose_box)", dtype);
+    if (rows == 0 || cols == 0) return DAB_OK;
+    DAB_REQUIRE(ctx, dst && src, DAB_ERR_ARG, "dab_adjoint_box: null pointer");
+    DAB_REQUIRE(ctx, src_ld >= rows && dst_ld >= cols, DAB_ERR_DIM_MISMATCH, "dab_adjoint_box: leading dimension smaller than the box");
+    if (dtype == DAB_C64) return launch_adjoint<float>(ctx, dst, dst_ld, src, src_ld, rows, cols);
+    return launch_adjoint<double>(ctx, dst, dst_ld, src, src_ld, rows, cols);
+}
 
 extern "C" int32_t dab_transpose_box(dab_ctx* ctx, int32_t elem_bytes, void* dst, size_t dst_ld, const void* src, size_t src_ld, size_t rows,
                                      size_t cols) {

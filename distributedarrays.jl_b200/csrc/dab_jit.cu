@@ -183,6 +183,143 @@ DEV int jl_x_shr(int a, i64 n) {
 
 bool mentions_ext(const char* expr) { return expr && strstr(expr, "jl_x_") != nullptr; }
 
+// ComplexF32 / ComplexF64 values (jl_c64 / jl_c128: interleaved (re, im), Julia's Complex{T} layout), with Julia's definitions of the
+// operations the tracer serves on them.  Appended only to sources that use a complex type (an argument, output or value dtype, or one of
+// the names below in the expression), so every other generated kernel is byte-for-byte what it was.
+const char* kPreludeCplx = R"PRELUDE(
+struct jl_c128;
+struct __align__(8) jl_c64 {
+    float re, im;
+    jl_c64() = default;
+    DEV jl_c64(float r, float i) : re(r), im(i) {}
+    DEV jl_c64(float r) : re(r), im(0.f) {}
+    DEV jl_c64(double r) : re((float)r), im(0.f) {}
+    DEV jl_c64(int r) : re((float)r), im(0.f) {}
+    DEV jl_c64(i64 r) : re((float)r), im(0.f) {}
+    DEV jl_c64(bool r) : re(r ? 1.f : 0.f), im(0.f) {}
+    DEV explicit jl_c64(const jl_c128& z);
+};
+struct __align__(16) jl_c128 {
+    double re, im;
+    jl_c128() = default;
+    DEV jl_c128(double r, double i) : re(r), im(i) {}
+    DEV jl_c128(double r) : re(r), im(0.0) {}
+    DEV jl_c128(float r) : re((double)r), im(0.0) {}
+    DEV jl_c128(int r) : re((double)r), im(0.0) {}
+    DEV jl_c128(i64 r) : re((double)r), im(0.0) {}
+    DEV jl_c128(bool r) : re(r ? 1.0 : 0.0), im(0.0) {}
+    DEV jl_c128(const jl_c64& z) : re((double)z.re), im((double)z.im) {}
+};
+DEV jl_c64::jl_c64(const jl_c128& z) : re((float)z.re), im((float)z.im) {}
+// the 16-byte result slot of a ComplexF32 reduction: the value, then zeros
+struct __align__(16) jl_c64_slot {
+    jl_c64 v;
+    float pad[2];
+    jl_c64_slot() = default;
+    DEV jl_c64_slot(const jl_c128& z) : v(z), pad{0.f, 0.f} {}
+    DEV jl_c64_slot(bool b) : v(b), pad{0.f, 0.f} {}
+};
+DEV bool operator==(jl_c64 a, jl_c64 b) { return a.re == b.re && a.im == b.im; }
+DEV bool operator!=(jl_c64 a, jl_c64 b) { return !(a == b); }
+DEV bool operator==(jl_c128 a, jl_c128 b) { return a.re == b.re && a.im == b.im; }
+DEV bool operator!=(jl_c128 a, jl_c128 b) { return !(a == b); }
+DEV float jl_real(jl_c64 z) { return z.re; }
+DEV double jl_real(jl_c128 z) { return z.re; }
+DEV float jl_imag(jl_c64 z) { return z.im; }
+DEV double jl_imag(jl_c128 z) { return z.im; }
+DEV jl_c64 jl_conj(jl_c64 z) { return jl_c64(z.re, -z.im); }
+DEV jl_c128 jl_conj(jl_c128 z) { return jl_c128(z.re, -z.im); }
+DEV jl_c64 jl_neg(jl_c64 z) { return jl_c64(-z.re, -z.im); }
+DEV jl_c128 jl_neg(jl_c128 z) { return jl_c128(-z.re, -z.im); }
+DEV bool jl_isnan(jl_c64 z) { return z.re != z.re || z.im != z.im; }
+DEV bool jl_isnan(jl_c128 z) { return z.re != z.re || z.im != z.im; }
+DEV bool jl_isinf(jl_c64 z) { return jl_isinf(z.re) || jl_isinf(z.im); }
+DEV bool jl_isinf(jl_c128 z) { return jl_isinf(z.re) || jl_isinf(z.im); }
+DEV bool jl_isfinite(jl_c64 z) { return jl_isfinite(z.re) && jl_isfinite(z.im); }
+DEV bool jl_isfinite(jl_c128 z) { return jl_isfinite(z.re) && jl_isfinite(z.im); }
+// + - * between complex values; * is (ac - bd, ad + bc), every operation rounded separately
+#define JL_CPLX_ARITH(C, R)                                                                                        \
+DEV C jl_add(C a, C b) { return C(jl_add(a.re, b.re), jl_add(a.im, b.im)); }                                        \
+DEV C jl_sub(C a, C b) { return C(jl_sub(a.re, b.re), jl_sub(a.im, b.im)); }                                        \
+DEV C jl_mul(C a, C b) { return C(jl_sub(jl_mul(a.re, b.re), jl_mul(a.im, b.im)), jl_add(jl_mul(a.re, b.im), jl_mul(a.im, b.re))); } \
+/* mixed real / complex: Julia's specialised methods, the real operand is NOT promoted to complex first */          \
+DEV C jl_add(R x, C z) { return C(jl_add(x, z.re), z.im); }                                                         \
+DEV C jl_add(C z, R x) { return C(jl_add(z.re, x), z.im); }                                                         \
+DEV C jl_sub(R x, C z) { return C(jl_sub(x, z.re), -z.im); }                                                        \
+DEV C jl_sub(C z, R x) { return C(jl_sub(z.re, x), z.im); }                                                         \
+DEV C jl_mul(R x, C z) { return C(jl_mul(x, z.re), jl_mul(x, z.im)); }                                              \
+DEV C jl_mul(C z, R x) { return C(jl_mul(z.re, x), jl_mul(z.im, x)); }                                              \
+DEV C jl_div(C z, R x) { return C(jl_div(z.re, x), jl_div(z.im, x)); }                                              \
+DEV R jl_abs2(C z) { return jl_add(jl_mul(z.re, z.re), jl_mul(z.im, z.im)); }
+JL_CPLX_ARITH(jl_c64, float)
+JL_CPLX_ARITH(jl_c128, double)
+// ComplexF64 division: Baudin & Smith's robust algorithm with Julia's scaling of operands near the overflow / underflow thresholds
+// (halve above floatmax/2; multiply by bs = 2/eps^2 = 2^105 below 2 floatmin/eps, so that subnormal operands are brought well inside the
+// normal range and b*r cannot underflow again)
+DEV double jl_cdiv2_(double a, double b, double c, double d, double r, double t) {
+    if (r != 0.0) {
+        const double br = __dmul_rn(b, r);
+        return br != 0.0 ? __dmul_rn(__dadd_rn(a, br), t) : __dadd_rn(__dmul_rn(a, t), __dmul_rn(__dmul_rn(b, t), r));
+    }
+    return __dmul_rn(__dadd_rn(a, __dmul_rn(d, __ddiv_rn(b, c))), t);
+}
+DEV void jl_cdiv1_(double a, double b, double c, double d, double* p, double* q) {
+    const double r = __ddiv_rn(d, c), t = __ddiv_rn(1.0, __dadd_rn(c, __dmul_rn(d, r)));
+    *p = jl_cdiv2_(a, b, c, d, r, t);
+    *q = jl_cdiv2_(b, -a, c, d, r, t);
+}
+DEV jl_c128 jl_div(jl_c128 z, jl_c128 w) {
+    double a = z.re, b = z.im, c = w.re, d = w.im;
+    const double ab = fmax(fabs(a), fabs(b)), cd = fmax(fabs(c), fabs(d));
+    const double halfov = 0x1p1023, twoun = 0x1p-969, be = 0x1p105;   // floatmax/2, 2 floatmin/eps, 2/eps^2
+    double s = 1.0;
+    if (ab >= halfov) { a *= 0.5; b *= 0.5; s *= 2.0; }
+    if (cd >= halfov) { c *= 0.5; d *= 0.5; s *= 0.5; }
+    if (ab <= twoun) { a *= be; b *= be; s /= be; }
+    if (cd <= twoun) { c *= be; d *= be; s *= be; }
+    double p, q;
+    if (fabs(d) <= fabs(c)) {
+        jl_cdiv1_(a, b, c, d, &p, &q);
+    } else {
+        jl_cdiv1_(b, a, d, c, &p, &q);
+        q = -q;
+    }
+    return jl_c128(__dmul_rn(p, s), __dmul_rn(q, s));
+}
+DEV jl_c128 jl_inv(jl_c128 w) { return jl_div(jl_c128(1.0, 0.0), w); }
+// ComplexF32 / and inv: widened to ComplexF64 and rounded once, as Julia does
+DEV jl_c64 jl_div(jl_c64 z, jl_c64 w) { return jl_c64(jl_div(jl_c128(z), jl_c128(w))); }
+DEV jl_c64 jl_inv(jl_c64 w) { return jl_c64(jl_inv(jl_c128(w))); }
+DEV jl_c64 jl_div(float x, jl_c64 z) { return jl_mul(x, jl_inv(z)); }
+DEV jl_c128 jl_div(double x, jl_c128 z) { return jl_mul(x, jl_inv(z)); }
+// abs = hypot: Float32 through exact Float64 squares, Float64 with CUDA's hypot (no intermediate overflow); Inf if a component is Inf
+DEV float jl_abs(jl_c64 z) {
+    if (isinf(z.re) || isinf(z.im)) return __int_as_float(0x7f800000);   // hypot(Inf, NaN) = Inf
+    const double x = z.re, y = z.im;
+    return (float)__dsqrt_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)));
+}
+DEV double jl_abs(jl_c128 z) { return hypot(z.re, z.im); }
+// angle(z) = atan(imag z, real z); angle(x::Real) = atan(0, x); cis(x) = Complex(cos x, sin x) (libdevice, <= 2 ulp)
+DEV float jl_angle(jl_c64 z) { return atan2f(z.im, z.re); }
+DEV double jl_angle(jl_c128 z) { return atan2(z.im, z.re); }
+DEV float jl_angle(float x) { return atan2f(0.f, x); }
+DEV double jl_angle(double x) { return atan2(0.0, x); }
+DEV jl_c64 jl_cis(float x) { return jl_c64(cosf(x), sinf(x)); }
+DEV jl_c128 jl_cis(double x) { return jl_c128(cos(x), sin(x)); }
+)PRELUDE";
+
+bool is_cplx_dt(int32_t dt) { return dt == DAB_C64 || dt == DAB_C128; }
+
+bool uses_cplx(const char* expr, int32_t dt0, int nargs, const int32_t* dts) {
+    if (is_cplx_dt(dt0)) return true;
+    for (int k = 0; k < nargs; ++k)
+        if (is_cplx_dt(dts[k])) return true;
+    const char* names[] = {"jl_c64", "jl_c128", "jl_cis(", "jl_angle(", nullptr};
+    for (int i = 0; expr && names[i]; ++i)
+        if (strstr(expr, names[i])) return true;
+    return false;
+}
+
 const char* ctype_of(int32_t dt) {
     switch (dt) {
         case DAB_F32: return "float";
@@ -190,6 +327,8 @@ const char* ctype_of(int32_t dt) {
         case DAB_I32: return "int";
         case DAB_I64: return "long long";
         case DAB_U8: return "bool";
+        case DAB_C64: return "jl_c64";
+        case DAB_C128: return "jl_c128";
         default: return nullptr;
     }
 }
@@ -297,6 +436,7 @@ std::unordered_map<std::string, Compiled> g_cache;
 std::string build_source(const char* expr, int32_t out_dt, int nargs, const int32_t* dts, const bool* is_arr) {
     std::string s = kPrelude;
     if (mentions_ext(expr)) s += kPreludeExt;
+    if (uses_cplx(expr, out_dt, nargs, dts)) s += kPreludeCplx;
     s += "typedef ";
     s += ctype_of(out_dt);
     s += " OUT_T;\n";
@@ -502,6 +642,14 @@ bool mr_spec(int32_t val_dt, int32_t op, MrSpec* sp) {
             default: return false;
         }
     }
+    if (is_cplx_dt(val_dt)) {  // complex fp64 carrier; sums add componentwise in the value type inside a tile, products widen first
+        const char* out = val_dt == DAB_C64 ? "jl_c64_slot" : "jl_c128";
+        switch (op) {
+            case DAB_SUM: *sp = {vt, "jl_c128", out, "jl_add(a, b)", "jl_add(a, b)", "jl_c128(0.0, 0.0)"}; return true;
+            case DAB_PROD: *sp = {"jl_c128", "jl_c128", out, "jl_mul(a, b)", "jl_mul(a, b)", "jl_c128(1.0, 0.0)"}; return true;
+            default: return false;
+        }
+    }
     switch (op) {
         case DAB_SUM:
         case DAB_COUNT:
@@ -554,7 +702,8 @@ std::string build_mr_source(const char* expr, int32_t val_dt, int32_t op, int na
     std::string s = kPrelude;
     if (val_dt == DAB_I128 || mentions_i128(expr)) s += kPreludeI128;
     if (mentions_ext(expr)) s += kPreludeExt;
-    if (val_dt == DAB_I128) s += "#define DAB_ACC16 1\n";   // 16-byte carrier: shuffles and the result slot move four words
+    if (uses_cplx(expr, val_dt, nargs, dts)) s += kPreludeCplx;
+    if (val_dt == DAB_I128 || is_cplx_dt(val_dt)) s += "#define DAB_ACC16 1\n";   // 16-byte carrier: shuffles and the result slot move four words
     s += std::string("typedef ") + vtype_of(val_dt) + " VAL_T;\n";
     for (int k = 0; k < nargs; ++k) s += std::string("typedef ") + ctype_of(dts[k]) + " T" + std::to_string(k) + ";\n";
     s += std::string("typedef ") + sp.tile_t + " TILE_T;\ntypedef " + sp.acc_t + " ACC_T;\ntypedef " + sp.out_t + " OUT_T;\n";
@@ -701,6 +850,7 @@ int32_t dab_jit_compile_check(const char* expr, int32_t out_dtype, int32_t nargs
     for (int k = 0; k < nargs; ++k) {
         if (!ctype_of(arg_dtypes[k])) return dab_fail(nullptr, DAB_ERR_ARG, "dab_jit_compile_check: bad dtype of arg %d", k);
         is_arr[k] = arg_is_array[k] != 0;
+        if (!is_arr[k] && arg_dtypes[k] == DAB_C128) return dab_fail(nullptr, DAB_ERR_ARG, "a ComplexF64 scalar does not fit the 8-byte scalar slot of arg %d (pass complex(re, im) of two Float64 scalars)", k);
     }
     std::vector<char> cubin;
     int32_t st = compile_cubin(nullptr, build_source(expr, out_dtype, nargs, arg_dtypes, is_arr), &cubin);
@@ -724,6 +874,7 @@ int32_t dab_broadcast_expr(dab_ctx* ctx, const char* expr, int32_t out_dtype, vo
     for (int k = 0; k < nargs; ++k) {
         DAB_REQUIRE(ctx, ctype_of(arg_dtypes[k]), DAB_ERR_ARG, "dab_broadcast_expr: bad dtype of arg %d", k);
         is_arr[k] = arg_ptrs[k] != nullptr;
+        DAB_REQUIRE(ctx, is_arr[k] || arg_dtypes[k] != DAB_C128, DAB_ERR_ARG, "dab_broadcast_expr: a ComplexF64 scalar does not fit the 8-byte scalar slot of arg %d (pass complex(re, im) of two Float64 scalars)", k);
         key += std::to_string(arg_dtypes[k]) + (is_arr[k] ? "a" : "s");
     }
     key += "|";
@@ -808,6 +959,7 @@ int32_t dab_mapreduce_expr(dab_ctx* ctx, const char* expr, int32_t val_dtype, in
     for (int k = 0; k < nargs; ++k) {
         DAB_REQUIRE(ctx, ctype_of(arg_dtypes[k]), DAB_ERR_ARG, "dab_mapreduce_expr: bad dtype of arg %d", k);
         is_arr[k] = arg_ptrs[k] != nullptr;
+        DAB_REQUIRE(ctx, is_arr[k] || arg_dtypes[k] != DAB_C128, DAB_ERR_ARG, "dab_mapreduce_expr: a ComplexF64 scalar does not fit the 8-byte scalar slot of arg %d (pass complex(re, im) of two Float64 scalars)", k);
         key += std::to_string(arg_dtypes[k]) + (is_arr[k] ? "a" : "s");
         if (is_arr[k] && ((uintptr_t)arg_ptrs[k] % (4 * dab_dtype_size(arg_dtypes[k])))) vec_ok = false;
     }
@@ -878,6 +1030,7 @@ int32_t dab_jit_compile_check_reduce(const char* expr, int32_t val_dtype, int32_
     for (int k = 0; k < nargs; ++k) {
         if (!ctype_of(arg_dtypes[k])) return dab_fail(nullptr, DAB_ERR_ARG, "bad dtype of arg %d", k);
         is_arr[k] = arg_is_array[k] != 0;
+        if (!is_arr[k] && arg_dtypes[k] == DAB_C128) return dab_fail(nullptr, DAB_ERR_ARG, "a ComplexF64 scalar does not fit the 8-byte scalar slot of arg %d (pass complex(re, im) of two Float64 scalars)", k);
     }
     std::vector<char> cubin;
     int32_t st = compile_cubin(nullptr, build_mr_source(expr, val_dtype, op, nargs, arg_dtypes, is_arr, sp), &cubin,

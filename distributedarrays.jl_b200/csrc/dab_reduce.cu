@@ -52,10 +52,18 @@ struct AffineStore {
     }
 };
 
+// CTAs per SM the reduce kernel is compiled for: 8 (a 32-register budget) for the real element types; 6 (40 registers) for Complex{T},
+// whose tile tree holds two components per value and would spill at 32; 4 (64 registers) for abs of ComplexF32, which computes hypot
+// through fp64 squares.  Every choice keeps >= 1024 threads per SM, each with 4 x 16-byte loads in flight.
+template <typename T, typename Map>
+struct RdMinBlocks {
+    static constexpr int value = !is_cplx<T>::value ? 8 : (std::is_same<Map, CMapF<float, DAB_MAP_ABS>>::value ? 4 : 6);
+};
+
 // Result slot layout (16 bytes at `out`): [0..8) the result in its result dtype, [8..16) the wide accumulator (fp64 for
 // float SUM/PROD -- lets the host see the un-rounded carrier; tests use it).
 template <typename T, typename Map, typename R, typename Out, typename St>
-__global__ void __launch_bounds__(RD_THREADS, 8) reduce_kernel(const T* __restrict__ x, size_t n, size_t head, Map map,
+__global__ void __launch_bounds__(RD_THREADS, RdMinBlocks<T, Map>::value) reduce_kernel(const T* __restrict__ x, size_t n, size_t head, Map map,
                                                              typename R::A* __restrict__ partials, unsigned int* counter,
                                                              void* out, int finalize_mode, long long n_for_all, int tiles_per_cta,
                                                              FusedComm fc, St st) {
@@ -176,6 +184,11 @@ __global__ void __launch_bounds__(RD_THREADS, 8) reduce_kernel(const T* __restri
                 h[1] = 0ull;
                 __threadfence_system();
             }
+        } else if constexpr (is_cplx<Out>::value) {  // complex sum / product: rounded once to Complex{T}, [0, 2*sizeof(T)) of the slot
+            using CT = decltype(Out::re);
+            const Out res{(CT)fin.re, (CT)fin.im};
+            memset(out, 0, 16);
+            memcpy(out, &res, sizeof(Out));
         } else {  // extrema: the (min, max) pair fills the slot (8 bytes for 4-byte T, 16 for 8-byte T)
             memset(out, 0, 16);
             memcpy(out, &fin, sizeof(A));
@@ -334,6 +347,46 @@ int32_t reduce_t(dab_ctx* ctx, int32_t op, int32_t map, const void* param, const
     }
 }
 
+// Complex{T} chunks: the same kernel with Cplx<T> elements (a 16-byte load carries 2 ComplexF32 or 1 ComplexF64).
+template <typename T>
+int32_t reduce_c(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, const Cplx<T>* x, size_t n, void* out) {
+    using Z = Cplx<T>;
+    if ((uintptr_t)x % sizeof(Z))
+        return dab_fail(ctx, DAB_ERR_ARG, "dab_reduce: complex dtype %d needs %d-byte aligned data", dtype, (int)sizeof(Z));
+    switch (map) {
+        case DAB_MAP_ID:
+            if (op == DAB_SUM) return launch_reduce<Z, CMapF<T, DAB_MAP_ID>, CSumTraits<T>, Z>(ctx, x, n, {(T)0}, out, 0);
+            if (op == DAB_PROD) return launch_reduce<Z, CMapF<T, DAB_MAP_ID>, CProdTraits<T>, Z>(ctx, x, n, {(T)0}, out, 0);
+            break;
+        case DAB_MAP_NEG:
+            if (op == DAB_SUM) return launch_reduce<Z, CMapF<T, DAB_MAP_NEG>, CSumTraits<T>, Z>(ctx, x, n, {(T)0}, out, 0);
+            if (op == DAB_PROD) return launch_reduce<Z, CMapF<T, DAB_MAP_NEG>, CProdTraits<T>, Z>(ctx, x, n, {(T)0}, out, 0);
+            break;
+#define ABSMAP(FN)                                                                                                      \
+    case FN:                                                                                                            \
+        if (op == DAB_SUM) return launch_reduce<Z, CMapF<T, FN>, SumTraits<T>, T>(ctx, x, n, {(T)0}, out, 0);            \
+        if (op == DAB_MAX) return launch_reduce<Z, CMapF<T, FN>, MaxTraits<T>, T>(ctx, x, n, {(T)0}, out, 0);            \
+        if (op == DAB_MIN) return launch_reduce<Z, CMapF<T, FN>, MinTraits<T>, T>(ctx, x, n, {(T)0}, out, 0);            \
+        break;
+            ABSMAP(DAB_MAP_ABS)
+            ABSMAP(DAB_MAP_ABS2)
+#undef ABSMAP
+#define PREDMAP(FN)                                                                                                     \
+    case FN: {                                                                                                          \
+        const int mode = op == DAB_ALL ? 1 : (op == DAB_ANY ? 2 : 0);                                                   \
+        if (op == DAB_ALL || op == DAB_ANY || op == DAB_COUNT || op == DAB_SUM)                                         \
+            return launch_reduce<Z, CPredF<T, FN>, CountTraits, long long>(ctx, x, n, {(T)0}, out, mode);               \
+        break;                                                                                                          \
+    }
+            PREDMAP(DAB_MAP_NONZERO)
+            PREDMAP(DAB_MAP_ISNAN)
+#undef PREDMAP
+        default: break;
+    }
+    return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_reduce: op %d with map %d is not served for complex dtype %d (no host fallback)", op, map,
+                    dtype);
+}
+
 // The deferred dab_affine y .= a.*x .+ b and the reduction of y as ONE kernel: reads x, writes y, reduces y (8 B/element of
 // Float32 instead of 8 + 4).  Same CTA geometry, element-to-thread mapping and fold as reduce_arith<T, DAB_MAP_ID> on y.
 template <typename T>
@@ -389,6 +442,12 @@ int32_t empty_result(dab_ctx* ctx, int32_t dtype, int32_t op, void* out_dev) {
             } else if (dtype == DAB_F64) {
                 double one = 1.0;
                 memcpy(buf, &one, 8);
+            } else if (dtype == DAB_C64) {
+                const float one[2] = {1.f, 0.f};
+                memcpy(buf, one, 8);
+            } else if (dtype == DAB_C128) {
+                const double one[2] = {1.0, 0.0};
+                memcpy(buf, one, 16);
             } else {
                 long long one = 1;
                 memcpy(buf, &one, 8);
@@ -413,6 +472,16 @@ extern "C" {
 
 int32_t dab_reduce_result_dtype(int32_t dtype, int32_t op, int32_t map, int32_t* out_dtype) {
     if (!out_dtype) return DAB_ERR_ARG;
+    if (dtype == DAB_C64 || dtype == DAB_C128) {
+        const int32_t comp = dtype == DAB_C64 ? DAB_F32 : DAB_F64;
+        const bool id = map == DAB_MAP_ID || map == DAB_MAP_NEG, mag = map == DAB_MAP_ABS || map == DAB_MAP_ABS2;
+        const bool pred = map == DAB_MAP_NONZERO || map == DAB_MAP_ISNAN;
+        if (id && (op == DAB_SUM || op == DAB_PROD)) *out_dtype = dtype;
+        else if (mag && (op == DAB_SUM || op == DAB_MAX || op == DAB_MIN)) *out_dtype = comp;
+        else if (pred && (op == DAB_SUM || op == DAB_COUNT || op == DAB_ALL || op == DAB_ANY)) *out_dtype = DAB_I64;
+        else return dab_fail(nullptr, DAB_ERR_UNSUPPORTED, "op %d with map %d is not served for complex dtype %d", op, map, dtype);
+        return DAB_OK;
+    }
     const bool pred = map >= DAB_MAP_EQ;  // predicate maps yield Bool: sum/count/all/any -> Int64
     switch (op) {
         case DAB_SUM:
@@ -446,6 +515,15 @@ int32_t dab_reduce(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, const v
     DAB_FLUSH(ctx);
     DAB_REQUIRE(ctx, out_dev && (x || n == 0), DAB_ERR_ARG, "dab_reduce: null pointer");
     DAB_REQUIRE(ctx, op >= DAB_SUM && op <= DAB_EXTREMA, DAB_ERR_ARG, "dab_reduce: bad op %d", op);
+    if (dtype == DAB_C64 || dtype == DAB_C128) {
+        int32_t rdt;
+        if (dab_reduce_result_dtype(dtype, op, map, &rdt) != DAB_OK)
+            return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_reduce: op %d with map %d is not served for complex dtype %d (no host fallback)", op,
+                            map, dtype);
+        if (n == 0) return empty_result(ctx, map == DAB_MAP_ABS || map == DAB_MAP_ABS2 ? rdt : dtype, op, out_dev);
+        if (dtype == DAB_C64) return reduce_c<float>(ctx, dtype, op, map, (const Cplx<float>*)x, n, out_dev);
+        return reduce_c<double>(ctx, dtype, op, map, (const Cplx<double>*)x, n, out_dev);
+    }
     if (n == 0) return empty_result(ctx, dtype, op, out_dev);
     // predicate maps turn the value into a Bool: only SUM/ALL/ANY/COUNT make sense
     switch (dtype) {
@@ -556,6 +634,46 @@ int32_t dab_combine_ordered(int32_t rdt, int32_t op, const void* partials, size_
                 case DAB_MAX: FOLD(uint8_t, a > b ? a : b)
                 case DAB_MIN: FOLD(uint8_t, a < b ? a : b)
                 default: break;
+            }
+            break;
+        case DAB_C64:
+            if (op == DAB_SUM || op == DAB_PROD) {  // Float32 arithmetic, each operation rounded (volatile: no wider intermediates)
+                const float* v = (const float*)partials;
+                volatile float re = v[0], im = v[1];
+                for (size_t i = 1; i < p; ++i) {
+                    const float br = v[2 * i], bi = v[2 * i + 1];
+                    if (op == DAB_SUM) {
+                        re = re + br;
+                        im = im + bi;
+                    } else {
+                        volatile float rr = re * br, ii = im * bi, ri = re * bi, ir = im * br;
+                        re = rr - ii;
+                        im = ri + ir;
+                    }
+                }
+                ((float*)out)[0] = re;
+                ((float*)out)[1] = im;
+                return DAB_OK;
+            }
+            break;
+        case DAB_C128:
+            if (op == DAB_SUM || op == DAB_PROD) {
+                const double* v = (const double*)partials;
+                volatile double re = v[0], im = v[1];
+                for (size_t i = 1; i < p; ++i) {
+                    const double br = v[2 * i], bi = v[2 * i + 1];
+                    if (op == DAB_SUM) {
+                        re = re + br;
+                        im = im + bi;
+                    } else {
+                        volatile double rr = re * br, ii = im * bi, ri = re * bi, ir = im * br;
+                        re = rr - ii;
+                        im = ri + ir;
+                    }
+                }
+                ((double*)out)[0] = re;
+                ((double*)out)[1] = im;
+                return DAB_OK;
             }
             break;
         default: break;

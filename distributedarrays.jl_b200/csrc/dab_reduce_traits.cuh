@@ -205,5 +205,74 @@ __device__ __forceinline__ typename R::A block_reduce(typename R::A acc, typenam
     return acc;  // valid in thread 0
 }
 
+// ---- complex element types: Cplx<T> (ComplexF32 / ComplexF64) -------------------------------------------------------------------
+template <typename Z>
+struct is_cplx : std::false_type {};
+template <typename T>
+struct is_cplx<Cplx<T>> : std::true_type {};
+
+// Julia's complex + is componentwise; * is (ac - bd, ad + bc) with every operation rounded separately (never contracted).
+template <typename T>
+__device__ __forceinline__ Cplx<T> cadd(Cplx<T> a, Cplx<T> b) { return {jl::add(a.re, b.re), jl::add(a.im, b.im)}; }
+template <typename T>
+__device__ __forceinline__ Cplx<T> cmul(Cplx<T> a, Cplx<T> b) {
+    return {jl::sub(jl::mul(a.re, b.re), jl::mul(a.im, b.im)), jl::add(jl::mul(a.re, b.im), jl::mul(a.im, b.re))};
+}
+template <typename T>
+__device__ __forceinline__ Cplx<double> cwiden(Cplx<T> v) { return {(double)v.re, (double)v.im}; }
+
+// sum: each component added in T inside a tile step (like the real kernel's register tree), carried in fp64
+template <typename T>
+struct CSumTraits {
+    using A = Cplx<double>;
+    using W = Cplx<T>;
+    __device__ static __forceinline__ A identity() { return {0.0, 0.0}; }
+    __device__ static __forceinline__ W pre(W v) { return v; }
+    __device__ static __forceinline__ W tile(W a, W b) { return cadd(a, b); }
+    __device__ static __forceinline__ A lift(W v) { return cwiden(v); }
+    __device__ static __forceinline__ A comb(A a, A b) { return cadd(a, b); }
+};
+// product: every value widened to the complex fp64 carrier first, rounded once to T at the end
+template <typename T>
+struct CProdTraits {
+    using A = Cplx<double>;
+    using W = Cplx<double>;
+    __device__ static __forceinline__ A identity() { return {1.0, 0.0}; }
+    __device__ static __forceinline__ W pre(Cplx<T> v) { return cwiden(v); }
+    __device__ static __forceinline__ W tile(W a, W b) { return cmul(a, b); }
+    __device__ static __forceinline__ A lift(W v) { return v; }
+    __device__ static __forceinline__ A comb(A a, A b) { return cmul(a, b); }
+};
+
+// abs(z) = hypot(re, im): Float32 through exact fp64 squares (one rounding for the sum, one for the root, one back to Float32), Inf when
+// either component is infinite even if the other is NaN; Float64 with CUDA's hypot (<= 2 ulp, no intermediate overflow, same Inf rule)
+__device__ __forceinline__ float cabs(Cplx<float> z) {
+    if (isinf(z.re) || isinf(z.im)) return __int_as_float(0x7f800000);  // hypot(Inf, NaN) = Inf, as Julia's hypot
+    const double x = z.re, y = z.im;
+    return (float)__dsqrt_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)));
+}
+__device__ __forceinline__ double cabs(Cplx<double> z) { return hypot(z.re, z.im); }
+
+template <typename T, int FN>
+struct CMapF {  // Complex{T} -> Complex{T} (identity, -z) or T (abs, abs2)
+    using V = typename std::conditional<FN == DAB_MAP_ABS || FN == DAB_MAP_ABS2, T, Cplx<T>>::type;
+    T p;
+    __device__ __forceinline__ V operator()(Cplx<T> z) const {
+        if constexpr (FN == DAB_MAP_ABS) return cabs(z);
+        else if constexpr (FN == DAB_MAP_ABS2) return jl::add(jl::mul(z.re, z.re), jl::mul(z.im, z.im));
+        else if constexpr (FN == DAB_MAP_NEG) return Cplx<T>{jl::neg(z.re), jl::neg(z.im)};
+        else return z;
+    }
+};
+template <typename T, int FN>
+struct CPredF {  // Complex{T} -> Bool: !iszero(z), isnan(z)
+    using V = int;
+    T p;
+    __device__ __forceinline__ V operator()(Cplx<T> z) const {
+        if constexpr (FN == DAB_MAP_ISNAN) return (z.re != z.re) || (z.im != z.im);
+        else return (z.re != (T)0) || (z.im != (T)0);  // NONZERO
+    }
+};
+
 
 }  // namespace

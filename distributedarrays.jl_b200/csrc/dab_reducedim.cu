@@ -470,6 +470,14 @@ extern "C" {
 
 int32_t dab_reducedim(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, const void* x, size_t inner, size_t reduce, size_t outer,
                       void* out, int32_t accumulate) {
+    if (dtype == DAB_C64 || dtype == DAB_C128) {
+        // Complex{T}: Julia's + is componentwise, so a complex SUM over (inner, reduce, outer) IS the real SUM over (2 inner, reduce, outer)
+        // of the interleaved components.  No other op or map is served for the complex codes.
+        if (op != DAB_SUM || map != DAB_MAP_ID)
+            return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_reducedim: op %d with map %d is not served for complex dtype %d (%s; SUM with MAP_ID is)",
+                            op, map, dtype, dtype == DAB_C64 ? "ComplexF32" : "ComplexF64");
+        return dab_reducedim(ctx, dtype == DAB_C64 ? DAB_F32 : DAB_F64, op, map, x, 2 * inner, reduce, outer, out, accumulate);
+    }
     DAB_ENTER(ctx);
     const size_t nout = inner * outer;
     if (nout == 0) return DAB_OK;

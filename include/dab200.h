@@ -66,7 +66,16 @@ enum {
 /* ---- element types ----------------------------------------------------------------- */
 enum { DAB_F32 = 0, DAB_F64 = 1, DAB_I32 = 2, DAB_I64 = 3, DAB_U8 = 4 /* Bool */,
        DAB_I128 = 5 /* Int128: ONLY as the value type of dab_mapreduce_expr (f widens, e.g. x -> Int128(x)^2; test/darray.jl:286-294);
-                       there are no arrays of it.  Its result fills the whole 16-byte slot (two's complement, little endian). */ };
+                       there are no arrays of it.  Its result fills the whole 16-byte slot (two's complement, little endian). */,
+       DAB_C64 = 6 /* ComplexF32 */, DAB_C128 = 7 /* ComplexF64 */ };
+/* Complex element types are stored interleaved (re, im), as Julia's Complex{T}.  Entry points that accept them:
+ *   dab_fill, dab_reduce / dab_reduce_host / dab_mapreduce_all / dab_reduce_result_dtype / dab_combine_ordered (see there),
+ *   dab_broadcast_expr / dab_mapreduce_expr and their compile checks (argument, output and value types), dab_adjoint_box, and the
+ *   byte movers that take an element size (dab_copy_box, dab_gather_box, dab_transpose_box with 8 / 16 bytes, dab_h2d, ...).
+ * dab_reducedim takes them for SUM with MAP_ID only and runs it as the real SUM over (2*inner, reduce, outer) of the components (Julia's
+ * complex + is componentwise); any other op or map returns DAB_ERR_UNSUPPORTED naming the dtype.  drand of a complex array calls
+ * dab_rand_u01 on the real view of 2n components at global offset 2g.  Every other entry point returns DAB_ERR_UNSUPPORTED (or
+ * DAB_ERR_ARG) for them, naming the dtype. */
 
 /* ---- reduce operators  (op argument of Base.mapreduce; src/mapreduce.jl:31) ----------- */
 enum {
@@ -215,13 +224,21 @@ int32_t dab_jit_compile_check_reduce(const char* expr, int32_t val_dtype, int32_
  * predicate maps, else NULL.  n == 0: SUM->0, PROD->1, ALL->1, ANY/COUNT->0, MAX/MIN -> DAB_ERR_EMPTY. */
 int32_t dab_reduce(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, const void* map_param, const void* x, size_t n,
                    void* out_dev);
+/* Complex dtypes (C64 / C128; x 8- resp. 16-byte aligned):
+ *   SUM / PROD with MAP_ID or MAP_NEG -> complex result: it fills [0, 2*sizeof(T)) of the slot, the rest is zero (no separate carrier).
+ *     Sums add each component in T over a 16-byte tile step and carry them in fp64 (Julia's complex + is componentwise); products
+ *     multiply (ac - bd, ad + bc) with every operation rounded separately, in a complex fp64 carrier, rounded once to T.
+ *   SUM / MAX / MIN with MAP_ABS2 (re*re + im*im) or MAP_ABS (hypot) -> real result of the component type, laid out as for that type.
+ *   COUNT / ANY / ALL with MAP_NONZERO or MAP_ISNAN (either component NaN) -> Int64.
+ *   Anything else (MAX / MIN / EXTREMA with MAP_ID, PROD of a map, other maps) -> DAB_ERR_UNSUPPORTED. */
 /* Same, then copies the 16-byte result slot to out_host and syncs (== remotecall_fetch, src/mapreduce.jl:31). */
 int32_t dab_reduce_host(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, const void* map_param, const void* x,
                         size_t n, void* out_host);
 /* result dtype of dab_reduce for (dtype, op, map). */
 int32_t dab_reduce_result_dtype(int32_t dtype, int32_t op, int32_t map, int32_t* out_dtype);
 /* Caller-side combine  reduce(op, results)  (src/mapreduce.jl:26,34): P < 16 so a plain LEFT FOLD in
- * procs(d) order, in the result dtype (Float32 partials fold in Float32).  Host arrays. */
+ * procs(d) order, in the result dtype (Float32 partials fold in Float32; ComplexF32 partials fold in Float32 arithmetic,
+ * componentwise for SUM and as (ac - bd, ad + bc) for PROD).  Host arrays. */
 int32_t dab_combine_ordered(int32_t result_dtype, int32_t op, const void* partials_host, size_t p, void* out_host);
 
 /* ==== dimensional reduction K5 / K6 =====================================================
@@ -278,6 +295,10 @@ int32_t dab_gemm(dab_ctx* ctx, int32_t dtype, int32_t transA, size_t m, size_t n
  * shared-memory tile, so the fetched block is never materialised untransposed.  elem_bytes in {1,2,4,8,16}. */
 int32_t dab_transpose_box(dab_ctx* ctx, int32_t elem_bytes, void* dst, size_t dst_ld, const void* src, size_t src_ld, size_t rows,
                           size_t cols);
+/* dst[j + i*dst_ld] = conj(src[i + j*src_ld]): the per-piece body of copy(::Adjoint{<:Complex,<:DArray}) -- dab_transpose_box's tile
+ * scheme with the imaginary component negated on the way through (sign bit flipped: NaN payloads kept).  src may be a PEER pointer.
+ * dtype DAB_C64 or DAB_C128 (the adjoint of a real matrix is its transpose: dab_transpose_box). */
+int32_t dab_adjoint_box(dab_ctx* ctx, int32_t dtype, void* dst, size_t dst_ld, const void* src, size_t src_ld, size_t rows, size_t cols);
 
 /* ==== sort K11 (widening row f4; HBM-bound integer work) ===================================
  * out = sort(in) for one chunk: the  sort(lp; kwargs...)  of sample_n_setup_ref (src/sort.jl:8) and the
@@ -364,7 +385,9 @@ int32_t dab_group_end(dab_ctx* ctx);
 int32_t dab_send(dab_ctx* ctx, const void* send_dev, size_t nbytes, int32_t peer);
 int32_t dab_recv(dab_ctx* ctx, void* recv_dev, size_t nbytes, int32_t peer);
 /* sum(d) in one call: chunk reduce (dab_reduce) -> allgather of the P chunk results -> ordered left
- * fold (dab_combine_ordered) -> host scalar.  Exactly src/mapreduce.jl:29-35. */
+ * fold (dab_combine_ordered) -> host scalar.  Exactly src/mapreduce.jl:29-35.  out_host: 8 bytes, 16 for a ComplexF64 result.
+ * Complex results always take the dab_reduce + allgather + dab_combine_ordered path (the fused mailbox combine below carries
+ * 8-byte results). */
 int32_t dab_mapreduce_all(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, const void* map_param, const void* x,
                           size_t n, void* out_host);
 

@@ -19,6 +19,7 @@
 #   src/mapreduce.jl:34  reduce(op, results)              (DArray method below)                      dab_mapreduce_all
 #   src/linalg.jl:95-97,141 localpart(A)*xj, localpart(A)'*xj   Base.:*                                 dab_gemv
 #   src/linalg.jl:1-17   transpose!(lp, rp)               LinearAlgebra.transpose! / adjoint!        dab_transpose_box
+#   src/linalg.jl:1-17   adjoint!(lp, rp), complex T      LinearAlgebra.adjoint!                     dab_adjoint_box
 #   src/sort.jl:8,22,61  sort(localpart(d)), sort!(lp)    Base.sort / Base.sort!                     dab_sort
 #   src/sort.jl:8,22,61  sort(localpart(d); by = f)       sort_by (keys = f.(a) by broadcast)        dab_sort_by_key
 #   src/mapreduce.jl:205 mapslices(f, localpart(y), dims) mapslices_sort / svdvals_batched       dab_sort_slices / dab_svdvals_batched
@@ -54,6 +55,7 @@ end
 
 dab_dtype(::Type{Float32}) = Int32(0); dab_dtype(::Type{Float64}) = Int32(1)
 dab_dtype(::Type{Int32}) = Int32(2);   dab_dtype(::Type{Int64}) = Int32(3); dab_dtype(::Type{Bool}) = Int32(4)
+dab_dtype(::Type{ComplexF32}) = Int32(6); dab_dtype(::Type{ComplexF64}) = Int32(7)   # interleaved (re, im), Julia's own layout
 
 # ---- the chunk type ------------------------------------------------------------------------------------------------------------
 mutable struct B200Array{T,N} <: AbstractArray{T,N}
@@ -171,7 +173,9 @@ end
 # ---- reductions --------------------------------------------------------------------------------------------------------------------
 const OPS = Dict{Any,Int32}(Base.add_sum => 0, (+) => 0, Base.mul_prod => 1, (*) => 1, max => 2, min => 3)
 const MAPS = Dict{Any,Int32}(identity => 0, abs => 1, abs2 => 2, (-) => 3)
-result_type(::Type{T}, op) where {T} = (T <: AbstractFloat || op >= 2) ? T : Int64          # add_sum / mul_prod widen Int32
+result_type(::Type{T}, op, f = identity) where {T} = (T <: AbstractFloat || op >= 2) ? T : Int64          # add_sum / mul_prod widen Int32
+# Complex{T}: sum / prod of z or -z are Complex{T}; abs / abs2 maps give T (the 16-byte slot holds re, im)
+result_type(::Type{Complex{T}}, op, f = identity) where {T<:Union{Float32,Float64}} = (f === abs || f === abs2) ? T : Complex{T}
 
 function Base.mapreduce(f, op, a::B200Array{T}; dims = :, init = nothing) where {T}         # src/mapreduce.jl:23,31,64
     haskey(OPS, op) && haskey(MAPS, f) || error("DArrayB200: mapreduce($f, $op) is not served by a kernel (no host fallback)")
@@ -179,7 +183,7 @@ function Base.mapreduce(f, op, a::B200Array{T}; dims = :, init = nothing) where 
     out = zeros(UInt64, 2)
     check(ccall((:dab_reduce_host, libdab), Int32, (Ptr{Cvoid}, Int32, Int32, Int32, Ptr{Cvoid}, Ptr{Cvoid}, Csize_t, Ptr{Cvoid}),
                 ctx(), dab_dtype(T), OPS[op], MAPS[f], C_NULL, a.ptr, length(a), out), ctx())
-    reinterpret(result_type(T, OPS[op]), out)[1]
+    reinterpret(result_type(T, OPS[op], f), out)[1]
 end
 Base.reduce(op, a::B200Array; kw...) = mapreduce(identity, op, a; kw...)
 
@@ -187,7 +191,7 @@ function mapreducedim(f, op, a::B200Array{T,N}, dims, init) where {T,N}
     region = Tuple(dims)
     all(d -> d >= 1, region) || throw(ArgumentError("region dimension(s) must be ≥ 1, got $dims"))
     rdims = ntuple(i -> i in region ? 1 : size(a, i), N)
-    R = B200Array{result_type(T, OPS[op]),N}(undef, rdims)
+    R = B200Array{result_type(T, OPS[op], f),N}(undef, rdims)   # complex T: SUM of z only (dab_reducedim refuses other ops / maps)
     init === nothing || fill!(R, init)
     # one (inner, reduce, outer) pass per maximal run of reduced dims; single leading / single trailing run shown
     k = findfirst(i -> !(i in region), 1:N)
@@ -210,7 +214,7 @@ function Base._mapreduce(f, op, ::IndexCartesian, d::DArray{T,N,<:B200Array}) wh
             a = localpart(d); out = zeros(UInt64, 2)
             check(ccall((:dab_mapreduce_all, libdab), Int32, (Ptr{Cvoid}, Int32, Int32, Int32, Ptr{Cvoid}, Ptr{Cvoid}, Csize_t, Ptr{Cvoid}),
                         ctx(), dab_dtype(T), OPS[op], MAPS[f], C_NULL, a.ptr, length(a), out), ctx())
-            reinterpret(result_type(T, OPS[op]), out)[1]
+            reinterpret(result_type(T, OPS[op], f), out)[1]
         end
     end
     first(results)        # every worker already holds the left-folded result
@@ -258,6 +262,13 @@ function LinearAlgebra.transpose!(dst::B200Array{T,2}, src::B200Array{T,2}) wher
     dst
 end
 LinearAlgebra.adjoint!(dst::B200Array{T,2}, src::B200Array{T,2}) where {T<:Real} = transpose!(dst, src)
+# adjoint!(lp, rp) of copy(::Adjoint{<:Complex,<:DArray})  (src/linalg.jl:1-17): transpose and conjugate in one pass
+function LinearAlgebra.adjoint!(dst::B200Array{T,2}, src::B200Array{T,2}) where {T<:Union{ComplexF32,ComplexF64}}
+    rows, cols = size(src)
+    check(ccall((:dab_adjoint_box, libdab), Int32, (Ptr{Cvoid}, Int32, Ptr{Cvoid}, Csize_t, Ptr{Cvoid}, Csize_t, Csize_t, Csize_t),
+                ctx(), dab_dtype(T), dst.ptr, cols, src.ptr, rows, rows, cols), ctx())
+    dst
+end
 
 # sort(localpart(d)) / sort!(lp_sorting)  (src/sort.jl:8, 22, 61); keys only, isless order
 function Base.sort!(a::B200Array{T,1}; kw...) where {T}

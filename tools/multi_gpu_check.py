@@ -140,6 +140,18 @@ def main():
     rt.barrier()
     log("ok: A*x, A'*x, mul!, copy(transpose(A)) across ranks")
 
+    # ---- ComplexF64: sum (allgather + ordered complex fold, every rank) and copy(adjoint(A)) with pieces pulled from peers
+    Z = dab.drand((203, 157), dtype=np.complex128, seed=41)
+    hz = dab.to_array(Z)
+    k = 2.0 ** 24
+    ex = complex(np.round(hz.real * k).astype(np.int64).sum() / k, np.round(hz.imag * k).astype(np.int64).sum() / k)
+    s = complex(dab.sum(Z))
+    assert abs(s.real - ex.real) <= 1e-13 * ex.real and abs(s.imag - ex.imag) <= 1e-13 * ex.imag, (s, ex)
+    H = dab.to_array(dab.adjoint(Z).copy())
+    assert np.array_equal(H.real, hz.T.real) and np.array_equal(H.imag, -hz.T.imag)
+    rt.barrier()
+    log("ok: ComplexF64 sum and copy(adjoint(A)) across ranks")
+
     # ---- samplesort across ranks: pieces travel by grouped NCCL send/recv; layout and boundaries equal the oracle's
     for T in (np.int64, np.float64):
         rs = np.random.default_rng(77)
