@@ -169,12 +169,20 @@ class Expr:
     def __pow__(self, p):
         if is_ctag(self.jt) or is_ctag(Expr.wrap(p).jt):
             raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "^ with a complex operand is not served (complex transcendental functions)")
-        if isinstance(p, (int, np.integer)) and not isinstance(p, (bool, np.bool_)) and 1 <= int(p) <= 3:  # Base.literal_pow: x^2 == x*x, x^3 == x*x*x
-            r = self
-            for _ in range(int(p) - 1):
-                r = binop("mul", r, self)
+        if isinstance(p, (int, np.integer)) and not isinstance(p, (bool, np.bool_)) and -2 <= int(p) <= 3:
+            # Base.literal_pow: x^0 == one(x), x^2 == x*x, x^3 == x*x*x, x^-1 == inv(x), x^-2 == (i = inv(x); i*i)
+            p = int(p)
+            if p == 0:
+                return convert(Expr.wrap(1), self.jt)
+            b = unop("inv", self) if p < 0 else self
+            r = b
+            for _ in range(abs(p) - 1):
+                r = binop("mul", r, b)
             return r
         pe = Expr.wrap(p)
+        if self.jt == "f32" and pe.jt in ("bool", "i32", "i64"):
+            # ^(x::Float32, n::Integer) (base/math.jl): n == -2 and n == 3 in Float32, otherwise power_by_squaring in Float64
+            return Expr("m_powi", (self, convert(pe, "i64")), "f32")
         if promote(self.jt, pe.jt)[0] != "f":
             # Julia's integer ^ is power_by_squaring and throws DomainError for negative exponents: no kernel serves it
             raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "integer ^ integer is not served by the GPU backend")
@@ -229,9 +237,28 @@ def _cbinop(op: str, a: Expr, b: Expr) -> Expr:
     return Expr(op, (a, b), jt)
 
 
+def _exact_int(e: Expr, ft: str) -> bool:
+    """An Int64 constant that ``ft`` holds exactly: comparing it after the conversion is the exact comparison."""
+    return e.op == "const" and float(_NPT[ft].type(e.val)) == e.val
+
+
 def binop(op: str, a: Expr, b: Expr) -> Expr:
     if is_ctag(a.jt) or is_ctag(b.jt):
         return _cbinop(op, a, b)
+    # base/bool.jl: Bool * x and Bool + x with a float x are not promotion (Julia's "strong zero" and signed-zero rules)
+    if op in ("mul", "add") and "bool" in (a.jt, b.jt) and (a.jt[0] == "f" or b.jt[0] == "f"):
+        c, x = (a, b) if a.jt == "bool" else (b, a)
+        if op == "mul":   # *(x::Bool, y::AbstractFloat) = ifelse(x, y, copysign(zero(y), y))
+            return Expr("ifelse", (c, x, Expr("m_copysign", (convert(Expr.wrap(0), x.jt), x), x.jt)), x.jt)
+        # +(x::Bool, y::AbstractFloat) = ifelse(x, oneunit(y) + y, y)
+        return Expr("ifelse", (c, binop("add", convert(Expr.wrap(1), x.jt), x), x), x.jt)
+    if a.jt == b.jt == "bool" and op == "mul":
+        op = "and"                                        # *(x::Bool, y::Bool) = x & y
+    # base/float.jl: ==, <, <= between Int64 and a float type compare the values exactly (no rounding of the Int64)
+    if op in _CMP and {a.jt, b.jt} in ({"i64", "f32"}, {"i64", "f64"}):
+        i, f = (a, b) if a.jt == "i64" else (b, a)
+        if not _exact_int(i, f.jt):
+            return Expr("m_" + op, (a, b), "bool")
     jt = promote(a.jt, b.jt)
     if op == "div" and jt[0] != "f":
         jt = "f64"  # Int / Int -> Float64
@@ -277,9 +304,9 @@ def unop(op: str, a: Expr) -> Expr:
         a = convert(a, "f64")  # sqrt(::Int) -> Float64
     if op in ("isnan", "isinf", "isfinite"):
         return Expr(op, (a,), "bool")
-    if op in ("x_trunc", "x_round") and a.jt == "bool":
-        a = convert(a, "i64")
-    if a.jt == "bool" and op in ("neg", "abs", "abs2"):
+    if a.jt == "bool" and op in ("abs", "abs2", "x_trunc", "x_round"):
+        return a                                          # abs(x::Bool) = x, abs2 = x & x, round / trunc of an Integer = x
+    if a.jt == "bool" and op == "neg":
         a = convert(a, "i64")
     return Expr(op, (a,), a.jt)
 
@@ -510,6 +537,10 @@ def trace(f: Callable, arg_tags: Sequence[str]) -> Expr:
 _FN2 = {"add": "jl_add", "sub": "jl_sub", "mul": "jl_mul", "div": "jl_div", "rem": "jl_rem", "mod": "jl_mod", "idiv": "jl_idiv",
         "max": "jl_max", "min": "jl_min", "pow": "jl_pow", "and": "jl_and", "or": "jl_or", "xor": "jl_xor", "lt": "jl_lt", "le": "jl_le",
         "gt": "jl_gt", "ge": "jl_ge", "eq": "jl_eq", "ne": "jl_ne", "x_shl": "jl_x_shl", "x_shr": "jl_x_shr"}
+# Julia methods that are not "promote, then operate": the jl_m_* helpers of dab_jit.cu's kPreludeMethods block (appended only to
+# sources that use one): copysign for Bool * float, the exact Int64-vs-float comparisons, Float32 ^ Integer
+_FN2.update({"m_copysign": "jl_m_copysign", "m_powi": "jl_m_powi"})
+_FN2.update({"m_" + c: "jl_m_" + c for c in ("lt", "le", "gt", "ge", "eq", "ne")})
 
 
 def _lit(jt: str, v) -> str:

@@ -183,6 +183,62 @@ DEV int jl_x_shr(int a, i64 n) {
 
 bool mentions_ext(const char* expr) { return expr && strstr(expr, "jl_x_") != nullptr; }
 
+// Julia methods that are not "promote both operands, then operate" (the tracer spells them jl_m_*).  Appended only to sources that use
+// one, so every other generated kernel stays byte-identical.
+//   copysign        -- Bool * x = ifelse(b, x, copysign(zero(x), x)) for a float x (base/bool.jl)
+//   eq ne lt le ... -- Int64 against Float32 / Float64 compares the values exactly (base/float.jl), without rounding the Int64
+//   powi            -- ^(x::Float32, n::Integer) (base/math.jl): n == -2 is inv(x)^2 and n == 3 is x*x*x in Float32, otherwise
+//                      Float32(power_by_squaring(Float64(x), n)), from inv(Float64(x)) when n < 0; the magnitude of a typemin n is 2^63
+const char* kPreludeMethods = R"PRELUDE(
+DEV float jl_m_copysign(float a, float b) { return copysignf(a, b); }
+DEV double jl_m_copysign(double a, double b) { return copysign(a, b); }
+// three-way comparison of an Int64 with a Float64 value: -1, 0, 1, or 2 when f is NaN
+DEV int jl_m_cmp(i64 a, double f) {
+    if (f != f) return 2;
+    if (f >= 0x1p63) return -1;
+    if (f < -0x1p63) return 1;
+    const double t = trunc(f);
+    const i64 ti = (i64)t;                          // exact: |t| < 2^63 or t == -2^63
+    if (a != ti) return a < ti ? -1 : 1;
+    const double fr = f - t;                        // exact
+    return fr > 0.0 ? -1 : (fr < 0.0 ? 1 : 0);
+}
+DEV int jl_m_cmp(double f, i64 a) { const int c = jl_m_cmp(a, f); return c == 2 ? 2 : -c; }
+DEV int jl_m_cmp(i64 a, float f) { return jl_m_cmp(a, (double)f); }
+DEV int jl_m_cmp(float f, i64 a) { return jl_m_cmp((double)f, a); }
+template <typename A, typename B> DEV bool jl_m_eq(A a, B b) { return jl_m_cmp(a, b) == 0; }
+template <typename A, typename B> DEV bool jl_m_ne(A a, B b) { return jl_m_cmp(a, b) != 0; }
+template <typename A, typename B> DEV bool jl_m_lt(A a, B b) { return jl_m_cmp(a, b) == -1; }
+template <typename A, typename B> DEV bool jl_m_le(A a, B b) { const int c = jl_m_cmp(a, b); return c == -1 || c == 0; }
+template <typename A, typename B> DEV bool jl_m_gt(A a, B b) { return jl_m_cmp(a, b) == 1; }
+template <typename A, typename B> DEV bool jl_m_ge(A a, B b) { const int c = jl_m_cmp(a, b); return c == 1 || c == 0; }
+// Base.power_by_squaring(x, p) for p >= 0, operation by operation (a shift by the full width gives 0)
+DEV double jl_m_pbs(double x, u64 p) {
+    if (p == 1) return x;
+    if (p == 0) return 1.0;
+    if (p == 2) return __dmul_rn(x, x);
+    int t = __ffsll((long long)p);                  // trailing_zeros(p) + 1
+    p = t >= 64 ? 0 : p >> t;
+    while (--t > 0) x = __dmul_rn(x, x);
+    double y = x;
+    while (p > 0) {
+        t = __ffsll((long long)p);
+        p = t >= 64 ? 0 : p >> t;
+        while (--t >= 0) x = __dmul_rn(x, x);
+        y = __dmul_rn(y, x);
+    }
+    return y;
+}
+DEV float jl_m_powi(float x, i64 n) {
+    if (n == -2) { const float i = __fdiv_rn(1.0f, x); return __fmul_rn(i, i); }
+    if (n == 3) return __fmul_rn(__fmul_rn(x, x), x);
+    if (n < 0) return (float)jl_m_pbs(__ddiv_rn(1.0, (double)x), 0ull - (u64)n);
+    return (float)jl_m_pbs((double)x, (u64)n);
+}
+)PRELUDE";
+
+bool mentions_methods(const char* expr) { return expr && strstr(expr, "jl_m_") != nullptr; }
+
 // ComplexF32 / ComplexF64 values (jl_c64 / jl_c128: interleaved (re, im), Julia's Complex{T} layout), with Julia's definitions of the
 // operations the tracer serves on them.  Appended only to sources that use a complex type (an argument, output or value dtype, or one of
 // the names below in the expression), so every other generated kernel is byte-for-byte what it was.
@@ -436,6 +492,7 @@ std::unordered_map<std::string, Compiled> g_cache;
 std::string build_source(const char* expr, int32_t out_dt, int nargs, const int32_t* dts, const bool* is_arr) {
     std::string s = kPrelude;
     if (mentions_ext(expr)) s += kPreludeExt;
+    if (mentions_methods(expr)) s += kPreludeMethods;
     if (uses_cplx(expr, out_dt, nargs, dts)) s += kPreludeCplx;
     s += "typedef ";
     s += ctype_of(out_dt);
@@ -702,6 +759,7 @@ std::string build_mr_source(const char* expr, int32_t val_dt, int32_t op, int na
     std::string s = kPrelude;
     if (val_dt == DAB_I128 || mentions_i128(expr)) s += kPreludeI128;
     if (mentions_ext(expr)) s += kPreludeExt;
+    if (mentions_methods(expr)) s += kPreludeMethods;
     if (uses_cplx(expr, val_dt, nargs, dts)) s += kPreludeCplx;
     if (val_dt == DAB_I128 || is_cplx_dt(val_dt)) s += "#define DAB_ACC16 1\n";   // 16-byte carrier: shuffles and the result slot move four words
     s += std::string("typedef ") + vtype_of(val_dt) + " VAL_T;\n";

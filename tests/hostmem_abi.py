@@ -30,6 +30,8 @@ import ctypes as C
 
 import numpy as np
 
+import julia_scalar as jl
+
 F32, F64, I32, I64, U8 = range(5)
 _NP = {F32: np.dtype(np.float32), F64: np.dtype(np.float64), I32: np.dtype(np.int32), I64: np.dtype(np.int64), U8: np.dtype(np.uint8)}
 SIGN64 = np.uint64(0x8000000000000000)
@@ -202,17 +204,17 @@ class HostMemABI:
         return 0
 
     # -- the elementwise entry points the REAL run_local chooses between (so its routing, its stride tables and collapse_dims run on CPU)
-    _UN = {0: lambda v: v, 1: np.abs, 2: lambda v: v * v, 3: np.negative, 4: np.sqrt, 5: lambda v: v.dtype.type(1) / v, 6: np.floor, 7: np.ceil,
-           8: np.sign}
+    # Julia's methods (tests/julia_scalar.py), not NumPy's stand-ins: np.maximum / np.sign differ at -0.0, and ÷ through Float64 is wrong for
+    # large Int64 values and zero divisors
+    _UN = {0: lambda v: v, 1: lambda v: jl.vun("abs", v), 2: lambda v: jl.vun("abs2", v), 3: lambda v: jl.vun("neg", v),
+           4: lambda v: jl.vun("sqrt", v), 5: lambda v: jl.vun("inv", v), 6: lambda v: jl.vun("floor", v), 7: lambda v: jl.vun("ceil", v),
+           8: lambda v: jl.vun("sign", v)}
+    _BINOPS = ("add", "sub", "mul", "div", "rem", "max", "min", "mod", "idiv", "and", "or", "xor")
 
     @staticmethod
     def _bin(op, a, b):
         a, b = np.asarray(a), np.asarray(b)
-        with np.errstate(all="ignore"):
-            if op == 8:                                             # IDIV: Julia div, truncated
-                return np.trunc(a.astype(np.float64) / b.astype(np.float64)).astype(a.dtype)
-            return {0: np.add, 1: np.subtract, 2: np.multiply, 3: np.divide, 4: np.fmod, 5: np.maximum, 6: np.minimum, 7: np.mod,
-                    9: np.bitwise_and, 10: np.bitwise_or, 11: np.bitwise_xor}[op](a, b)
+        return jl.vbin(HostMemABI._BINOPS[op], a, b).astype(a.dtype)
 
     def dab_affine(self, ctx, dtype, y, x, a, b, n):
         dt = _NP[int(dtype)]
@@ -604,22 +606,26 @@ def eval_expr(e, args):
     with np.errstate(all="ignore"):
         if e.op == "ifelse":
             return np.where(a[0], a[1], a[2])
-        two = {"add": np.add, "sub": np.subtract, "mul": np.multiply, "div": np.divide, "rem": np.fmod, "mod": np.mod,
-               "max": np.maximum, "min": np.minimum, "pow": np.power, "and": np.bitwise_and, "or": np.bitwise_or, "xor": np.bitwise_xor,
-               "lt": np.less, "le": np.less_equal, "gt": np.greater, "ge": np.greater_equal, "eq": np.equal, "ne": np.not_equal}
-        if e.op in two:
-            r = two[e.op](a[0], a[1])
+        if e.op in ("add", "sub", "mul", "div", "rem", "mod", "max", "min", "and", "or", "xor", "lt", "le", "gt", "ge", "eq", "ne", "idiv"):
+            r = jl.vbin(e.op, a[0], a[1])
+        elif e.op == "pow":
+            r = np.power(a[0], a[1])
+        elif e.op == "m_copysign":
+            r = np.copysign(a[0], a[1])
+        elif e.op in ("m_eq", "m_ne", "m_lt", "m_le", "m_gt", "m_ge"):
+            r = jl.vcmp_exact(e.op[2:], a[0], a[1])
+        elif e.op == "m_powi":
+            r = np.vectorize(lambda x, n: jl.pow_f32_int(np.float32(x), int(n)), otypes=[np.float32])(a[0], a[1])
         elif e.op in ("x_shl", "x_shr"):
             r = np.vectorize(lambda x, n: jl_shift(int(x), int(n), 8 * npt[e.jt].itemsize, e.op == "x_shl"), otypes=[npt[e.jt]])(a[0], a[1])
-        elif e.op == "idiv":
-            r = np.trunc(np.asarray(a[0], dtype=np.float64) / np.asarray(a[1], dtype=np.float64))
+        elif e.op in ("abs", "abs2", "neg", "sign", "inv", "floor", "ceil", "x_trunc", "x_round"):
+            r = jl.vun(e.op.removeprefix("x_"), np.asarray(a[0]))
         else:
-            one = {"neg": np.negative, "abs": np.abs, "abs2": lambda x: x * x, "sqrt": np.sqrt, "inv": lambda x: x.dtype.type(1) / x, "floor": np.floor,
-                   "ceil": np.ceil, "sign": np.sign, "sin": np.sin, "cos": np.cos, "tan": np.tan, "exp": np.exp, "log": np.log,
+            one = {"sqrt": np.sqrt, "sin": np.sin, "cos": np.cos, "tan": np.tan, "exp": np.exp, "log": np.log,
                    "tanh": np.tanh, "isnan": np.isnan, "isinf": np.isinf, "isfinite": np.isfinite, "exp2": np.exp2, "log2": np.log2,
                    "log10": np.log10, "sinh": np.sinh, "cosh": np.cosh, "atan": np.arctan, "asin": np.arcsin, "acos": np.arccos,
                    "expm1": np.expm1, "log1p": np.log1p, "cbrt": np.cbrt, "x_asinh": np.arcsinh, "x_acosh": np.arccosh, "x_atanh": np.arctanh,
-                   "x_exp10": lambda x: np.power(x.dtype.type(10), x), "x_trunc": np.trunc, "x_round": np.rint,
+                   "x_exp10": lambda x: np.power(x.dtype.type(10), x),
                    "x_sinpi": lambda x: np.sin(np.pi * np.where(x > 0.5, 1.0 - x.astype(np.float64), x.astype(np.float64))),
                    "x_cospi": lambda x: np.where(x > 0.25, np.sin(np.pi * (0.5 - x.astype(np.float64))), np.cos(np.pi * x.astype(np.float64)))}
             if e.op in ("x_erf", "x_erfc", "x_erfinv", "x_erfcinv", "x_erfcx", "x_gamma", "x_loggamma"):
