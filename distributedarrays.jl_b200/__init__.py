@@ -6,7 +6,8 @@ loader shim).  The public names mirror DistributedArrays.jl's for this path: ``D
 (``map_inplace``), broadcast (``broadcast`` / ``broadcast_into``), ``reduce``, ``mapreduce``, ``sum``, ``prod``,
 ``maximum``, ``minimum``, ``all``, ``any``, ``count``, ``extrema``, ``mapslices`` (with ``sort``, ``svdvals``, ``eigvals``, reductions,
 elementwise and constant slice functions), ``ppeval`` (batched slice products ``ppeval(operator.matmul, A, B)``, ``eigvals`` of symmetric
-slices, and every ``mapslices`` slice function), ``Array(d)`` (``to_array``), range ``getindex``.
+slices, and every ``mapslices`` slice function), ``cumsum`` / ``cumprod`` / ``accumulate`` and their ``!`` forms
+(``cumsum_`` ...), ``Array(d)`` (``to_array``), range ``getindex``.
 
 Everything computes on the GPU through ``csrc/libdab200.so`` (C ABI: ``include/dab200.h``).  There is no CPU fallback:
 importing works anywhere, but the first op without the built extension or without an H100 raises.
@@ -28,6 +29,7 @@ from ._mapreduce import (all, any, axpy_, count, dot, extrema, isequal, mapreduc
                          prod, reduce, rmul_, sum)
 from ._linalg import Adjoint, Transpose, adjoint, copy_transposed, lmul_diag, matmat, matmul, mul_, mul_mat_, rmul_diag, transpose
 from ._sort import sort, sort_with_boundaries
+from ._scan import accumulate, accumulate_, cumprod, cumprod_, cumsum, cumsum_
 from ._slices import eigvals, mapslices, svdvals
 from ._ppeval import ppeval
 from .runtime import Runtime, init, myid, nworkers, runtime, workers

@@ -99,6 +99,9 @@ _SIGS = {
     "dab_reduce_result_dtype": (_i32, [_i32, _i32, _i32, C.POINTER(_i32)]),
     "dab_combine_ordered": (_i32, [_i32, _i32, _vp, _sz, _vp]),
     "dab_reducedim": (_i32, [_vp, _i32, _i32, _i32, _vp, _sz, _sz, _sz, _vp, _i32]),
+    "dab_scan": (_i32, [_vp, _i32, _i32, _i32, _vp, _sz, _sz, _sz, _vp, _vp]),
+    "dab_scan_totals": (_i32, [_vp, _i32, _i32, _i32, _vp, _sz, _sz, _sz, _vp]),
+    "dab_scan_carrier_dtype": (_i32, [_i32, _i32, _i32, C.POINTER(_i32)]),
     "dab_copy_box": (_i32, [_vp, _i32, _vp, C.POINTER(_sz), C.POINTER(_sz), _vp, C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz)]),
     "dab_gather_box": (_i32, [_vp, _i32, _i32, _vp, C.POINTER(C.c_longlong), _pvp, _vp, C.POINTER(C.c_longlong), _pvp, C.POINTER(_sz)]),
     "dab_gemv": (_i32, [_vp, _i32, _i32, _vp, _sz, _sz, _vp, _vp]),

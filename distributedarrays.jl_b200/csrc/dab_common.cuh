@@ -55,6 +55,12 @@ struct dab_ctx {
     cudaEvent_t stage_ev[2];
     void* sort_host;        // pinned: split-point staging of dab_sorted_split
     unsigned long long sort_epoch;  // one per digit pass ever launched: tags the look-back words so the scratch is never re-cleared
+    void* scan_dev;         // scan: tile ticket counter + look-back words (dab_scan.cu), zeroed once per allocation
+    size_t scan_dev_bytes;
+    unsigned long long scan_epoch;    // one per flat scan launch: tags its look-back words
+    unsigned long long scan_tickets;  // tickets drawn so far from the counter in scan_dev
+    void* scan_scratch;     // scan: segment totals of the split strided path
+    size_t scan_scratch_bytes;
     long long opt_combine_timeout_ms;  // dab_set_option("combine_timeout_ms"): how long the fused combine waits for a peer (default 120 s)
     long long opt_gemm_kc;  // dab_set_option("gemm_kc"): k extent summed inside tensor memory before a partial tile is drained (default 64)
     int opt_gemm_rawhi;     // dab_set_option("gemm_rawhi"): 1 = raw fp32 tile as the tf32 "hi" operand (hardware truncation), 0 = RN split

@@ -162,6 +162,8 @@ int32_t dab_shutdown(dab_ctx* ctx) {
     cudaFree(ctx->gather_slots);
     if (ctx->dim_scratch) cudaFree(ctx->dim_scratch);
     if (ctx->sort_dev) cudaFree(ctx->sort_dev);
+    if (ctx->scan_dev) cudaFree(ctx->scan_dev);
+    if (ctx->scan_scratch) cudaFree(ctx->scan_scratch);
     if (ctx->sort_host) cudaFreeHost(ctx->sort_host);
     for (int b = 0; b < 2; ++b)
         if (ctx->stage[b]) {

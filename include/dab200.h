@@ -252,6 +252,34 @@ int32_t dab_combine_ordered(int32_t result_dtype, int32_t op, const void* partia
 int32_t dab_reducedim(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, const void* x, size_t inner, size_t reduce,
                       size_t outer, void* out, int32_t accumulate);
 
+/* ==== scans K17: accumulate! / cumsum! / cumprod! =========================================
+ * Replaces Base's accumulate!(op, B, A; dims, init) (base/accumulate.jl: _accumulate!, accumulate_pairwise / the per-fibre loop
+ * with reduce_first) on one chunk collapsed to the column-major shape (inner, len, outer) around dims:
+ *   y[i + inner*(r + len*o)] = c[k] (op) x[i + inner*(len*o)] (op) ... (op) x[i + inner*(r + len*o)],  k = i + inner*o,
+ * where c is the carry slab: inner*outer values in the CARRIER type (below), the exclusive prefix contributed by init and by earlier
+ * chunks along dims.  carry == NULL: no prefix, the first output of every fibre is reduce_first(op, x) (converted to out_dtype).
+ * Served (in_dtype, op, out_dtype), op in SUM PROD MAX MIN (Julia's + * max min: NaN-propagating, max(-0.0, 0.0) = 0.0):
+ *   F32 / F64 / I64 -> the same type;  I32: SUM / PROD -> I64 (cumsum / cumprod: add_sum / mul_prod widen) or I32 (accumulate(+ / *):
+ *   wraps at 32 bits), MAX / MIN -> I32;  U8 (Bool): SUM -> I64, PROD -> U8 (AND), MAX / MIN -> U8 (OR / AND).
+ *   Anything else returns DAB_ERR_UNSUPPORTED.
+ * Carriers: F64 for float SUM / PROD (each output rounded once from the fp64 prefix), I64 for integer and Bool SUM / PROD (an I32
+ * result keeps the low 32 bits), the element type for MAX / MIN (dab_scan_carrier_dtype).  Float results are not bit-identical to
+ * Julia's sequential fold: the parallel order differs, and Float32 prefixes run in fp64 (DESIGN.md section 7).
+ * inner == 1: one single-pass kernel with a decoupled look-back across tiles; inner > 1: threads along inner walk len, split into
+ * segments (one extra read) when inner*outer cannot fill the GPU.  The 16-byte loads / stores need x / y aligned to 16 bytes (the host
+ * runtime's chunks are 256-byte aligned); a misaligned base is served for the whole call with coalesced element loads / stores -- the
+ * same results, without a head peel.  x == y (in place) is allowed when in and out elements have the same
+ * size; other overlaps are not.  Asynchronous on the ctx stream. */
+int32_t dab_scan(dab_ctx* ctx, int32_t in_dtype, int32_t op, int32_t out_dtype, const void* x, size_t inner, size_t len, size_t outer,
+                 const void* carry, void* y);
+/* totals[k] = x[i + inner*(len*o)] (op) ... (op) x[i + inner*(len - 1 + len*o)] in the carrier type, k = i + inner*o (the identity of op
+ * when len == 0): the chunk totals that the host folds, in grid order along dims, into the carries of the later chunks.  Same
+ * (in_dtype, op, out_dtype) table and kernels as dab_scan, storing only the totals. */
+int32_t dab_scan_totals(dab_ctx* ctx, int32_t in_dtype, int32_t op, int32_t out_dtype, const void* x, size_t inner, size_t len, size_t outer,
+                        void* totals);
+/* carrier dtype of dab_scan for (in_dtype, op, out_dtype); DAB_ERR_UNSUPPORTED when the triple is not served.  Host only. */
+int32_t dab_scan_carrier_dtype(int32_t in_dtype, int32_t op, int32_t out_dtype, int32_t* carrier_dtype);
+
 /* ==== slab / halo copy K8 ===============================================================
  * Replaces the owner-side  localpart(d)[idxs...]  + serialise + TCP + a[idxs...] = ...  of
  * setindex!(::Array, ::SubDArray, ...) (src/darray.jl:798-820), chunk() (:458) and the non-local

@@ -24,6 +24,7 @@
 #   src/sort.jl:8,22,61  sort(localpart(d); by = f)       sort_by (keys = f.(a) by broadcast)        dab_sort_by_key
 #   src/mapreduce.jl:205 mapslices(f, localpart(y), dims) mapslices_sort / svdvals_batched       dab_sort_slices / dab_svdvals_batched
 #   src/mapreduce.jl:315 _ppeval(f, localparts...; dim)   matmul_batched / eigvals_sym_batched  dab_matmul_batched / dab_eigvals_sym_batched
+#   (no reference method)  accumulate!(op, lp, lp; dims)   Base.accumulate! (cumsum! / cumprod!)   dab_scan
 module DArrayB200
 
 using Distributed, DistributedArrays, LinearAlgebra
@@ -203,6 +204,26 @@ function mapreducedim(f, op, a::B200Array{T,N}, dims, init) where {T,N}
     R
 end
 Base.mapreducedim!(f, op, R::B200Array, A::B200Array) = (copyto!(R, mapreduce(f, op, A; dims = findall(size(R) .!= size(A)))); R)  # src/mapreduce.jl:77
+
+# ---- scans: accumulate!(op, B, A; dims, init) on one chunk (base/accumulate.jl), ONE dab_scan launch ---------------------------------------------
+# op in + * max min (add_sum / mul_prod reach here as + / * through cumsum! / cumprod!); eltype(B) must be the result type of dab_scan's table.
+# init enters as the carry slab: inner*outer copies of init in the carrier type (dab_scan_carrier_dtype).  The cross-chunk carry of a DArray
+# whose dims is split is the host runtime's job (distributedarrays.jl_b200/_scan.py); this method serves one chunk.
+const SCAN_OPS = Dict{Any,Int32}(+ => 0, Base.add_sum => 0, * => 1, Base.mul_prod => 1, max => 2, min => 3)
+carrier_type(code::Int32, ::Type{T}) where {T} = code == Int32(1) ? Float64 : code == Int32(3) ? Int64 : T
+function Base.accumulate!(op, B::B200Array{R,N}, A::B200Array{T,N}; dims::Integer, init = nothing) where {R,T,N}
+    haskey(SCAN_OPS, op) || error("DArrayB200: accumulate!($op) is not served by a kernel (no host fallback)")
+    dims > 0 || throw(ArgumentError("dims must be a positive integer"))
+    axes(B) == axes(A) || throw(DimensionMismatch("shape of B must match A"))
+    dims > N && return copyto!(B, A)
+    c = Ref{Int32}(0)
+    check(ccall((:dab_scan_carrier_dtype, libdab), Int32, (Int32, Int32, Int32, Ref{Int32}), dab_dtype(T), SCAN_OPS[op], dab_dtype(R), c))
+    inner, len, outer = prod(size(A)[1:dims-1]), size(A, dims), prod(size(A)[dims+1:end])
+    carry = init === nothing ? nothing : fill!(B200Array{carrier_type(c[], T),1}(undef, (inner * outer,)), init)
+    check(ccall((:dab_scan, libdab), Int32, (Ptr{Cvoid}, Int32, Int32, Int32, Ptr{Cvoid}, Csize_t, Csize_t, Csize_t, Ptr{Cvoid}, Ptr{Cvoid}),
+                ctx(), dab_dtype(T), SCAN_OPS[op], dab_dtype(R), A.ptr, inner, len, outer, carry === nothing ? C_NULL : carry.ptr, B.ptr), ctx())
+    B
+end
 
 # ---- the combine seam: sum(d::DArray{T,N,<:B200Array}) in ONE call per worker ----------------------------------------------------------
 # replaces  results = asyncmap(procs(d)) do p; remotecall_fetch(...) end;  reduce(op, results)   (src/mapreduce.jl:29-35):
