@@ -7,7 +7,8 @@ loader shim).  The public names mirror DistributedArrays.jl's for this path: ``D
 ``maximum``, ``minimum``, ``all``, ``any``, ``count``, ``extrema``, ``mapslices`` (with ``sort``, ``svdvals``, ``eigvals``, reductions,
 elementwise and constant slice functions), ``ppeval`` (batched slice products ``ppeval(operator.matmul, A, B)``, ``eigvals`` of symmetric
 slices, and every ``mapslices`` slice function), ``cumsum`` / ``cumprod`` / ``accumulate`` and their ``!`` forms
-(``cumsum_`` ...), ``Array(d)`` (``to_array``), range ``getindex``.
+(``cumsum_`` ...), ``Array(d)`` (``to_array``), range ``getindex``; sparse DArrays (``distribute`` of a scipy.sparse matrix: CSC
+localparts, ``nnz``, ``A*x`` / ``A'*x`` / ``mul!``).
 
 Everything computes on the GPU through ``csrc/libdab200.so`` (C ABI: ``include/dab200.h``).  There is no CPU fallback:
 importing works anywhere, but the first op without the built extension or without an H100 raises.
@@ -32,6 +33,7 @@ from ._sort import sort, sort_with_boundaries
 from ._scan import accumulate, accumulate_, cumprod, cumprod_, cumsum, cumsum_
 from ._slices import eigvals, mapslices, svdvals
 from ._ppeval import ppeval
+from ._sparse import SparseChunk, SparseDArray
 from .runtime import Runtime, init, myid, nworkers, runtime, workers
 
 __all__ = [n for n in dir() if not n.startswith("_")]

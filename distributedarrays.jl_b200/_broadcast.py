@@ -110,6 +110,9 @@ class Expr:
             return Expr("const", (), "f32", float(v))
         if isinstance(v, (float, np.floating)):
             return Expr("const", (), "f64", float(v))  # Julia literal 1.5 is Float64
+        from ._sparse import SparseDArray, refuse
+        if isinstance(v, SparseDArray):
+            refuse("broadcast / map")
         raise TypeError(f"cannot use {type(v).__name__} inside a broadcast kernel")
 
     def _bin(self, op, other, swap=False):

@@ -601,7 +601,11 @@ def _mk_from_parts(rt, layout, by_pid):
 def distribute(A: np.ndarray, procs: Optional[Sequence[int]] = None, dist: Optional[Sequence[int]] = None,
                like: Optional[DArray] = None, rt: Optional[Runtime] = None) -> DArray:
     """``distribute(A; procs, dist)`` / ``distribute(A, DA)`` (reference src/darray.jl:544-570): every rank uploads the
-    slices ``A[idxs...]`` of its own workers (H2D), nothing else moves."""
+    slices ``A[idxs...]`` of its own workers (H2D), nothing else moves.  A host sparse matrix (``.tocsc()``) gives a sparse DArray
+    (``_sparse.distribute_sparse``)."""
+    if hasattr(A, "tocsc"):
+        from ._sparse import distribute_sparse
+        return distribute_sparse(A, procs, dist, like, rt)
     A = np.asarray(A)
     rt = rt or (like.rt if like is not None else runtime())
     dab_dtype(A.dtype)
@@ -740,7 +744,12 @@ def makelocal(d: DArray, J: Sequence[Range], pid: Optional[int] = None) -> B200A
 
 
 def to_array(d: DArray) -> np.ndarray:
-    """``Array(d)`` (src/darray.jl:574-582): gather every chunk into a host array (collective; on every rank)."""
+    """``Array(d)`` (src/darray.jl:574-582): gather every chunk into a host array (collective; on every rank).  A sparse DArray is
+    densified (``Array(d)`` of sparse localparts)."""
+    if not isinstance(d, DArray):
+        from ._sparse import SparseDArray, to_array as sparse_to_array
+        if isinstance(d, SparseDArray):
+            return sparse_to_array(d)
     a = np.empty(d.dims, dtype=d.dtype, order="F")
     mine = {pid: ch.to_numpy() for pid, ch in d.chunks.items()}
     for part in d.rt.allgather_object(mine):
@@ -760,6 +769,12 @@ def copyto(dest: DArray, src: np.ndarray) -> DArray:
         if tuple(src.dims) != dest.dims:
             raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, f"DArray has size {dest.dims} but the source has {tuple(src.dims)}")
         return broadcast_into(dest, lambda x: x, src)
+    if not isinstance(dest, DArray):
+        from ._sparse import refuse
+        refuse("copyto!")
+    if hasattr(src, "tocsc"):                                  # a host sparse matrix: copyto!(D, Matrix(S)) (ext/SparseArraysExt.jl:16)
+        from ._sparse import host_dense
+        src = host_dense(src)
     src = np.asarray(src)
     if tuple(src.shape) != dest.dims:
         raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, f"DArray has size {dest.dims} but array has {src.shape}")
@@ -774,6 +789,10 @@ def similar(d: DArray, dtype=None, dims=None) -> DArray:
     """``similar(d[, T[, dims]])`` (src/darray.jl:240-243): ``DArray(I -> Array{T}(undef, ...), dims, procs(d))`` -- uninitialised,
     on ``procs(d)`` with the DEFAULT distribution for those workers (a custom ``dist`` of ``d`` is not inherited, exactly as in the
     reference)."""
+    if not isinstance(d, DArray):
+        from ._sparse import SparseDArray, refuse
+        if isinstance(d, SparseDArray):
+            refuse("similar")
     dt = np.dtype(dtype) if dtype is not None else d.dtype
     return darray(lambda I: B200Array.empty(d.rt, shape_of(I), dt), d.dims if dims is None else dims, procs(d), dtype=dt, rt=d.rt)
 

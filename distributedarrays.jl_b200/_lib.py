@@ -105,6 +105,8 @@ _SIGS = {
     "dab_copy_box": (_i32, [_vp, _i32, _vp, C.POINTER(_sz), C.POINTER(_sz), _vp, C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz)]),
     "dab_gather_box": (_i32, [_vp, _i32, _i32, _vp, C.POINTER(C.c_longlong), _pvp, _vp, C.POINTER(C.c_longlong), _pvp, C.POINTER(_sz)]),
     "dab_gemv": (_i32, [_vp, _i32, _i32, _vp, _sz, _sz, _vp, _vp]),
+    "dab_spmv": (_i32, [_vp, _i32, _sz, _sz, _vp, _vp, _vp, _vp, _vp]),
+    "dab_csc_to_csr": (_i32, [_vp, _i32, _sz, _sz, _sz, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dab_gemm": (_i32, [_vp, _i32, _i32, _sz, _sz, _sz, _vp, _sz, _vp, _sz, _vp, _sz]),
     "dab_transpose_box": (_i32, [_vp, _i32, _vp, _sz, _vp, _sz, _sz, _sz]),
     "dab_adjoint_box": (_i32, [_vp, _i32, _vp, _sz, _vp, _sz, _sz, _sz]),

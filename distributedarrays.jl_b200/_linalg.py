@@ -6,6 +6,8 @@ Mirrors the reference's ``src/linalg.jl``:
 * ``mul!(y::DVector, A::DMatrix, x, a, b)`` and the Adjoint/Transpose forms (:78-167),
   ``A*x``, ``A'*x``, ``transpose(A)*x`` (:280-284, 293-301)                               -> K9 ``dab_gemv`` + the same partial
   exchange as mapreducedim_between (NCCL send/recv to the owner of each y chunk)
+* the same ``mul!`` / ``A*x`` / ``A'*x`` with SparseMatrixCSC chunks (``_sparse.SparseDArray``)                   -> K18 ``dab_spmv``
+  (A*x on the row-major copy K19 ``dab_csc_to_csr`` builds once per chunk), same exchange and fold
 * ``lmul!(D::Diagonal, DA)`` / ``rmul!(DA, D::Diagonal)`` (:169-187)                      -> fused broadcast with extrusion
 
 * ``mul!(C::DMatrix, A::DMatrix, B::AbstractMatrix, a, b)`` and the Adjoint/Transpose forms, ``A*B``, ``A'*B`` (:189-311)
@@ -21,6 +23,7 @@ import numpy as np
 
 from . import _lib
 from ._darray import B200Array, DArray, SubDArray, dab_dtype, darray
+from ._sparse import SparseDArray, refuse
 from .layout import make_layout, rlen, shape_of
 from .runtime import Runtime, close_remote_reads, exchange_stacks, fence, grouped_exchange, open_remote_reads
 
@@ -66,7 +69,7 @@ def adjoint(D: DArray) -> Adjoint:
 def _refuse_complex(what: str, *xs):
     """Complex matrix products (GEMV / GEMM) have no kernel yet: refuse on the host, before any allocation or launch."""
     for x in xs:
-        dt = x.parent.dtype if isinstance(x, Transpose) else (x.dtype if isinstance(x, (DArray, SubDArray)) else np.asarray(x).dtype)
+        dt = x.parent.dtype if isinstance(x, Transpose) else (x.dtype if isinstance(x, (DArray, SubDArray, SparseDArray)) else np.asarray(x).dtype)
         if np.dtype(dt).kind == "c":
             raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what} with element type {np.dtype(dt)} is not served (no complex GEMV / GEMM kernel)")
 
@@ -78,6 +81,8 @@ def copy_transposed(W: Transpose) -> DArray:
     Per result chunk: every intersecting source piece is pulled (peer loads when it lives on another GPU) and written transposed
     by one kernel -- the fetched block is never materialised untransposed."""
     D = W.parent
+    if isinstance(D, SparseDArray):
+        refuse("copy(transpose(A))")
     rt = D.rt
     R = darray(lambda I: B200Array.empty(rt, shape_of(I), D.dtype), W.dims, procs=list(D.layout.pids), dtype=D.dtype, rt=rt)
     fenced = open_remote_reads(rt, [D], "host")
@@ -139,6 +144,21 @@ def _unwrap(A) -> Tuple[DArray, bool]:
     return A, False
 
 
+def _refuse_sparse_matmat(M):
+    if isinstance(M, SparseDArray):
+        refuse("the product with a matrix (sparse x dense-matrix, SpMM)")
+
+
+def _gemv_tile(rt: Runtime, code: int, trans: bool, ch: B200Array, x_ptr: int, r_ptr: int):
+    """``R[i,j] = localpart(A)*xj`` / ``localpart(A)'*xj`` of a dense chunk: K9."""
+    _lib.call("dab_gemv", rt.ctx, code, 1 if trans else 0, C.c_void_p(ch.ptr), ch.shape[0], ch.shape[1], C.c_void_p(x_ptr), C.c_void_p(r_ptr))
+
+
+def _spmv_tile(rt: Runtime, code: int, trans: bool, ch, x_ptr: int, r_ptr: int):
+    """The same tile product of a SparseMatrixCSC chunk: K18 (SparseArrays' loops, bit for bit)."""
+    ch.matvec(trans, x_ptr, r_ptr)
+
+
 def _x_block(rt: Runtime, x, lo: int, hi: int, dtype: np.dtype) -> B200Array:
     """``convert(localtype(x), x[lo:hi])`` on this rank's GPU: host vectors are sliced and uploaded, DVectors halo-fetched."""
     n = hi - lo + 1
@@ -161,7 +181,10 @@ def mul_(y: DArray, A: Union[DArray, Transpose], x, alpha=1, beta=0) -> DArray:
     differ, ArgumentError when y's cuts do not match the matrix cuts along the kept dim."""
     _refuse_complex("mul!", y, A, x)
     M, trans = _unwrap(A)
+    if isinstance(y, SparseDArray):
+        refuse("mul! into it")
     if isinstance(x, (DArray, np.ndarray)) and len(np.shape(x) if not isinstance(x, DArray) else x.dims) == 2:
+        _refuse_sparse_matmat(M)
         return mul_mat_(y, A, x, alpha, beta)
     if M.ndim != 2 or y.ndim != 1:
         raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, "mul!: y must be a DVector and A a DMatrix")
@@ -182,6 +205,7 @@ def mul_(y: DArray, A: Union[DArray, Transpose], x, alpha=1, beta=0) -> DArray:
     isz, code = dt.itemsize, dab_dtype(dt)
     ypids = y.layout.pids
     remote_x = open_remote_reads(rt, [x] if isinstance(x, DArray) else [], "device")
+    tile_product = _spmv_tile if isinstance(M, SparseDArray) else _gemv_tile     # chosen by the chunk type, as localpart(A)*xj dispatches
 
     def tile_pid(i, j):                                    # procs(A)[i,j]  /  procs(A)[j,i]
         return L.pids[(j + i * g0) if trans else (i + j * g0)]
@@ -216,8 +240,7 @@ def mul_(y: DArray, A: Union[DArray, Transpose], x, alpha=1, beta=0) -> DArray:
                     puts.append((peers[orank] + st.bank + st.tables[orank][i] + j * plen * isz, rptr, plen * isz))
                 else:
                     sends[(i, j)] = rptr
-            _lib.call("dab_gemv", rt.ctx, code, 1 if trans else 0, C.c_void_p(ch.ptr), ch.shape[0], ch.shape[1], C.c_void_p(xblocks[j].ptr),
-                      C.c_void_p(rptr))
+            tile_product(rt, code, trans, ch, xblocks[j].ptr, rptr)
     # ---- ship the tile results to the owner of y's chunk i (the fetch(rij) of :113-115)
     if st.use_arena:
         for dst, src, nb in puts:                          # one-sided puts over NVLink into the consumer's arena bank
@@ -256,6 +279,7 @@ def matmul(A: Union[DArray, Transpose], x) -> DArray:
     M, trans = _unwrap(A)
     xnd = len(x.dims) if isinstance(x, DArray) else np.ndim(x)
     if xnd == 2:
+        _refuse_sparse_matmat(M)
         return matmat(A, x)
     if xnd != 1:
         raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, "A*x: x must be a vector or a matrix")
@@ -327,6 +351,9 @@ def mul_mat_(Cd: DArray, A: Union[DArray, Transpose], B, alpha=1, beta=0) -> DAr
     cuts of C's first dimension differ from A's."""
     _refuse_complex("mul!", Cd, A, B)
     M, trans = _unwrap(A)
+    _refuse_sparse_matmat(M)
+    if isinstance(Cd, SparseDArray) or isinstance(B, SparseDArray):
+        refuse("mul! of matrices")
     if M.ndim != 2 or Cd.ndim != 2:
         raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, "mul!: C and A must be DMatrices")
     rd, cd = (1, 0) if trans else (0, 1)
@@ -416,6 +443,7 @@ def matmat(A: Union[DArray, Transpose], B) -> DArray:
     here as a one-column grid (what ``distribute`` of a matrix no wider than tall gives on these workers)."""
     _refuse_complex("A*B", A, B)
     M, trans = _unwrap(A)
+    _refuse_sparse_matmat(M)
     if M.ndim != 2:
         raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, "A must be a DMatrix")
     bdt = B.dtype if isinstance(B, DArray) else np.asarray(B).dtype

@@ -402,7 +402,11 @@ def count(d: DArray, f: Optional[Callable] = None, dims=None):
 
 def nnz(d: DArray) -> int:
     """``nnz(A::DArray)`` (reference ext/SparseArraysExt.jl:7-12: the per-worker ``nnz(localpart)`` summed).  Chunks are dense here, so the
-    stored-entry count of the reference's sparse chunks becomes the number of nonzero elements -- one predicate count per localpart."""
+    stored-entry count of the reference's sparse chunks becomes the number of nonzero elements -- one predicate count per localpart.  A sparse
+    DArray counts its stored entries (explicit zeros included) from host metadata, without a launch."""
+    from ._sparse import SparseDArray
+    if isinstance(d, SparseDArray):
+        return d.nnz()
     return count(d, lambda x: x != 0)
 
 

@@ -153,6 +153,9 @@ def _slices_last(rt, ch: B200Array, d: int, temps: List[B200Array]) -> B200Array
 
 def ppeval(f, *D, dim=None) -> DArray:
     """``ppeval(f, D...; dim)`` (reference src/mapreduce.jl:300-323).  See the module docstring for the served ``f``."""
+    from ._sparse import SparseDArray, refuse
+    if any(isinstance(a, SparseDArray) for a in D):
+        refuse("ppeval")
     dim = _normalise_dim(dim, D)
     if not D or not isinstance(D[0], DArray):
         raise _lib.ArgumentError(_lib.ERR_ARG, "ppeval: the first argument must be a DArray (its procs are the workers)")

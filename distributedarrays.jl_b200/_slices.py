@@ -414,6 +414,9 @@ def _redistribute(D: DArray, p) -> DArray:
 
 def mapslices(f, D: DArray, dims) -> DArray:
     """``mapslices(f, D; dims)`` (reference src/mapreduce.jl:191-208).  See the module docstring for the served ``f``."""
+    from ._sparse import SparseDArray, refuse
+    if isinstance(D, SparseDArray):
+        refuse("mapslices")
     if isinstance(D, SubDArray):
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "mapslices of a view: make it a DArray first (DArray(view))")
     if D.dtype.kind == "c":

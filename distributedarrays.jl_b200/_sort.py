@@ -189,6 +189,9 @@ def sort(d: DArray, sample=True, by=None, alg=None, **kwargs) -> DArray:  # noqa
     ``by``: a traceable key function (same closures as broadcast / map); values are ordered stably by ``by(x)``.
     ``alg`` is accepted and ignored: a keys-only sort has one result whatever the algorithm, and the keyed sort is stable like
     Julia's default.  Called on the slice of ``mapslices(sort, D; dims)`` it stands for the per-slice sort (``dab_sort_slices``)."""
+    from ._sparse import SparseDArray, refuse
+    if isinstance(d, SparseDArray):
+        refuse("sort")
     from ._broadcast import Expr
     if isinstance(d, Expr):
         from . import _slices

@@ -68,6 +68,7 @@ struct dab_ctx {
     int opt_gemv_phase;     // dab_set_option("gemv_phase"): 1 (default) = phase-class kernel for A*x, 0 = the single-wave aligned / unit-wise pair
     int opt_gemv_t_cols;    // dab_set_option("gemv_t_cols"): columns one thread of the A'*x kernel carries (4 or 8)
     int opt_gemv_t_waves;   // dab_set_option("gemv_t_waves"): waves of CTAs the A'*x kernel is split into
+    int opt_spmv_group;     // dab_set_option("spmv_group"): lanes per row of dab_spmv (1, 2, 4, 8, 16 or 32); 0 (default) = from nnz / rows
     int opt_ew_tma;         // dab_set_option("ew_tma"): route aligned unary elementwise launches through the TMA-staged kernel
     dab_pending_affine pending;  // at most one deferred dab_affine; launched by the next entry or consumed by dab_reduce
     int defer_off;          // set by dab_stream: foreign work on the raw stream expects every call to be queued already

@@ -248,6 +248,12 @@ int32_t dab_set_option(dab_ctx* ctx, const char* key, int64_t value) {
         ctx->opt_gemv_t_waves = (int)value;
         return DAB_OK;
     }
+    if (strcmp(key, "spmv_group") == 0) {
+        if (value != 0 && value != 1 && value != 2 && value != 4 && value != 8 && value != 16 && value != 32)
+            return dab_fail(ctx, DAB_ERR_ARG, "spmv_group must be 0 (automatic) or a power of two up to 32");
+        ctx->opt_spmv_group = (int)value;
+        return DAB_OK;
+    }
     if (strcmp(key, "gemm_simt") == 0) {
         ctx->opt_gemm_simt = value != 0;
         return DAB_OK;

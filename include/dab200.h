@@ -133,7 +133,8 @@ int32_t dab_device_info(dab_ctx* ctx, int32_t* device, int32_t* sm_count, size_t
  * dab_affine and stops holding any back on this ctx from then on. */
 int32_t dab_stream(dab_ctx* ctx, void** stream);
 /* tuning switches; "combine_timeout_ms" = wall-clock bound of the fused combine's wait for a peer; "ew_tma" = 1 routes aligned unary elementwise launches through the TMA-staged (cp.async.bulk + mbarrier
- * ring) kernel instead of the default flat LDG/STG kernel -- identical results, measured slower (DESIGN.md section 3). */
+ * ring) kernel instead of the default flat LDG/STG kernel -- identical results, measured slower (DESIGN.md section 3); "spmv_group" = lanes per row of
+ * dab_spmv (1, 2, 4, 8, 16 or 32; 0 = chosen from nnz / rows) -- identical results, every group size folds in storage order. */
 int32_t dab_set_option(dab_ctx* ctx, const char* key, int64_t value);
 /* number of kernels this ctx has launched so far (bench.py's gpu_launches claim). */
 int32_t dab_launch_count(dab_ctx* ctx, uint64_t* launches);
@@ -305,6 +306,22 @@ int32_t dab_gather_box(dab_ctx* ctx, int32_t elem_bytes, int32_t ndim, void* dst
  * combined into y by the caller exactly as the reference does (scale y by b, add a*R[i,j] in j order,
  * :101-117).  Float products accumulate in fp64 and round once; Int32/Int64 wrap.  dtypes: F32 F64 I32 I64. */
 int32_t dab_gemv(dab_ctx* ctx, int32_t dtype, int32_t trans, const void* A, size_t m, size_t n, const void* x, void* r);
+
+/* ==== sparse tile products K18 / K19 (row f9: SparseMatrixCSC chunks) ======================
+ * K18.  out[r] = (((0 + val[p0]*x[idx[p0]]) + val[p0+1]*x[idx[p0+1]]) + ...) over p in [ptr[r], ptr[r+1]), r < nrows, in storage order,
+ * in the element type, every product and add rounded on its own; Int32 / Int64 wrap.  Replaces  localpart(A)*xj  and  localpart(A)'*xj
+ * (src/linalg.jl:95-97, 141) for a SparseMatrixCSC chunk, i.e. SparseArrays' _spmatmul! / _At_or_Ac_mul_B! loops: on the CSC arrays
+ * (ptr = colptr, idx = rowval) it is A'*x; on the row-major copy of dab_csc_to_csr it is A*x.  ptr: nrows + 1 Int64 (0-based offsets),
+ * idx: Int32, val and x: dtype; nnz = ptr[nrows] - ptr[0], below 2^32 (it chooses the lanes per row).  out is overwritten; an empty row
+ * gives 0.  dtypes F32 F64 I32 I64.  Asynchronous on the ctx stream. */
+int32_t dab_spmv(dab_ctx* ctx, int32_t dtype, size_t nrows, size_t nnz, const void* ptr, const void* idx, const void* val, const void* x,
+                 void* out);
+/* K19.  Row-major copy of one m x n CSC chunk (colptr: n + 1 Int64, rowval: Int32 sorted within each column, nzval: nnz of dtype) into
+ * rowptr (m + 1 Int64), colidx (Int32) and val, rows ascending and columns ascending within each row.  Packs row << 32 | k per stored
+ * entry and sorts the words with dab_sort (K11).  m, n <= 2^31 - 1 and nnz < 2^32 - 4096, otherwise DAB_ERR_UNSUPPORTED.  Sort scratch
+ * (16 bytes per entry) is allocated and freed stream-ordered.  dtypes F32 F64 I32 I64.  Asynchronous on the ctx stream. */
+int32_t dab_csc_to_csr(dab_ctx* ctx, int32_t dtype, size_t m, size_t n, size_t nnz, const void* colptr, const void* rowval, const void* nzval,
+                       void* rowptr, void* colidx, void* val);
 
 /* ==== Level-3 tile product K12 (widening row f4; the one contraction on the path: tensor-core roofline) =====================
  * R[m x n] (ldc) = op(A) * B on column-major operands of ONE worker: transA = 0 -> A is m x k (lda); transA = 1 -> op(A) = A^T with A

@@ -25,6 +25,7 @@
 #   src/mapreduce.jl:205 mapslices(f, localpart(y), dims) mapslices_sort / svdvals_batched       dab_sort_slices / dab_svdvals_batched
 #   src/mapreduce.jl:315 _ppeval(f, localparts...; dim)   matmul_batched / eigvals_sym_batched  dab_matmul_batched / dab_eigvals_sym_batched
 #   (no reference method)  accumulate!(op, lp, lp; dims)   Base.accumulate! (cumsum! / cumprod!)   dab_scan
+#   src/linalg.jl:95-97,141 localpart(A)*xj, SparseMatrixCSC chunks   Base.:* (SparseB200Chunk)   dab_spmv / dab_csc_to_csr
 module DArrayB200
 
 using Distributed, DistributedArrays, LinearAlgebra
@@ -224,6 +225,42 @@ function Base.accumulate!(op, B::B200Array{R,N}, A::B200Array{T,N}; dims::Intege
                 ctx(), dab_dtype(T), SCAN_OPS[op], dab_dtype(R), A.ptr, inner, len, outer, carry === nothing ? C_NULL : carry.ptr, B.ptr), ctx())
     B
 end
+
+# ---- SparseMatrixCSC chunks (UNVERIFIED, like the rest of this file): distribute(S) with a sparse S uploads each localpart as three device
+# arrays; Julia's 1-based colptr / rowval become 0-based on upload.  localpart(A)*xj and localpart(A)'*xj (src/linalg.jl:95-97, 141) are
+# SparseArrays' loops, i.e. dab_spmv on the row-major copy (built once by dab_csc_to_csr) or on the CSC arrays themselves.
+using SparseArrays: SparseMatrixCSC, getcolptr, rowvals, nonzeros
+mutable struct SparseB200Chunk{T} <: AbstractMatrix{T}
+    m::Int; n::Int; nnz::Int
+    colptr::B200Array{Int64,1}; rowval::B200Array{Int32,1}; nzval::B200Array{T,1}
+    csr::Union{Nothing,Tuple{B200Array{Int64,1},B200Array{Int32,1},B200Array{T,1}}}
+end
+Base.size(a::SparseB200Chunk) = (a.m, a.n)
+SparseArrays.nnz(a::SparseB200Chunk) = a.nnz
+function SparseB200Chunk(S::SparseMatrixCSC{T}) where {T<:Union{Float32,Float64,Int32,Int64}}
+    size(S, 1) <= typemax(Int32) || throw(ArgumentError("sparse chunks of more than 2^31-1 rows are not served"))
+    SparseB200Chunk{T}(size(S)..., nnz(S), B200Array(Int64.(getcolptr(S) .- 1)), B200Array(Int32.(rowvals(S) .- 1)), B200Array(copy(nonzeros(S))), nothing)
+end
+function row_major!(a::SparseB200Chunk{T}) where {T}
+    if a.csr === nothing
+        rp, ci, v = B200Array{Int64,1}(undef, (a.m + 1,)), B200Array{Int32,1}(undef, (a.nnz,)), B200Array{T,1}(undef, (a.nnz,))
+        check(ccall((:dab_csc_to_csr, libdab), Int32, (Ptr{Cvoid}, Int32, Csize_t, Csize_t, Csize_t, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid},
+                    Ptr{Cvoid}, Ptr{Cvoid}), ctx(), dab_dtype(T), a.m, a.n, a.nnz, a.colptr.ptr, a.rowval.ptr, a.nzval.ptr, rp.ptr, ci.ptr, v.ptr), ctx())
+        a.csr = (rp, ci, v)
+    end
+    a.csr
+end
+function spmv!(r::B200Array{T,1}, nrows, nnz, ptr, idx, val, x::B200Array{T,1}) where {T}
+    check(ccall((:dab_spmv, libdab), Int32, (Ptr{Cvoid}, Int32, Csize_t, Csize_t, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+                ctx(), dab_dtype(T), nrows, nnz, ptr.ptr, idx.ptr, val.ptr, x.ptr, r.ptr), ctx())
+    r
+end
+function Base.:*(a::SparseB200Chunk{T}, x::B200Array{T,1}) where {T}
+    rp, ci, v = row_major!(a)
+    spmv!(B200Array{T,1}(undef, (a.m,)), a.m, a.nnz, rp, ci, v, x)
+end
+Base.:*(a::Union{Adjoint{T,<:SparseB200Chunk{T}},Transpose{T,<:SparseB200Chunk{T}}}, x::B200Array{T,1}) where {T<:Real} =
+    (p = parent(a); spmv!(B200Array{T,1}(undef, (p.n,)), p.n, p.nnz, p.colptr, p.rowval, p.nzval, x))
 
 # ---- the combine seam: sum(d::DArray{T,N,<:B200Array}) in ONE call per worker ----------------------------------------------------------
 # replaces  results = asyncmap(procs(d)) do p; remotecall_fetch(...) end;  reduce(op, results)   (src/mapreduce.jl:29-35):

@@ -152,6 +152,22 @@ def main():
     rt.barrier()
     log("ok: ComplexF64 sum and copy(adjoint(A)) across ranks")
 
+    # ---- sparse chunks: A*x and A'*x with the tile products on every rank, bit for bit against the model of SparseArrays' loops
+    import scipy.sparse as sps
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import sparse_oracle as so
+    rs = np.random.default_rng(83)
+    Sh = sps.random(203, 157, density=0.1, random_state=rs, data_rvs=rs.standard_normal, format="csc")   # same seed on every rank
+    DS = dab.distribute(Sh)
+    trip = so.canonical_triplets(Sh)
+    for trans, xs in ((False, rs.standard_normal(157)), (True, rs.standard_normal(203))):
+        y = dab.to_array((DS.T if trans else DS) @ dab.distribute(xs))
+        assert so.same_bits(y, so.mul_model(trip, Sh.shape, DS.layout.cuts, xs, trans)), trans
+    assert dab.nnz(DS) == Sh.nnz
+    DS.close()
+    rt.barrier()
+    log("ok: sparse A*x and A'*x across ranks")
+
     # ---- samplesort across ranks: pieces travel by grouped NCCL send/recv; layout and boundaries equal the oracle's
     for T in (np.int64, np.float64):
         rs = np.random.default_rng(77)
