@@ -18,6 +18,7 @@ F32, F64, I32, I64, U8, I128, C64, C128 = range(8)     # I128: value type of dab
 SUM, PROD, MAX, MIN, ALL, ANY, COUNT, EXTREMA = range(8)
 MAP_ID, MAP_ABS, MAP_ABS2, MAP_NEG, MAP_SQRT, MAP_INV, MAP_FLOOR, MAP_CEIL, MAP_SIGN = range(9)
 MAP_EQ, MAP_NE, MAP_LT, MAP_LE, MAP_GT, MAP_GE, MAP_ISNAN, MAP_NONZERO = range(16, 24)
+FINDMAX, FINDMIN = range(2)                   # which of dab_findminmax / dab_findminmax_dim / dab_combine_findminmax
 ADD, SUB, MUL, DIV, REM, BMAX, BMIN, MOD, IDIV, AND, OR, XOR = range(12)
 SORT_SLICES_SMEM_LEN = 8192                   # longest fibre dab_sort_slices sorts in shared memory
 SVDVALS_MAX_K, SVDVALS_MAX_ELEMS = 32, 4096   # dab_svdvals_batched serves min(m, n) <= 32 and m * n <= 4096
@@ -99,6 +100,9 @@ _SIGS = {
     "dab_reduce_result_dtype": (_i32, [_i32, _i32, _i32, C.POINTER(_i32)]),
     "dab_combine_ordered": (_i32, [_i32, _i32, _vp, _sz, _vp]),
     "dab_reducedim": (_i32, [_vp, _i32, _i32, _i32, _vp, _sz, _sz, _sz, _vp, _i32]),
+    "dab_findminmax": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp, _sz, _vp]),
+    "dab_findminmax_dim": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp, _sz, _sz, _sz, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "dab_combine_findminmax": (_i32, [_i32, _i32, _vp, _sz, _vp]),
     "dab_scan": (_i32, [_vp, _i32, _i32, _i32, _vp, _sz, _sz, _sz, _vp, _vp]),
     "dab_scan_totals": (_i32, [_vp, _i32, _i32, _i32, _vp, _sz, _sz, _sz, _vp]),
     "dab_scan_carrier_dtype": (_i32, [_i32, _i32, _i32, C.POINTER(_i32)]),

@@ -90,6 +90,12 @@ enum {
                        only, MAP_ID only; the cross-worker fold takes min of mins / max of maxes)            */
 };
 
+/* ---- which argument of dab_findminmax / dab_findminmax_dim / dab_combine_findminmax ---- */
+enum {
+    DAB_FINDMAX = 0, /* Base.findmax: the later element wins when isless(best, x)    */
+    DAB_FINDMIN = 1  /* Base.findmin: the later element wins when isgreater(best, x) */
+};
+
 /* ---- map functions f of mapreduce(f, op, A) / unary broadcast ------------------------ */
 enum {
     DAB_MAP_ID = 0,
@@ -252,6 +258,31 @@ int32_t dab_combine_ordered(int32_t result_dtype, int32_t op, const void* partia
  * dab_reduce_result_dtype. */
 int32_t dab_reducedim(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, const void* x, size_t inner, size_t reduce,
                       size_t outer, void* out, int32_t accumulate);
+
+/* ==== findmax / findmin K20 ================================================================
+ * Replace Base's findmax(f, A) / findmin(f, A) (_findmax) and findminmax!(f, op, Rval, Rind, A) (the dims form) on one chunk.  The winner
+ * is the element with the largest order key, then the smallest linear index: Julia's isless order of f(x) for DAB_FINDMAX, reversed for
+ * DAB_FINDMIN, with every NaN on top for both (NaN wins, the first NaN is kept; findmax prefers +0.0, findmin -0.0; ties keep the earlier
+ * index).  dtype: F32 F64 I32 I64, and U8 holding Bool (0 / 1).  map: MAP_ID, MAP_ABS, MAP_ABS2 (Int32 abs / abs2 wrap as in Julia; both
+ * are the identity on Bool).  Complex dtypes and other maps -> DAB_ERR_UNSUPPORTED, a bad `which` -> DAB_ERR_ARG, before the context is
+ * touched.  x must be aligned to its element size; any 16-byte phase is served.
+ *
+ * dab_findminmax: out_dev gets 16 bytes: [0, 8) f(x[i]) as T (zero-padded; the element itself, so a NaN keeps its payload), [8, 16) i,
+ * the 0-based chunk-local linear index, as Int64.  map_param: unused (NULL).  n == 0 -> DAB_ERR_EMPTY. */
+int32_t dab_findminmax(dab_ctx* ctx, int32_t dtype, int32_t which, int32_t map, const void* map_param, const void* x, size_t n,
+                       void* out_dev);
+/* dab_findminmax_dim: x collapsed to (inner, reduce, outer) as in dab_reducedim; out_vals[i + inner*o] (T) and out_idx[i + inner*o]
+ * (Int64) are the winner of x[i + inner*(r + reduce*o)], r = 0 .. reduce-1.  out_idx is the 1-based GLOBAL linear index of the winner:
+ * its chunk-local position unravelled in chunk_dims[0..nd), shifted by the 0-based offsets[], ravelled in global_dims[] (nd <= 8;
+ * nd == 0: the position itself plus one).  idx_in (optional, MAP_ID only): an Int64 array shaped like x holding each value's 1-based
+ * global index already; the winner's index is then taken from it and compared as such (a second reduced run, the fold of exchanged
+ * slabs).  inner * outer == 0: nothing to do; reduce == 0 -> DAB_ERR_EMPTY. */
+int32_t dab_findminmax_dim(dab_ctx* ctx, int32_t dtype, int32_t which, int32_t map, const void* x, const int64_t* idx_in, size_t inner,
+                           size_t reduce, size_t outer, int32_t nd, const int64_t* chunk_dims, const int64_t* offsets,
+                           const int64_t* global_dims, void* out_vals, int64_t* out_idx);
+/* Host-only: the winner of `count` 16-byte records (value as T in [0, 8), Int64 index in [8, 16), any one index convention) under the
+ * order above, copied to out (16 bytes).  Lets the chunk results of dab_findminmax, made global, be folded in any order. */
+int32_t dab_combine_findminmax(int32_t dtype, int32_t which, const void* records, size_t count, void* out);
 
 /* ==== scans K17: accumulate! / cumsum! / cumprod! =========================================
  * Replaces Base's accumulate!(op, B, A; dims, init) (base/accumulate.jl: _accumulate!, accumulate_pairwise / the per-fibre loop

@@ -26,6 +26,7 @@
 #   src/mapreduce.jl:315 _ppeval(f, localparts...; dim)   matmul_batched / eigvals_sym_batched  dab_matmul_batched / dab_eigvals_sym_batched
 #   (no reference method)  accumulate!(op, lp, lp; dims)   Base.accumulate! (cumsum! / cumprod!)   dab_scan
 #   src/linalg.jl:95-97,141 localpart(A)*xj, SparseMatrixCSC chunks   Base.:* (SparseB200Chunk)   dab_spmv / dab_csc_to_csr
+#   (Base._findmax: scalar getindex)  findmax(f, d) / findmin(f, d)   (DArray methods below)   dab_findminmax / dab_combine_findminmax
 module DArrayB200
 
 using Distributed, DistributedArrays, LinearAlgebra
@@ -224,6 +225,44 @@ function Base.accumulate!(op, B::B200Array{R,N}, A::B200Array{T,N}; dims::Intege
     check(ccall((:dab_scan, libdab), Int32, (Ptr{Cvoid}, Int32, Int32, Int32, Ptr{Cvoid}, Csize_t, Csize_t, Csize_t, Ptr{Cvoid}, Ptr{Cvoid}),
                 ctx(), dab_dtype(T), SCAN_OPS[op], dab_dtype(R), A.ptr, inner, len, outer, carry === nothing ? C_NULL : carry.ptr, B.ptr), ctx())
     B
+end
+
+# ---- findmax / findmin (K20): ONE dab_findminmax launch per chunk; the chunk winners, made global through localindices, are folded by
+# dab_combine_findminmax (any order: the winner is the largest order key, then the smallest global linear index).  The index is Julia's:
+# an Int for a vector, a CartesianIndex otherwise.  Only DArrays of B200Array chunks with a served element type take these methods; every
+# other DArray keeps Base's generic findmax.  f outside identity / abs / abs2 is mapped first (f.(d), the elementwise kernels), and the
+# dims form is left to Base's generic findminmax! (the kernel-backed dims form is the host runtime's, distributedarrays.jl_b200/_findmax.py).
+const FIND_MAPS = Dict{Any,Int32}(identity => 0, abs => 1, abs2 => 2)
+const FindT = Union{Float32,Float64,Int32,Int64,Bool}
+const FindDArray{T,N} = DArray{T,N,<:B200Array{T,N}}
+function chunk_findminmax(a::B200Array{T}, which::Int32, f) where {T}
+    slot = B200Array{UInt8,1}(undef, (16,))
+    check(ccall((:dab_findminmax, libdab), Int32, (Ptr{Cvoid}, Int32, Int32, Int32, Ptr{Cvoid}, Ptr{Cvoid}, Csize_t, Ptr{Cvoid}),
+                ctx(), dab_dtype(T), which, FIND_MAPS[f], C_NULL, a.ptr, length(a), slot.ptr), ctx())
+    Array(slot)
+end
+function findminmax_darray(f, d::FindDArray{T,N}, which::Int32) where {T<:FindT,N}
+    isempty(d) && throw(ArgumentError("reducing over an empty collection is not allowed"))
+    recs = UInt8[]
+    for (p, I) in zip(procs(d), d.indices)
+        all(!isempty, I) || continue
+        r = remotecall_fetch(() -> chunk_findminmax(localpart(d), which, f), p)
+        li = reinterpret(Int64, r[9:16])[1]                                         # 0-based, chunk-local
+        c = CartesianIndices(map(length, I))[li + 1]
+        g = LinearIndices(size(d))[CartesianIndex(map((k, rng) -> first(rng) + k - 1, Tuple(c), I))]
+        append!(recs, r[1:8], reinterpret(UInt8, [Int64(g)]))
+    end
+    out = zeros(UInt8, 16)
+    check(ccall((:dab_combine_findminmax, libdab), Int32, (Int32, Int32, Ptr{Cvoid}, Csize_t, Ptr{Cvoid}), dab_dtype(T), which, recs, length(recs) ÷ 16, out))
+    v, g = reinterpret(T, out[1:sizeof(T)])[1], reinterpret(Int64, out[9:16])[1]
+    v, N == 1 ? Int(g) : CartesianIndices(size(d))[g]
+end
+for (fn, which) in ((:findmax, Int32(0)), (:findmin, Int32(1)))
+    @eval function Base.$fn(f, d::FindDArray{T}; dims = :) where {T<:FindT}
+        dims isa Colon || return invoke(Base.$fn, Tuple{Any,AbstractArray}, f, d; dims = dims)
+        haskey(FIND_MAPS, f) ? findminmax_darray(f, d, $which) : Base.$fn(identity, f.(d))
+    end
+    @eval Base.$fn(d::FindDArray{T}; dims = :) where {T<:FindT} = Base.$fn(identity, d; dims = dims)
 end
 
 # ---- SparseMatrixCSC chunks (UNVERIFIED, like the rest of this file): distribute(S) with a sparse S uploads each localpart as three device
