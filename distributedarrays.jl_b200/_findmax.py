@@ -21,9 +21,8 @@ import numpy as np
 from . import _lib
 from ._broadcast import broadcast, is_ctag
 from ._darray import B200Array, DArray, dab_dtype, is_complex
-from ._mapreduce import _gather_slots, _normalise_region, classify_map, exchange_plan, plan_reducedim
+from ._mapreduce import _gather_slots, _normalise_region, classify_map, gather_fibres, plan_reducedim
 from .layout import collapse_for_region, shape_of
-from .runtime import exchange_stacks, fence, grouped_exchange
 
 _SERVED_MAPS = (_lib.MAP_ID, _lib.MAP_ABS, _lib.MAP_ABS2)
 _I64 = C.c_int64
@@ -204,41 +203,14 @@ def _dims(which: int, mapc: int, d: DArray, dims):
         return DArray(Rlayout, d.dtype, Vchunks, rt), DArray(Rlayout, np.dtype(np.int64), Ichunks, rt)
     # ---- phase 1: every chunk reduced along the region, indices made global
     partial = {pid: _reduce_chunk(rt, d, pid, ch, reg_in, which, mapc) for pid, ch in d.chunks.items()}
-    # ---- phase 2: the (values, indices) slabs of a fibre gathered on the owner of the R chunk and folded there.  A stack holds the
-    # values of all members, then (8-byte aligned) their indices.
-    vbytes = [(plen * len(m) * isz + 7) & ~7 for plen, m in zip(plens, fibres)]
-    st = exchange_stacks(rt, [rt.rank_of(p) for p in Rpids],
-                         [0 if len(m) == 1 else vb + plen * len(m) * 8 for vb, plen, m in zip(vbytes, plens, fibres)])
-    my_tab = st.tables[rt.rank]
-    xp = exchange_plan(L, Rlayout, fibres, rt.rank_of, rt.rank)
-
-    def places(rl, slot, base):
-        plen = plens[rl]
-        return ((base + slot * plen * isz, plen * isz, 0), (base + vbytes[rl] + slot * plen * 8, plen * 8, 1))
-
+    # ---- phase 2: the (values, indices) slabs of a fibre gathered on the owner of the R chunk and folded there.  A fibre of one member
+    # gathers nothing: its slab is already on the owner.
+    stack_temp = 0
     try:
-        for rl, slot, mp in xp["local"]:
-            if plens[rl] and len(fibres[rl]) > 1:
-                for dst, nb, which_arr in places(rl, slot, st.base + my_tab[rl]):
-                    _lib.call("dab_d2d", rt.ctx, C.c_void_p(dst), C.c_void_p(partial[mp][which_arr].ptr), nb)
-        if st.use_arena:
-            peers = rt.arena()["peers"]
-            for mp, peer, rl in xp["sends"]:
-                slot = fibres[rl].index(L.pids.index(mp))
-                if plens[rl]:
-                    for dst, nb, which_arr in places(rl, slot, peers[peer] + st.bank + st.tables[peer][rl]):
-                        _lib.call("dab_d2d", rt.ctx, C.c_void_p(dst), C.c_void_p(partial[mp][which_arr].ptr), nb)
-            fence(rt, "device")                      # every producer's puts have landed
-        else:
-            sends, recvs = [], []
-            for mp, peer, rl in xp["sends"]:
-                for k in (0, 1):
-                    sends.append((partial[mp][k].ptr, plens[rl] * (isz if k == 0 else 8), peer))
-            for rl, slot, _, peer in xp["recvs"]:
-                for dst, nb, _k in places(rl, slot, st.base + my_tab[rl]):
-                    recvs.append((dst, nb, peer))
-            grouped_exchange(rt, sends, recvs)
-        for rl, off in my_tab.items():
+        st, stacks = gather_fibres(rt, L, Rlayout, [m if len(m) > 1 else [] for m in fibres], [(plen * isz, plen * 8) for plen in plens],
+                                   {pid: (v.ptr, i.ptr) for pid, (v, i) in partial.items()})
+        stack_temp = st.temp
+        for rl, (vbase, ibase) in stacks.items():
             owner, members = Rpids[rl], fibres[rl]
             shape = shape_of(Rindices[rl])
             if len(members) == 1:                    # the owner's own slab is the result (no reduced dim cut across chunks)
@@ -247,12 +219,11 @@ def _dims(which: int, mapc: int, d: DArray, dims):
                 Vchunks[owner], Ichunks[owner] = v, i
                 continue
             Vch, Ich = B200Array.empty(rt, shape, d.dtype), B200Array.empty(rt, shape, np.int64)
-            base = st.base + off
-            _lib.call("dab_findminmax_dim", rt.ctx, code, which, _lib.MAP_ID, C.c_void_p(base), C.c_void_p(base + vbytes[rl]), plens[rl],
+            _lib.call("dab_findminmax_dim", rt.ctx, code, which, _lib.MAP_ID, C.c_void_p(vbase), C.c_void_p(ibase), plens[rl],
                       len(members), 1, 0, None, None, None, C.c_void_p(Vch.ptr), C.c_void_p(Ich.ptr))
             Vchunks[owner], Ichunks[owner] = Vch, Ich
     finally:
-        rt.free_temp(st.temp)
+        rt.free_temp(stack_temp)
         for v, i in partial.values():
             v.free()
             i.free()

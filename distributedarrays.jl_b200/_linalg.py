@@ -25,7 +25,7 @@ from . import _lib
 from ._darray import B200Array, DArray, SubDArray, dab_dtype, darray
 from ._sparse import SparseDArray, refuse
 from .layout import make_layout, rlen, shape_of
-from .runtime import Runtime, close_remote_reads, exchange_stacks, fence, grouped_exchange, open_remote_reads
+from .runtime import Runtime, close_remote_reads, deliver, exchange_stacks, grouped_exchange, open_remote_reads
 
 _GEMV_DTYPES = (np.dtype(np.float32), np.dtype(np.float64), np.dtype(np.int32), np.dtype(np.int64))
 
@@ -213,13 +213,12 @@ def mul_(y: DArray, A: Union[DArray, Transpose], x, alpha=1, beta=0) -> DArray:
     # ---- where the tile results are combined: on the owner of y's chunk i, a stack of gj slots of plen each
     st = exchange_stacks(rt, [rt.rank_of(p) for p in ypids], [rlen(ix[0]) * gj * isz for ix in y.layout.indices])
     my_tab = st.tables[rt.rank]
-    peers = rt.arena()["peers"] if st.use_arena else None
 
     # ---- R[i,j] = localpart(A) * xj on the tile owners (src/linalg.jl:90-98); a tile whose consumer is this rank is written straight
     # into its slot of the stack
     temps: List[B200Array] = []
     xblocks: Dict[int, B200Array] = {}
-    puts, sends = [], {}
+    remote: Dict[Tuple[int, int], int] = {}                # (i, j) -> the tile result shipped to another rank
     for j in range(gj):
         for i in range(gi):
             pid = tile_pid(i, j)
@@ -235,23 +234,14 @@ def mul_(y: DArray, A: Union[DArray, Transpose], x, alpha=1, beta=0) -> DArray:
             else:
                 r = B200Array.empty(rt, (plen,), dt, temp=True)
                 temps.append(r)
-                rptr = r.ptr
-                if st.use_arena:
-                    puts.append((peers[orank] + st.bank + st.tables[orank][i] + j * plen * isz, rptr, plen * isz))
-                else:
-                    sends[(i, j)] = rptr
+                rptr = remote[i, j] = r.ptr
             tile_product(rt, code, trans, ch, xblocks[j].ptr, rptr)
-    # ---- ship the tile results to the owner of y's chunk i (the fetch(rij) of :113-115)
-    if st.use_arena:
-        for dst, src, nb in puts:                          # one-sided puts over NVLink into the consumer's arena bank
-            if nb:
-                _lib.call("dab_d2d", rt.ctx, C.c_void_p(dst), C.c_void_p(src), nb)
-        fence(rt, "device")                                # every producer's puts have landed; also: every reader of x is done with it
-    elif rt.world > 1:
+    # ---- ship the tile results to the owner of y's chunk i (the fetch(rij) of :113-115); with the arena, the device fence this ends with
+    # also means every reader of x is done with it
+    if rt.world > 1:
         plan = matvec_exchange_plan(L, y.layout, trans, rt.rank_of, rt.rank)   # same (i, j) order on both sides of every pair
-        sends = [(sends[(i, j)], plen * isz, peer) for i, j, plen, peer in plan["sends"] if plen]
-        recvs = [(st.base + my_tab[i] + j * plen * isz, plen * isz, peer) for i, j, plen, peer in plan["recvs"] if plen]
-        grouped_exchange(rt, sends, recvs)
+        deliver(rt, st, [(remote[i, j], plen * isz, peer, i, j * plen * isz) for i, j, plen, peer in plan["sends"]],
+                [(peer, i, j * plen * isz, plen * isz) for i, j, plen, peer in plan["recvs"]])
     # ---- scale y (:101-111), then add!(localpart(y), R[i,j], α) for each j (:114-117; j order) -- one fused launch per y chunk
     a_s, b_s = np.asarray(alpha, dtype=dt), np.asarray(beta, dtype=dt)
     for i, off in my_tab.items():

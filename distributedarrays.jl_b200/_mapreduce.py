@@ -15,6 +15,7 @@ from __future__ import annotations
 import builtins
 import ctypes as C
 import operator
+from itertools import accumulate
 from typing import Callable, Dict, Optional, Sequence, Tuple
 
 import numpy as np
@@ -23,7 +24,7 @@ from . import _lib
 from ._broadcast import Expr, broadcast, is_ctag, tag_of, trace, _NPT
 from ._darray import B200Array, DArray, component_dtype, dab_dtype, is_complex, np_dtype
 from .layout import Layout, collapse_for_region, ravel, shape_of, unravel
-from .runtime import close_remote_reads, exchange_stacks, fence, grouped_exchange, open_remote_reads
+from .runtime import close_remote_reads, deliver, exchange_stacks, open_remote_reads
 
 _OPS = {"+": _lib.SUM, "add": _lib.SUM, "sum": _lib.SUM, "*": _lib.PROD, "mul": _lib.PROD, "prod": _lib.PROD, "max": _lib.MAX,
         "min": _lib.MIN}
@@ -530,6 +531,32 @@ def exchange_plan(L: Layout, Rlayout: Layout, fibres, rank_of: Callable[[int], i
     return {"owned": owned, "local": local, "recvs": recvs, "sends": sends}
 
 
+def gather_fibres(rt, L: Layout, Rlayout: Layout, fibres, plane_bytes, slabs):
+    """Collects the slabs of every fibre on the owner of its result chunk, in fibre order: the exchange of ``mapreducedim_between!``
+    (reference src/mapreduce.jl:71-81), also used by the scan carry and findmax.  Collective.
+
+    A slab has one or more planes (findmax: values, then indices); ``plane_bytes[rl]`` gives the bytes of one member's slab in each
+    plane for result chunk ``rl``, and ``slabs[pid]`` the device pointer of each plane of member chunk ``pid`` on this rank.  The stack of
+    ``rl`` holds its planes back to back, plane ``p`` taking ``len(fibres[rl]) * plane_bytes[rl][p]`` bytes rounded up to 8, slot ``s`` at
+    ``s * plane_bytes[rl][p]``.  Returns the ``Stacks`` (the caller frees ``temp`` after the folds that read them) and, for every result
+    chunk owned by this rank, the device address of each plane of its stack."""
+    offs = [list(accumulate(((len(m) * nb + 7) & ~7 for nb in pb), initial=0)) for m, pb in zip(fibres, plane_bytes)]
+    st = exchange_stacks(rt, [rt.rank_of(p) for p in Rlayout.pids], [o[-1] for o in offs])
+    try:
+        xp = exchange_plan(L, Rlayout, fibres, rt.rank_of, rt.rank)
+        slot_of = {(rl, L.pids[m]): s for rl, members in enumerate(fibres) for s, m in enumerate(members)}
+        # (plane, its offset in the stack, bytes per slot) of each result chunk; an empty plane moves nothing and may have no slab
+        planes = [[(p, off, nb) for p, (off, nb) in enumerate(zip(o, pb)) if nb] for o, pb in zip(offs, plane_bytes)]
+        sends = [(slabs[mp][p], nb, rt.rank, rl, off + slot * nb) for rl, slot, mp in xp["local"] for p, off, nb in planes[rl]]
+        sends += [(slabs[mp][p], nb, orank, rl, off + slot_of[rl, mp] * nb) for mp, orank, rl in xp["sends"] for p, off, nb in planes[rl]]
+        recvs = [(mrank, rl, off + slot * nb, nb) for rl, slot, _, mrank in xp["recvs"] for _, off, nb in planes[rl]]
+        deliver(rt, st, sends, recvs)
+    except BaseException:
+        rt.free_temp(st.temp)
+        raise
+    return st, {rl: [st.base + st.tables[rt.rank][rl] + off for off in offs[rl][:-1]] for rl in xp["owned"]}
+
+
 def mapreducedim(f: Optional[Callable], op, d: DArray, dims, init=None) -> DArray:
     """``mapreduce(f, op, d; dims[, init])`` -> DArray R (reference src/mapreduce.jl:42-94)."""
     rt = d.rt
@@ -559,6 +586,8 @@ def mapreducedim(f: Optional[Callable], op, d: DArray, dims, init=None) -> DArra
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"reductions of {src.dtype} values with dims are served for + only")
     rdt = _result_dtype(src.dtype, opc, mapc)
     L = src.layout
+    partial: Dict[int, B200Array] = {}
+    stack_temp = 0
     try:
         if not reg_in or d.size == 0:
             # ``isempty(region) -> copyto!(R, A)`` (src/mapreduce.jl:89-91; f and init are NOT applied there) and
@@ -576,36 +605,15 @@ def mapreducedim(f: Optional[Callable], op, d: DArray, dims, init=None) -> DArra
         Rlayout, fibres = plan_reducedim(L, reg_in)
         Rpids, Rindices = Rlayout.pids, Rlayout.indices
         # ---- phase 1: mapreducedim_within (src/mapreduce.jl:54-66)
-        partial: Dict[int, B200Array] = {}
         for pid, ch in src.chunks.items():
             partial[pid] = reduce_chunk_dims(rt, ch, reg_in, opc, mapc, rdt)
         # ---- phase 2: mapreducedim_between! (src/mapreduce.jl:71-81): the partial slabs of a fibre are gathered on the owner of the R
-        # chunk, in grid order.  Multi-rank: one-sided puts over NVLink into the owner's exchange arena + a device-side barrier (no NCCL
-        # launch, no host sync); slabs too large for the arena, or DAB_FUSED_COMBINE=0, take the grouped ncclSend/ncclRecv path.
+        # chunk, in grid order, and folded there
         Rchunks: Dict[int, B200Array] = {}
-        isz = rdt.itemsize
         plens = [int(np.prod(shape_of(ix))) for ix in Rindices]
-        st = exchange_stacks(rt, [rt.rank_of(p) for p in Rpids], [plen * len(members) * isz for plen, members in zip(plens, fibres)])
-        my_tab = st.tables[rt.rank]
-        xp = exchange_plan(L, Rlayout, fibres, rt.rank_of, rt.rank)
-        for rl, slot, mp in xp["local"]:
-            plen = plens[rl]
-            if plen:
-                _lib.call("dab_d2d", rt.ctx, C.c_void_p(st.base + my_tab[rl] + slot * plen * isz), C.c_void_p(partial[mp].ptr), plen * isz)
-        if st.use_arena:
-            peers = rt.arena()["peers"]
-            for mp, peer, rl in xp["sends"]:
-                plen = plens[rl]
-                slot = fibres[rl].index(L.pids.index(mp))
-                if plen:
-                    _lib.call("dab_d2d", rt.ctx, C.c_void_p(peers[peer] + st.bank + st.tables[peer][rl] + slot * plen * isz), C.c_void_p(partial[mp].ptr),
-                              plen * isz)
-            fence(rt, "device")                                    # every producer's puts have landed
-        else:
-            sends = [(partial[mp].ptr, partial[mp].size * isz, peer) for mp, peer, _ in xp["sends"]]
-            recvs = [(st.base + my_tab[rl] + slot * plens[rl] * isz, plens[rl] * isz, peer) for rl, slot, _, peer in xp["recvs"]]
-            grouped_exchange(rt, sends, recvs)
-        for rl, off in my_tab.items():
+        st, stacks = gather_fibres(rt, L, Rlayout, fibres, [(plen * rdt.itemsize,) for plen in plens], {pid: (p.ptr,) for pid, p in partial.items()})
+        stack_temp = st.temp
+        for rl, (base,) in stacks.items():
             owner = Rpids[rl]
             Rch = B200Array.empty(rt, shape_of(Rindices[rl]), rdt)
             acc = 0
@@ -615,14 +623,14 @@ def mapreducedim(f: Optional[Callable], op, d: DArray, dims, init=None) -> DArra
                           C.c_void_p(v.ctypes.data))
                 acc = 1
             # Base.mapreducedim!(identity, op, localpart(R), Bfull): accumulate the partial slabs of the fibre, in grid order, onto R
-            _lib.call("dab_reducedim", rt.ctx, dab_dtype(rdt), opc, _lib.MAP_ID, C.c_void_p(st.base + off), plens[rl], len(fibres[rl]), 1,
+            _lib.call("dab_reducedim", rt.ctx, dab_dtype(rdt), opc, _lib.MAP_ID, C.c_void_p(base), plens[rl], len(fibres[rl]), 1,
                       C.c_void_p(Rch.ptr), acc)
             Rchunks[owner] = Rch
-        rt.free_temp(st.temp)
-        for p in partial.values():
-            p.free()
         return DArray(Rlayout, rdt, Rchunks, rt)
     finally:
+        rt.free_temp(stack_temp)                                   # stream-ordered: after the folds that read the stacks
+        for p in partial.values():
+            p.free()
         if tmp is not None:
             tmp.close()
 

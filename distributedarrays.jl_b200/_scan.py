@@ -3,9 +3,9 @@
 The reference has none: Base's generic ``accumulate!`` writes ``similar(A)`` element by element, which ends in ``setindex!`` on a DArray.
 Here every chunk is scanned by ONE ``dab_scan`` launch (include/dab200.h, K17).  When ``dims`` is split across workers, chunk ``g`` along
 ``dims`` starts from the carry ``init (op) total_0 (op) ... (op) total_(g-1)``: every earlier chunk reduces itself to a slab of carriers
-(``dab_scan_totals``), the slabs travel to the later chunks like the partial slabs of ``mapreducedim_between!`` (exchange arena puts +
-device fence, or grouped NCCL send / recv), and each consumer folds its stack of slabs in grid order with one small ``dab_scan`` along
-the stack.  The plan of who sends which total to whom is a pure function of the layout (``carry_plan``), so every rank derives the same.
+(``dab_scan_totals``), the slabs travel to the later chunks like the partial slabs of ``mapreducedim_between!``
+(``_mapreduce.gather_fibres``), and each consumer folds its stack of slabs in grid order with one small ``dab_scan`` along the stack.
+The plan of who sends which total to whom is a pure function of the layout (``carry_plan``), so every rank derives the same.
 """
 from __future__ import annotations
 
@@ -17,9 +17,9 @@ import numpy as np
 
 from . import _lib
 from ._darray import DArray, SubDArray, B200Array, copyto, dab_dtype, is_complex, makelocal, similar
-from ._mapreduce import _op_code, exchange_plan
+from ._mapreduce import _op_code, gather_fibres
 from .layout import Layout, ravel, shape_of, unravel
-from .runtime import close_remote_reads, exchange_stacks, fence, grouped_exchange, open_remote_reads
+from .runtime import close_remote_reads, open_remote_reads
 
 _UNDEF_DIMS = "UndefKeywordError: keyword argument `dims` not assigned"
 
@@ -145,7 +145,6 @@ def _run(opc: int, dest: DArray, src: DArray, dims: int, R: np.dtype, ival):
         shapes = [shape_of(ix) for ix in L.indices]
         plens = [int(np.prod(s[:k] + s[k + 1:], dtype=np.int64)) for s in shapes]
         fibres = carry_plan(L, dims) if L.grid[k] > 1 else [[] for _ in L.pids]
-        stacks = None
         if L.grid[k] > 1:
             # chunk totals of every chunk with a successor along dims, then the totals travel to the chunks after it
             G = L.grid[k]
@@ -157,26 +156,8 @@ def _run(opc: int, dest: DArray, src: DArray, dims: int, R: np.dtype, ival):
                     temps.append(t)
                     _lib.call("dab_scan_totals", rt.ctx, icode, opc, ocode, C.c_void_p(x.ptr), *_shape3(shapes[rl], k), C.c_void_p(t.ptr))
                     totals[pid] = t
-            st = exchange_stacks(rt, [rt.rank_of(p) for p in L.pids], [plen * len(m) * isz for plen, m in zip(plens, fibres)])
+            st, stacks = gather_fibres(rt, L, L, fibres, [(plen * isz,) for plen in plens], {pid: (t.ptr,) for pid, t in totals.items()})
             stack_temp = st.temp
-            tab = st.tables[rt.rank]
-            xp = exchange_plan(L, L, fibres, rt.rank_of, rt.rank)
-            for rl, slot, mp in xp["local"]:
-                if plens[rl]:
-                    _lib.call("dab_d2d", rt.ctx, C.c_void_p(st.base + tab[rl] + slot * plens[rl] * isz), C.c_void_p(totals[mp].ptr), plens[rl] * isz)
-            if st.use_arena:
-                peers = rt.arena()["peers"]
-                for mp, peer, rl in xp["sends"]:
-                    slot = fibres[rl].index(L.pids.index(mp))
-                    if plens[rl]:
-                        _lib.call("dab_d2d", rt.ctx, C.c_void_p(peers[peer] + st.bank + st.tables[peer][rl] + slot * plens[rl] * isz),
-                                  C.c_void_p(totals[mp].ptr), plens[rl] * isz)
-                fence(rt, "device")                    # every producer's puts have landed
-            else:
-                sends = [(totals[mp].ptr, plens[rl] * isz, peer) for mp, peer, rl in xp["sends"] if plens[rl]]
-                recvs = [(st.base + tab[rl] + slot * plens[rl] * isz, plens[rl] * isz, peer) for rl, slot, _, peer in xp["recvs"] if plens[rl]]
-                grouped_exchange(rt, sends, recvs)
-            stacks = (st, tab)
         for pid, out in dest.chunks.items():
             rl = L.pids.index(pid)
             if out.size == 0:
@@ -191,7 +172,7 @@ def _run(opc: int, dest: DArray, src: DArray, dims: int, R: np.dtype, ival):
             g = len(fibres[rl])
             if g:
                 # fold the stack of totals in grid order, seeded with init: one small scan along the stack, its last row is the carry
-                base = stacks[0].base + stacks[1][rl]
+                base = stacks[rl][0]
                 _lib.call("dab_scan", rt.ctx, ccode, opc, ccode, C.c_void_p(base), plens[rl], g, 1, C.c_void_p(carry) if carry else None,
                           C.c_void_p(base))
                 carry = base + (g - 1) * plens[rl] * isz

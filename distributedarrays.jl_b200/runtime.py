@@ -346,8 +346,7 @@ def exchange_stacks(rt, owners: Sequence[int], nbytes: Sequence[int]) -> Stacks:
     """Where the consumers of an exchange collect what they receive: one stack per result chunk ``c``, of ``nbytes[c]`` bytes
     rounded up to 256, on rank ``owners[c]``; each rank's stacks lie back to back in chunk order.  Every rank derives the same
     tables, so a producer knows the offset of a stack inside its consumer's buffer.  With several ranks, and every rank's
-    stacks fitting one bank, the stacks sit in the exchange arena and producers put into ``arena()["peers"][r] + bank +
-    offset``.  Otherwise they sit in a private temporary and arrive by ``grouped_exchange``."""
+    stacks fitting one bank, the stacks sit in the exchange arena; otherwise in a private temporary.  ``deliver`` fills them."""
     tables: Dict[int, Dict[int, int]] = {r: {} for r in range(rt.world)}
     totals = [0] * rt.world
     for c, (r, nb) in enumerate(zip(owners, nbytes)):
@@ -358,6 +357,30 @@ def exchange_stacks(rt, owners: Sequence[int], nbytes: Sequence[int]) -> Stacks:
         return Stacks(tables, True, bank, rt.arena()["peers"][rt.rank] + bank, 0)
     temp = rt.alloc_temp(max(totals[rt.rank], 16))
     return Stacks(tables, False, 0, temp, temp)
+
+
+def deliver(rt, st: Stacks, sends: Sequence, recvs: Sequence):
+    """Moves slabs into the exchange stacks ``st`` of their consumers.  ``sends``: ``(source pointer, bytes, consumer rank, result chunk,
+    byte offset in that chunk's stack)``; ``recvs``: ``(producer rank, result chunk, byte offset, bytes)``, used without the arena only.
+    Sends to this rank's own stacks are device copies, issued first and in list order.  With the arena every other send is a put into
+    its consumer's bank, and every rank then fences the device once, also a rank with nothing to send.  Without it the other sends and
+    the receives go to one ``grouped_exchange`` in list order, so both sides must derive their lists from the same plan.  Zero-byte
+    entries are skipped on both sides."""
+    mine = st.tables[rt.rank]
+    remote = []
+    for src, nb, dst, c, off in sends:
+        if nb and dst == rt.rank:
+            _lib.call("dab_d2d", rt.ctx, C.c_void_p(st.base + mine[c] + off), C.c_void_p(src), nb)
+        elif nb:
+            remote.append((src, nb, dst, c, off))
+    if st.use_arena:
+        peers = rt.arena()["peers"]
+        for src, nb, dst, c, off in remote:
+            _lib.call("dab_d2d", rt.ctx, C.c_void_p(peers[dst] + st.bank + st.tables[dst][c] + off), C.c_void_p(src), nb)
+        fence(rt, "device")                                   # every producer's puts have landed
+    else:
+        grouped_exchange(rt, [(src, nb, dst) for src, nb, dst, _, _ in remote],
+                         [(st.base + mine[c] + off, nb, src) for src, c, off, nb in recvs if nb])
 
 
 def init(workers_per_rank: int = 1, device: Optional[int] = None, use_dist: Optional[bool] = None) -> Runtime:

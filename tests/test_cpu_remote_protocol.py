@@ -180,3 +180,137 @@ def test_exchange_stacks_at_world_1_never_touch_the_arena(dab):
     st = exchange_stacks(rt, owners, nbytes)
     assert st.tables == {0: {0: 0, 1: 3072, 2: 6144, 3: 9216, 4: 12288, 5: 15360, 6: 18432, 7: 21504}}
     assert not st.use_arena and st.temp == 0x5000 and rt.log == [("alloc_temp", 24576)]
+
+
+# ---- deliver: slabs into the exchange stacks ------------------------------------------------------------------------------------------
+
+TABLES = {0: {0: 0, 1: 512}, 1: {2: 0}}
+# (source, bytes, consumer rank, result chunk, offset): a put, a local copy, a zero-byte put, a local copy
+SENDS = [(0x100, 8, 1, 2, 16), (0x200, 16, 0, 1, 32), (0x300, 0, 1, 2, 0), (0x400, 24, 0, 0, 0)]
+RECVS = [(1, 0, 8, 8), (1, 1, 0, 0), (1, 1, 16, 4)]                 # (producer rank, result chunk, offset, bytes)
+
+
+def test_deliver_with_the_arena_puts_then_fences_once_on_every_rank(dab, lib_calls):
+    from darray_b200.runtime import Stacks, deliver
+    bank = 8 << 20
+    rt = StandIn(rank=0)
+    deliver(rt, Stacks(TABLES, True, bank, PEERS[0] + bank, 0), SENDS, RECVS)
+    assert lib_calls == [("dab_d2d", PEERS[0] + bank + 512 + 32, 0x200, 16), ("dab_d2d", PEERS[0] + bank, 0x400, 24),
+                         ("dab_d2d", PEERS[1] + bank + 16, 0x100, 8)]
+    assert rt.log == ["device_barrier"]
+    del lib_calls[:]
+    rt = StandIn(rank=1)                                            # nothing to send: the fence is collective all the same
+    deliver(rt, Stacks(TABLES, True, bank, PEERS[1] + bank, 0), [], [(0, 2, 16, 8)])
+    assert lib_calls == [] and rt.log == ["device_barrier"]
+
+
+def test_deliver_without_the_arena_is_one_grouped_exchange(dab, lib_calls):
+    from darray_b200.runtime import Stacks, deliver
+    rt = StandIn(rank=0)
+    deliver(rt, Stacks(TABLES, False, 0, 0x5000, 0x5000), SENDS, RECVS)
+    assert lib_calls == [("dab_d2d", 0x5000 + 512 + 32, 0x200, 16), ("dab_d2d", 0x5000, 0x400, 24), ("dab_group_start",),
+                         ("dab_send", 0x100, 8, 1), ("dab_recv", 0x5000 + 8, 8, 1), ("dab_recv", 0x5000 + 512 + 16, 4, 1), ("dab_group_end",)]
+    assert rt.log == []
+
+
+def test_deliver_at_world_1_copies_only(dab, lib_calls):
+    from darray_b200.runtime import Stacks, deliver
+    rt = StandIn(world=1)
+    deliver(rt, Stacks({0: {0: 0, 1: 256}}, False, 0, 0x5000, 0x5000), [(0x100, 8, 0, 1, 8), (0x200, 0, 0, 0, 0), (0x300, 4, 0, 0, 0)], [])
+    assert lib_calls == [("dab_d2d", 0x5000 + 256 + 8, 0x100, 8), ("dab_d2d", 0x5000, 0x300, 4)] and rt.log == []
+
+
+# ---- gather_fibres: the slabs of every fibre on the owner of its result chunk, run on both ranks of a world of 2 ------------------------
+
+
+def _reducedim_case(dab, shape, nprocs, region, wpr, isz):
+    from darray_b200._mapreduce import plan_reducedim
+    from darray_b200.layout import shape_of
+    L = dab.make_layout(shape, list(range(1, nprocs + 1)))
+    R, fibres = plan_reducedim(L, region)
+    plens = [int(np.prod(shape_of(ix))) for ix in R.indices]
+    return L, R, fibres, [(plen * isz,) for plen in plens], wpr
+
+
+def _findmax_case(dab, shape, dist, region, wpr, isz):
+    """As ``_findmax._dims`` calls it: values and indices, a fibre of one member gathers nothing."""
+    from darray_b200._mapreduce import plan_reducedim
+    from darray_b200.layout import shape_of
+    L = dab.make_layout(shape, list(range(1, int(np.prod(dist)) + 1)), dist)
+    R, fibres = plan_reducedim(L, region)
+    plens = [int(np.prod(shape_of(ix))) for ix in R.indices]
+    return L, R, [m if len(m) > 1 else [] for m in fibres], [(plen * isz, plen * 8) for plen in plens], wpr
+
+
+def _scan_case(dab, shape, dist, dims, wpr, isz):
+    """As ``_scan._run`` calls it: the carry slabs of every chunk along ``dims``."""
+    from darray_b200._scan import carry_plan
+    from darray_b200.layout import shape_of
+    L = dab.make_layout(shape, list(range(1, int(np.prod(dist)) + 1)), dist)
+    k = dims - 1
+    plens = [int(np.prod([s for a, s in enumerate(shape_of(ix)) if a != k])) for ix in L.indices]
+    return L, L, carry_plan(L, dims), [(plen * isz,) for plen in plens], wpr
+
+
+GATHER_CASES = [("reducedim", args, tables) for kind, args, tables, _ in STACK_CASES if kind == "reducedim"] + [
+    ("findmax", ((14, 9), (2, 3), (2,), 3, 4), None),               # Float32 values of 3 x 7 per stack: a value plane of 84 bytes
+    ("findmax", ((14, 9), (1, 3), (1,), 2, 8), None),               # reduced dim not cut: fibres of one member, nothing moves
+    ("scan", ((30, 20), (2, 4), 2, 4, 8), None),
+    ("scan", ((9, 12), (1, 4), 2, 2, 8), None),
+]
+
+
+def _slab(pid, p):
+    return (pid << 24) | (p << 20)
+
+
+def _gather_on_both_ranks(dab, lib_calls, case, arena):
+    from darray_b200._mapreduce import gather_fibres
+    L, R, fibres, plane_bytes, wpr = case
+    runs = []
+    for rank in (0, 1):
+        rt = StandIn(rank=rank, wpr=wpr, bank_bytes=(8 << 20) if arena else -1)      # -1: not even empty stacks fit
+        del lib_calls[:]
+        slabs = {pid: tuple(_slab(pid, p) for p in range(len(plane_bytes[0]))) for pid in L.pids if rt.rank_of(pid) == rank}
+        st, planes = gather_fibres(rt, L, R, fibres, plane_bytes, slabs)
+        runs.append((rt, st, planes, list(lib_calls)))
+    return runs
+
+
+def _expected_writes(L, fibres, plane_bytes, planes):
+    """Every (address, source, bytes) the owner's fold reads: slot s of plane p of result chunk rl holds member s's slab of plane p."""
+    return sorted((planes[rl][p] + s * nb, _slab(L.pids[m], p), nb) for rl in planes for p, nb in enumerate(plane_bytes[rl]) if nb
+                  for s, m in enumerate(fibres[rl]))
+
+
+@pytest.mark.parametrize("kind, args, tables", GATHER_CASES)
+def test_gather_fibres_with_the_arena_writes_every_slot_once(dab, lib_calls, kind, args, tables):
+    case = {"reducedim": _reducedim_case, "findmax": _findmax_case, "scan": _scan_case}[kind](dab, *args)
+    L, R, fibres, plane_bytes, _ = case
+    runs = _gather_on_both_ranks(dab, lib_calls, case, arena=True)
+    writes, expected = [], []
+    for rank, (rt, st, planes, calls) in enumerate(runs):
+        assert st.use_arena and rt.log == ["arena_next_bank", "device_barrier"]
+        assert tables is None or st.tables == tables
+        assert set(planes) == {rl for rl, p in enumerate(R.pids) if rt.rank_of(p) == rank}
+        assert all(c[0] == "dab_d2d" for c in calls)
+        writes += [c[1:] for c in calls]
+        expected += _expected_writes(L, fibres, plane_bytes, planes)
+    assert sorted(writes) == sorted(expected)
+
+
+@pytest.mark.parametrize("kind, args, tables", GATHER_CASES)
+def test_gather_fibres_without_the_arena_pairs_sends_and_receives(dab, lib_calls, kind, args, tables):
+    case = {"reducedim": _reducedim_case, "findmax": _findmax_case, "scan": _scan_case}[kind](dab, *args)
+    L, R, fibres, plane_bytes, _ = case
+    runs = _gather_on_both_ranks(dab, lib_calls, case, arena=False)
+    for rank, (rt, st, planes, calls) in enumerate(runs):
+        assert not st.use_arena and all(e[0] == "alloc_temp" for e in rt.log)
+        assert tables is None or st.tables == tables
+        other = 1 - rank
+        sends = [c[1:3] for c in runs[other][3] if c[0] == "dab_send" and c[3] == rank]
+        recvs = [c[1:3] for c in calls if c[0] == "dab_recv" and c[3] == other]
+        assert [nb for _, nb in sends] == [nb for _, nb in recvs]    # NCCL pairs them in issue order
+        writes = [c[1:] for c in calls if c[0] == "dab_d2d"] + [(dst, src, nb) for (src, _), (dst, nb) in zip(sends, recvs)]
+        assert sorted(writes) == _expected_writes(L, fibres, plane_bytes, planes)
+        assert all(c[2] for c in calls if c[0] in ("dab_send", "dab_recv"))

@@ -4,8 +4,9 @@
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port 29517 tools/multi_gpu_check.py
 
 Checks, against the CPU oracle regenerated on every rank: sum / maximum with the NCCL all-gather + ordered left fold,
-mapreducedim with the grouped send/recv between-phase, one-sided halo reads over CUDA IPC peer mappings, broadcast across
-mismatched layouts; then times the C5 halo read (256 MiB slab from the next rank) and prints one JSON line per metric (rank 0).
+mapreducedim with the grouped send/recv between-phase, findmax / findmin with dims and cumsum / accumulate along a dim cut
+across ranks, one-sided halo reads over CUDA IPC peer mappings, broadcast across mismatched layouts; then times the C5 halo
+read (256 MiB slab from the next rank) and prints one JSON line per metric (rank 0).
 """
 import ctypes as C
 import json
@@ -74,6 +75,23 @@ def main():
     dI = dab.distribute(Ai, dist=(P, 1))
     assert np.array_equal(dab.to_array(dab.mapreduce(lambda t: t * t, "+", dI, dims=1)), (Ai * Ai).sum(axis=0, keepdims=True))
     log("ok: mapreducedim with cross-rank between-phase")
+
+    # ---- findmax / findmin with dims, and scans, along a dim cut across ranks: (value, index) slabs and scan carries travel between ranks
+    rows, cols = np.indices(A.shape)
+    lin = rows + cols * R + 1                                           # Julia's 1-based column-major linear index
+    for grid in ((P, 1), (1, P)):
+        dB, dI = dab.distribute(A, dist=grid), dab.distribute(Ai, dist=grid)
+        for dims, ax in ((1, 0), (2, 1)):
+            for find, arg in ((dab.findmax, np.argmax), (dab.findmin, np.argmin)):     # NumPy's first index of the extreme is Julia's
+                v, i = find(dB, dims=dims)
+                k = np.expand_dims(arg(A, axis=ax), ax)
+                assert np.array_equal(dab.to_array(v), np.take_along_axis(A, k, ax)), (grid, dims)
+                assert np.array_equal(dab.to_array(i), np.take_along_axis(lin, k, ax)), (grid, dims)
+            assert np.array_equal(dab.to_array(dab.cumsum(dI, dims=dims)), np.cumsum(Ai, axis=ax)), (grid, dims)
+            assert np.allclose(dab.to_array(dab.cumsum(dB, dims=dims)), np.cumsum(A64, axis=ax), rtol=1e-6), (grid, dims)
+            got = dab.to_array(dab.accumulate("max", dB, dims=dims, init=F32(0.25)))
+            assert np.array_equal(got, np.maximum(np.maximum.accumulate(A, axis=ax), F32(0.25))), (grid, dims)
+    log("ok: findmax / findmin with dims, cumsum and accumulate along dims cut across ranks")
 
     # ---- halo reads: one-sided peer loads over CUDA IPC
     dA.share()
