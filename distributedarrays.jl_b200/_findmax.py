@@ -22,7 +22,7 @@ from . import _lib
 from ._broadcast import broadcast, is_ctag
 from ._darray import B200Array, DArray, dab_dtype, is_complex
 from ._mapreduce import _gather_slots, _normalise_region, classify_map, gather_fibres, plan_reducedim
-from .layout import collapse_for_region, shape_of
+from .layout import reduction_passes, shape_of
 
 _SERVED_MAPS = (_lib.MAP_ID, _lib.MAP_ABS, _lib.MAP_ABS2)
 _I64 = C.c_int64
@@ -164,22 +164,15 @@ def _reduce_chunk(rt, d: DArray, pid: int, ch: B200Array, reg_in, which: int, ma
             _lib.call("dab_fill", rt.ctx, code, C.c_void_p(vals.ptr), n, C.c_void_p(np.zeros(1, dtype=np.uint64).ctypes.data))
             _lib.call("dab_fill", rt.ctx, _lib.I64, C.c_void_p(idx.ptr), n, C.c_void_p(np.full(1, -1, dtype=np.int64).ctypes.data))
         return vals, idx
-    runs = collapse_for_region(list(ch.shape), set(reg_in))
-    ext = [e for _, e in runs]
     vals = idx = None
-    for ri in range(len(runs) - 1, -1, -1):
-        if not runs[ri][0]:
-            continue
-        inner = int(np.prod(ext[:ri])) if ri else 1
-        outer = int(np.prod(ext[ri + 1:])) if ri + 1 < len(ext) else 1
+    for inner, red, outer in reduction_passes(ch.shape, reg_in):
         if vals is None:
-            vals, idx = _chunk_pass(rt, code, which, mapc, ch.ptr, 0, inner, ext[ri], outer, gl, d.dtype)
+            vals, idx = _chunk_pass(rt, code, which, mapc, ch.ptr, 0, inner, red, outer, gl, d.dtype)
         else:
-            nv, ni = _chunk_pass(rt, code, which, _lib.MAP_ID, vals.ptr, idx.ptr, inner, ext[ri], outer, gl, d.dtype)
+            nv, ni = _chunk_pass(rt, code, which, _lib.MAP_ID, vals.ptr, idx.ptr, inner, red, outer, gl, d.dtype)
             vals.free()
             idx.free()
             vals, idx = nv, ni
-        ext[ri] = 1
     if vals is None:
         vals, idx = _chunk_pass(rt, code, which, mapc, ch.ptr, 0, ch.size, 1, 1, gl, d.dtype)
     return vals, idx

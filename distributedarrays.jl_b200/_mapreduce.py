@@ -23,7 +23,7 @@ import numpy as np
 from . import _lib
 from ._broadcast import Expr, broadcast, is_ctag, tag_of, trace, _NPT
 from ._darray import B200Array, DArray, component_dtype, dab_dtype, is_complex, np_dtype
-from .layout import Layout, collapse_for_region, ravel, shape_of, unravel
+from .layout import Layout, ravel, reduction_passes, shape_of, unravel
 from .runtime import close_remote_reads, deliver, exchange_stacks, open_remote_reads
 
 _OPS = {"+": _lib.SUM, "add": _lib.SUM, "sum": _lib.SUM, "*": _lib.PROD, "mul": _lib.PROD, "prod": _lib.PROD, "max": _lib.MAX,
@@ -454,23 +454,13 @@ def _normalise_region(dims, ndim: int) -> Tuple[int, ...]:
 def reduce_chunk_dims(rt, ch: B200Array, region_in: Sequence[int], op: int, mapc: int, out_dtype: np.dtype) -> B200Array:
     """``mapreduce(f, op, localpart(A), dims=region)`` (reference src/mapreduce.jl:64) on one chunk.
     Every maximal run of reduced dims is one (inner, reduce, outer) kernel pass, last run first."""
-    shape = list(ch.shape)
-    runs = collapse_for_region(shape, set(region_in))
     cur, cur_dtype, cur_map, owned = ch, ch.dtype, mapc, False
-    # positions of runs: process reduced runs from the last to the first so `inner` stays the untouched prefix
-    ext = [e for _, e in runs]
-    for ri in range(len(runs) - 1, -1, -1):
-        if not runs[ri][0]:
-            continue
-        inner = int(np.prod(ext[:ri])) if ri else 1
-        red = ext[ri]
-        outer = int(np.prod(ext[ri + 1:])) if ri + 1 < len(ext) else 1
+    for inner, red, outer in reduction_passes(ch.shape, region_in):
         nxt = B200Array.empty(rt, (inner * outer,), out_dtype, temp=True)
         _lib.call("dab_reducedim", rt.ctx, dab_dtype(cur_dtype), op, cur_map, C.c_void_p(cur.ptr), inner, red, outer, C.c_void_p(nxt.ptr), 0)
         if owned:
             cur.free()  # stream-ordered: no host sync needed
         cur, cur_dtype, cur_map, owned = nxt, out_dtype, _lib.MAP_ID, True
-        ext[ri] = 1
     rshape = tuple(1 if (k + 1) in region_in else s for k, s in enumerate(ch.shape))
     if not owned:  # nothing reduced (cannot happen when region_in is non-empty)
         return ch

@@ -125,6 +125,12 @@ int32_t dab_flush_pending(dab_ctx* ctx);
         DAB_CUDA((ctx), cudaGetLastError());       \
     } while (0)
 
+// Grow-on-demand device scratch owned by the ctx (*buf of *have bytes): returns at once when it holds `bytes`; otherwise waits for
+// the stream (earlier launches may still use the old buffer), frees it, allocates `bytes` and, with `zero`, clears the new buffer
+// in stream order.  ctx->dim_scratch is shared by the split partials of dab_reducedim, dab_findminmax_dim and dab_gemv: one
+// stream, so never two launches' partials at once.
+int32_t dab_scratch_grow(dab_ctx* ctx, void** buf, size_t* have, size_t bytes, bool zero);
+
 static inline size_t dab_dtype_size(int32_t dt) {
     switch (dt) {
         case DAB_F32: return 4;

@@ -57,6 +57,20 @@ int32_t dab_fail_cuda(dab_ctx* ctx, cudaError_t e, const char* what, const char*
                     (int)e, cudaGetErrorString(e), what, file, line);
 }
 
+int32_t dab_scratch_grow(dab_ctx* ctx, void** buf, size_t* have, size_t bytes, bool zero) {
+    if (*have >= bytes) return DAB_OK;
+    if (*buf) {
+        DAB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        DAB_CUDA(ctx, cudaFree(*buf));
+        *buf = nullptr;
+        *have = 0;
+    }
+    DAB_CUDA(ctx, cudaMalloc(buf, bytes));
+    if (zero) DAB_CUDA(ctx, cudaMemsetAsync(*buf, 0, bytes, ctx->stream));
+    *have = bytes;
+    return DAB_OK;
+}
+
 extern "C" {
 
 int32_t dab_abi_version(void) { return DAB_ABI_VERSION; }

@@ -25,7 +25,6 @@
 
 namespace {
 
-constexpr int FM_UNROLL = 4;
 constexpr unsigned long long FM_NONE = ~0ull;  // "no element yet": loses every tie against a real index
 
 template <typename T> struct FmEnc;
@@ -111,7 +110,7 @@ __global__ void __launch_bounds__(RD_THREADS, 5) findminmax_kernel(const T* __re
 
     const size_t nvec = (n - head) / VPT;
     const int4* xv = reinterpret_cast<const int4*>(x + head);
-    constexpr size_t TILE = (size_t)RD_THREADS * FM_UNROLL;
+    constexpr size_t TILE = (size_t)RD_THREADS * RD_UNROLL;
     const size_t ntiles = nvec / TILE;
     U bk = 0;
     unsigned long long bi = FM_NONE;
@@ -124,11 +123,11 @@ __global__ void __launch_bounds__(RD_THREADS, 5) findminmax_kernel(const T* __re
     for (size_t t = t_end; t > t_beg;) {
         --t;
         const size_t base = t * TILE + threadIdx.x;
-        int4 r[FM_UNROLL];
+        int4 r[RD_UNROLL];
 #pragma unroll
-        for (int u = 0; u < FM_UNROLL; ++u) r[u] = ld_stream(xv + base + (size_t)u * RD_THREADS);
+        for (int u = 0; u < RD_UNROLL; ++u) r[u] = ld_stream(xv + base + (size_t)u * RD_THREADS);
 #pragma unroll
-        for (int u = FM_UNROLL - 1; u >= 0; --u) {
+        for (int u = RD_UNROLL - 1; u >= 0; --u) {
             const Pack<T> p = as_pack<T>(r[u]);
             const unsigned long long i0 = head + (base + (size_t)u * RD_THREADS) * VPT;
 #pragma unroll
@@ -152,37 +151,10 @@ __global__ void __launch_bounds__(RD_THREADS, 5) findminmax_kernel(const T* __re
         for (size_t i = head + nvec * VPT + threadIdx.x; i < n; i += RD_THREADS) acc = R::comb(acc, A{order_key<T, MIN>(map(x[i])), i});
     }
     acc = block_reduce<R>(acc, smem);
-    // two-level last-CTA-out combine over the ticket counters of reduce_kernel (self-resetting; same stream, so never concurrent)
-    A* gpartials = partials + DAB_MAX_REDUCE_BLOCKS;
-    const unsigned int ngroups = (gridDim.x + RD_THREADS - 1) / RD_THREADS;
-    const unsigned int g = blockIdx.x / RD_THREADS;
-    const unsigned int gsize = (g == ngroups - 1) ? gridDim.x - g * RD_THREADS : RD_THREADS;
+    // the ticket counters and partials of reduce_kernel (same stream, so never concurrent)
+    A fin;
+    if (!last_cta_out<R>(acc, partials, counter, smem, is_last, fin)) return;
     if (threadIdx.x == 0) {
-        partials[blockIdx.x] = acc;
-        __threadfence();
-        const unsigned int ticket = atomicAdd(counter + 1 + g, 1u);
-        is_last = (ticket == gsize - 1);
-    }
-    __syncthreads();
-    if (!is_last) return;
-    __threadfence();
-    A v = threadIdx.x < gsize ? partials[(size_t)g * RD_THREADS + threadIdx.x] : R::identity();
-    v = block_reduce<R>(v, smem);
-    if (threadIdx.x == 0) {
-        counter[1 + g] = 0;
-        gpartials[g] = v;
-        __threadfence();
-        const unsigned int ticket = atomicAdd(counter, 1u);
-        is_last = (ticket == ngroups - 1);
-    }
-    __syncthreads();
-    if (!is_last) return;
-    __threadfence();
-    A fin = R::identity();
-    for (unsigned int i = threadIdx.x; i < ngroups; i += RD_THREADS) fin = R::comb(fin, gpartials[i]);
-    fin = block_reduce<R>(fin, smem);
-    if (threadIdx.x == 0) {
-        *counter = 0;
         const T val = map(x[fin.idx]);  // the element itself, mapped: NaN payloads survive
         memset(out, 0, 16);
         memcpy(out, &val, sizeof(T));
@@ -193,16 +165,9 @@ __global__ void __launch_bounds__(RD_THREADS, 5) findminmax_kernel(const T* __re
 
 template <typename T, int FN, bool MIN>
 int32_t launch_findminmax(dab_ctx* ctx, const T* x, size_t n, void* out) {
-    constexpr int VPT = 16 / sizeof(T);
-    size_t head = ((16 - ((uintptr_t)x & 15)) & 15) / sizeof(T);
-    if (head > n) head = n;
-    const size_t tiles = (n - head) / ((size_t)VPT * RD_THREADS * FM_UNROLL);
-    size_t k = 2;  // 32 KiB of input per CTA
-    if ((tiles + k - 1) / k > (size_t)DAB_MAX_REDUCE_BLOCKS) k = (tiles + DAB_MAX_REDUCE_BLOCKS - 1) / DAB_MAX_REDUCE_BLOCKS;
-    size_t grid = (tiles + k - 1) / k;
-    if (grid < 1) grid = 1;
-    findminmax_kernel<T, FN, MIN><<<(unsigned)grid, RD_THREADS, 0, ctx->stream>>>(x, n, head, (FmBest<FmKey<T>>*)ctx->block_partials,
-                                                                                   ctx->counter, out, (int)k);
+    const FlatGrid fg = flat_grid(x, n);
+    findminmax_kernel<T, FN, MIN><<<(unsigned)fg.grid, RD_THREADS, 0, ctx->stream>>>(x, n, fg.head, (FmBest<FmKey<T>>*)ctx->block_partials,
+                                                                                      ctx->counter, out, fg.tiles_per_cta);
     DAB_LAUNCHED(ctx);
     return DAB_OK;
 }
@@ -424,19 +389,6 @@ __global__ void fm_slot_to_out_kernel(const void* __restrict__ slot, FmGlobal gl
     *out_i = gl((unsigned long long)i);
 }
 
-int32_t fm_scratch(dab_ctx* ctx, size_t bytes) {  // the split partials share dab_reducedim's scratch (same stream, never concurrent)
-    if (ctx->dim_scratch_bytes >= bytes) return DAB_OK;
-    if (ctx->dim_scratch) {
-        DAB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        DAB_CUDA(ctx, cudaFree(ctx->dim_scratch));
-        ctx->dim_scratch = nullptr;
-        ctx->dim_scratch_bytes = 0;
-    }
-    DAB_CUDA(ctx, cudaMalloc(&ctx->dim_scratch, bytes));
-    ctx->dim_scratch_bytes = bytes;
-    return DAB_OK;
-}
-
 template <typename T, int FN, bool MIN, bool IDX>
 int32_t launch_fmdim(dab_ctx* ctx, const T* x, const long long* idx_in, size_t inner, size_t red, size_t outer, const FmGlobal& gl, T* out_v,
                      long long* out_i) {
@@ -452,26 +404,19 @@ int32_t launch_fmdim(dab_ctx* ctx, const T* x, const long long* idx_in, size_t i
     // the 16-byte strided kernel: whole vectors of outputs, an aligned base, 4- or 8-byte T, no index input, enough vectors to fill the GPU
     constexpr int VPT = 16 / sizeof(T);
     const bool vec = !IDX && sizeof(T) >= 4 && inner > 1 && inner % VPT == 0 && ((uintptr_t)x & 15) == 0 && nout / VPT >= 4096;
-    int nsplit = 1;
-    size_t want, max_split;
+    int nsplit;
     if (inner == 1) {
         const int G = red >= 64 ? 32 : 4;
-        const size_t target_groups = target_ctas * (RD_THREADS / G);
-        max_split = red / ((size_t)G * 64);  // every lane keeps >= 64 elements of its split
-        want = outer >= target_groups ? 1 : (target_groups + outer - 1) / outer;
+        nsplit = dim_nsplit(outer, target_ctas * (RD_THREADS / G), red / ((size_t)G * 64));  // every lane keeps >= 64 elements of its split
     } else {
         const size_t base_ctas = vec ? (nout / VPT + RD_THREADS - 1) / RD_THREADS : (nout + RD_THREADS - 1) / RD_THREADS;
-        max_split = red / 256;
-        want = base_ctas >= 4 * target_ctas ? 1 : (4 * target_ctas + base_ctas - 1) / base_ctas;
+        nsplit = dim_nsplit(base_ctas, 4 * target_ctas, red / 256);
     }
-    if (max_split < 1) max_split = 1;
-    nsplit = (int)(want < max_split ? want : max_split);
-    if (nsplit > 1024) nsplit = 1024;
     T* pv = nullptr;
     unsigned long long* pi = nullptr;
     if (nsplit > 1) {
         const size_t parts = nout * (size_t)nsplit;
-        int32_t st = fm_scratch(ctx, parts * 16);
+        int32_t st = dab_scratch_grow(ctx, &ctx->dim_scratch, &ctx->dim_scratch_bytes, parts * 16, false);
         if (st != DAB_OK) return st;
         pi = (unsigned long long*)ctx->dim_scratch;
         pv = (T*)(pi + parts);

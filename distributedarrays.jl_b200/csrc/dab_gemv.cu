@@ -469,19 +469,6 @@ __global__ void __launch_bounds__(GV_THREADS) gemv_finish_kernel(const typename 
     y[k] = (T)acc;
 }
 
-int32_t gv_scratch(dab_ctx* ctx, size_t bytes) {
-    if (ctx->dim_scratch_bytes >= bytes) return DAB_OK;
-    if (ctx->dim_scratch) {
-        DAB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        DAB_CUDA(ctx, cudaFree(ctx->dim_scratch));
-        ctx->dim_scratch = nullptr;
-        ctx->dim_scratch_bytes = 0;
-    }
-    DAB_CUDA(ctx, cudaMalloc(&ctx->dim_scratch, bytes));
-    ctx->dim_scratch_bytes = bytes;
-    return DAB_OK;
-}
-
 int ceil_log2(size_t v) {
     int l = 0;
     while (((size_t)1 << l) < v) ++l;
@@ -507,7 +494,7 @@ int32_t launch_n_cfg(dab_ctx* ctx, const T* A, size_t m, size_t n, const T* x, T
     nsplit = (n + cps - 1) / cps;
     Acc* part = nullptr;
     if (nsplit > 1) {
-        int32_t st = gv_scratch(ctx, nsplit * m * sizeof(Acc));
+        int32_t st = dab_scratch_grow(ctx, &ctx->dim_scratch, &ctx->dim_scratch_bytes, nsplit * m * sizeof(Acc), false);
         if (st != DAB_OK) return st;
         part = (Acc*)ctx->dim_scratch;
     }
@@ -554,7 +541,7 @@ int32_t launch_n_phase(dab_ctx* ctx, const T* A, size_t m, size_t n, const T* x,
     size_t cps = (nk + nsplit - 1) / nsplit;
     nsplit = (nk + cps - 1) / cps;
     const size_t ny = nsplit * VEC;
-    int32_t st = gv_scratch(ctx, ny * m * sizeof(Acc));
+    int32_t st = dab_scratch_grow(ctx, &ctx->dim_scratch, &ctx->dim_scratch_bytes, ny * m * sizeof(Acc), false);
     if (st != DAB_OK) return st;
     Acc* part = (Acc*)ctx->dim_scratch;
     DAB_REQUIRE(ctx, gx <= 0x7fffffffull, DAB_ERR_ARG, "dab_gemv: too many row tiles");
@@ -595,7 +582,7 @@ int32_t launch_t(dab_ctx* ctx, const T* A, size_t m, size_t n, const T* x, T* y)
     nsplit = (m + rps - 1) / rps;
     Acc* part = nullptr;
     if (nsplit > 1) {
-        int32_t st = gv_scratch(ctx, nsplit * n * sizeof(Acc));
+        int32_t st = dab_scratch_grow(ctx, &ctx->dim_scratch, &ctx->dim_scratch_bytes, nsplit * n * sizeof(Acc), false);
         if (st != DAB_OK) return st;
         part = (Acc*)ctx->dim_scratch;
     }
@@ -638,7 +625,7 @@ int32_t launch_t_phase(dab_ctx* ctx, const T* A, size_t m, size_t n, const T* x,
     nsplit = (words + wps - 1) / wps;
     Acc* part = nullptr;
     if (nsplit > 1) {
-        int32_t st = gv_scratch(ctx, nsplit * n * sizeof(Acc));
+        int32_t st = dab_scratch_grow(ctx, &ctx->dim_scratch, &ctx->dim_scratch_bytes, nsplit * n * sizeof(Acc), false);
         if (st != DAB_OK) return st;
         part = (Acc*)ctx->dim_scratch;
     }

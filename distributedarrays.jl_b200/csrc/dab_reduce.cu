@@ -23,8 +23,6 @@
 
 namespace {
 
-constexpr int RD_UNROLL = 4;
-
 // What the reduce kernel does with each loaded value before the map.  NoStore: nothing (plain reduction of x).
 struct NoStore {
     template <typename T>
@@ -132,39 +130,10 @@ __global__ void __launch_bounds__(RD_THREADS, RdMinBlocks<T, Map>::value) reduce
             acc = R::comb(acc, R::lift(R::pre(map(st.scalar(x[i], i)))));
     }
     acc = block_reduce<R>(acc, smem);
-    // ---- two-level "last one out" combine: deterministic, no second launch, tail latency of a few microseconds.
-    //  level 1: CTAs form groups of RD_THREADS; the last CTA of a group to finish folds the group's partials (one per thread);
-    //  level 2: the last group to finish folds the <= DAB_MAX_REDUCE_BLOCKS/RD_THREADS group partials and writes the result.
-    A* gpartials = partials + DAB_MAX_REDUCE_BLOCKS;
-    const unsigned int ngroups = (gridDim.x + RD_THREADS - 1) / RD_THREADS;
-    const unsigned int g = blockIdx.x / RD_THREADS;
-    const unsigned int gsize = (g == ngroups - 1) ? gridDim.x - g * RD_THREADS : RD_THREADS;
+    // the last CTA to finish writes the result (tail latency of a few microseconds)
+    A fin;
+    if (!last_cta_out<R>(acc, partials, counter, smem, is_last, fin)) return;
     if (threadIdx.x == 0) {
-        partials[blockIdx.x] = acc;
-        __threadfence();
-        unsigned int ticket = atomicAdd(counter + 1 + g, 1u);
-        is_last = (ticket == gsize - 1);
-    }
-    __syncthreads();
-    if (!is_last) return;
-    __threadfence();
-    A v = threadIdx.x < gsize ? partials[(size_t)g * RD_THREADS + threadIdx.x] : R::identity();
-    v = block_reduce<R>(v, smem);
-    if (threadIdx.x == 0) {
-        counter[1 + g] = 0;  // self-reset for the next launch on this stream
-        gpartials[g] = v;
-        __threadfence();
-        unsigned int ticket = atomicAdd(counter, 1u);
-        is_last = (ticket == ngroups - 1);
-    }
-    __syncthreads();
-    if (!is_last) return;
-    __threadfence();
-    A fin = R::identity();
-    for (unsigned int i = threadIdx.x; i < ngroups; i += RD_THREADS) fin = R::comb(fin, gpartials[i]);
-    fin = block_reduce<R>(fin, smem);
-    if (threadIdx.x == 0) {
-        *counter = 0;
         if constexpr (std::is_arithmetic<A>::value) {
             Out res;
             if (finalize_mode == 1) res = (Out)(fin == (A)n_for_all);  // ALL
@@ -263,15 +232,8 @@ __global__ void __launch_bounds__(RD_THREADS, RdMinBlocks<T, Map>::value) reduce
 
 template <typename T, typename Map, typename R, typename Out, typename St = NoStore>
 int32_t launch_reduce(dab_ctx* ctx, const T* x, size_t n, Map map, void* out, int finalize_mode, St st = St()) {
-    constexpr int VPT = 16 / sizeof(T);
-    size_t head = ((16 - ((uintptr_t)x & 15)) & 15) / sizeof(T);
-    if (head > n) head = n;
-    if constexpr (!std::is_same<St, NoStore>::value) st.yv = reinterpret_cast<int4*>(st.y + head);
-    size_t tiles = (n - head) / ((size_t)VPT * RD_THREADS * RD_UNROLL);
-    size_t k = 2;  // 32 KiB of input per CTA
-    if ((tiles + k - 1) / k > (size_t)DAB_MAX_REDUCE_BLOCKS) k = (tiles + DAB_MAX_REDUCE_BLOCKS - 1) / DAB_MAX_REDUCE_BLOCKS;
-    size_t grid = (tiles + k - 1) / k;
-    if (grid < 1) grid = 1;
+    const FlatGrid fg = flat_grid(x, n);
+    if constexpr (!std::is_same<St, NoStore>::value) st.yv = reinterpret_cast<int4*>(st.y + fg.head);
     FusedComm fc;
     memset(&fc, 0, sizeof(fc));
     if (ctx->fuse_op >= 0 && ctx->mbox_ranks > 1) {
@@ -287,8 +249,8 @@ int32_t launch_reduce(dab_ctx* ctx, const T* x, size_t n, Map map, void* out, in
         fc.nranks = 1;
         fc.op = ctx->fuse_op;
     }
-    reduce_kernel<T, Map, R, Out, St><<<(unsigned)grid, RD_THREADS, 0, ctx->stream>>>(x, n, head, map, (typename R::A*)ctx->block_partials,
-                                                                                      ctx->counter, out, finalize_mode, (long long)n, (int)k, fc, st);
+    reduce_kernel<T, Map, R, Out, St><<<(unsigned)fg.grid, RD_THREADS, 0, ctx->stream>>>(
+        x, n, fg.head, map, (typename R::A*)ctx->block_partials, ctx->counter, out, finalize_mode, (long long)n, fg.tiles_per_cta, fc, st);
     DAB_LAUNCHED(ctx);
     return DAB_OK;
 }

@@ -1,4 +1,5 @@
-// dab_reduce_traits.cuh -- reduction traits, map functors and block-level reduction shared by dab_reduce.cu / dab_reducedim.cu
+// dab_reduce_traits.cuh -- reduction traits, map functors, block-level reduction and the launch plumbing shared by the reduction
+// kernels (dab_reduce.cu, dab_reducedim.cu, dab_findminmax.cu; dab_scan.cu uses the traits)
 #pragma once
 #include <type_traits>
 
@@ -7,6 +8,38 @@
 namespace {
 
 constexpr int RD_THREADS = 256;
+constexpr int RD_UNROLL = 4;  // 16-byte loads in flight per thread in the flat-grid kernels
+
+// ---- flat grid of the whole-chunk kernels (reduce_kernel, findminmax_kernel) ----------------------------------------------------
+// x[0, head) is the misaligned head, then tiles of RD_THREADS * RD_UNROLL 16-byte vectors.  CTA b owns the tiles_per_cta consecutive
+// tiles from b * tiles_per_cta: 32 KiB of input per CTA (2 tiles), more once the grid would exceed DAB_MAX_REDUCE_BLOCKS, which is
+// what keeps one partial per CTA inside ctx->block_partials.
+struct FlatGrid {
+    size_t head, grid;
+    int tiles_per_cta;
+};
+template <typename T>
+FlatGrid flat_grid(const T* x, size_t n) {
+    constexpr int VPT = 16 / sizeof(T);
+    size_t head = ((16 - ((uintptr_t)x & 15)) & 15) / sizeof(T);
+    if (head > n) head = n;
+    const size_t tiles = (n - head) / ((size_t)VPT * RD_THREADS * RD_UNROLL);
+    size_t k = 2;
+    if ((tiles + k - 1) / k > (size_t)DAB_MAX_REDUCE_BLOCKS) k = (tiles + DAB_MAX_REDUCE_BLOCKS - 1) / DAB_MAX_REDUCE_BLOCKS;
+    size_t grid = (tiles + k - 1) / k;
+    if (grid < 1) grid = 1;
+    return FlatGrid{head, grid, (int)k};
+}
+
+// ---- split count of the dims kernels (dab_reducedim.cu, dab_findminmax.cu) ------------------------------------------------------
+// Splits of the reduced extent that bring `have` work units up to `target`: ceil(target / have) when have < target, at most
+// max_split (taken as >= 1) and 1024.  The partials of the splits go to ctx->dim_scratch.
+inline int dim_nsplit(size_t have, size_t target, size_t max_split) {
+    if (max_split < 1) max_split = 1;
+    const size_t want = have >= target ? 1 : (target + have - 1) / have;
+    const int nsplit = (int)(want < max_split ? want : max_split);
+    return nsplit > 1024 ? 1024 : nsplit;
+}
 
 // ---------------------------------------------------------------------------------------------------------------
 // Reduce "traits": V = value type after the map, W = value type inside a tile step, A = accumulator carried across tiles /
@@ -203,6 +236,49 @@ __device__ __forceinline__ typename R::A block_reduce(typename R::A acc, typenam
         for (int d = 4; d > 0; d >>= 1) acc = R::comb(acc, shfl_down<A>(acc, d));
     }
     return acc;  // valid in thread 0
+}
+
+// ---- two-level "last one out" combine of the flat-grid kernels: deterministic, no second launch ---------------------------------
+//  level 1: CTAs form groups of RD_THREADS; the last CTA of a group to finish folds the group's partials (one per thread);
+//  level 2: the last group to finish folds the <= DAB_MAX_REDUCE_BLOCKS / RD_THREADS group partials.
+// partials is ctx->block_partials: DAB_MAX_REDUCE_BLOCKS CTA partials, then the group partials.  counter is ctx->counter: [0] counts
+// the groups, [1 + g] the CTAs of group g; the last CTA zeroes them again for the next launch on the stream.  acc is this CTA's
+// block_reduce result (valid in thread 0); smem and is_last are the kernel's shared scratch (a __shared__ flag declared here instead
+// changes the SASS of every caller).  Returns true in the last CTA only, where thread 0 holds the combined value in fin.
+template <typename R>
+__device__ __forceinline__ bool last_cta_out(typename R::A acc, typename R::A* partials, unsigned int* counter, typename R::A* smem, bool& is_last,
+                                             typename R::A& fin) {
+    using A = typename R::A;
+    A* gpartials = partials + DAB_MAX_REDUCE_BLOCKS;
+    const unsigned int ngroups = (gridDim.x + RD_THREADS - 1) / RD_THREADS;
+    const unsigned int g = blockIdx.x / RD_THREADS;
+    const unsigned int gsize = (g == ngroups - 1) ? gridDim.x - g * RD_THREADS : RD_THREADS;
+    if (threadIdx.x == 0) {
+        partials[blockIdx.x] = acc;
+        __threadfence();
+        const unsigned int ticket = atomicAdd(counter + 1 + g, 1u);
+        is_last = (ticket == gsize - 1);
+    }
+    __syncthreads();
+    if (!is_last) return false;
+    __threadfence();
+    A v = threadIdx.x < gsize ? partials[(size_t)g * RD_THREADS + threadIdx.x] : R::identity();
+    v = block_reduce<R>(v, smem);
+    if (threadIdx.x == 0) {
+        counter[1 + g] = 0;
+        gpartials[g] = v;
+        __threadfence();
+        const unsigned int ticket = atomicAdd(counter, 1u);
+        is_last = (ticket == ngroups - 1);
+    }
+    __syncthreads();
+    if (!is_last) return false;
+    __threadfence();
+    A f = R::identity();
+    for (unsigned int i = threadIdx.x; i < ngroups; i += RD_THREADS) f = R::comb(f, gpartials[i]);
+    fin = block_reduce<R>(f, smem);
+    if (threadIdx.x == 0) *counter = 0;
+    return true;
 }
 
 // ---- complex element types: Cplx<T> (ComplexF32 / ComplexF64) -------------------------------------------------------------------

@@ -336,19 +336,6 @@ __global__ void __launch_bounds__(RD_THREADS) rdim_finish_kernel(const typename 
     }
 }
 
-int32_t ensure_scratch(dab_ctx* ctx, size_t bytes) {
-    if (ctx->dim_scratch_bytes >= bytes) return DAB_OK;
-    if (ctx->dim_scratch) {
-        DAB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        DAB_CUDA(ctx, cudaFree(ctx->dim_scratch));
-        ctx->dim_scratch = nullptr;
-        ctx->dim_scratch_bytes = 0;
-    }
-    DAB_CUDA(ctx, cudaMalloc(&ctx->dim_scratch, bytes));
-    ctx->dim_scratch_bytes = bytes;
-    return DAB_OK;
-}
-
 template <typename T, typename Map, typename R, typename Out>
 int32_t launch_rdim(dab_ctx* ctx, const T* x, size_t inner, size_t red, size_t outer, Map map, Out* out, int accumulate) {
     using A = typename R::A;
@@ -365,14 +352,10 @@ int32_t launch_rdim(dab_ctx* ctx, const T* x, size_t inner, size_t red, size_t o
             return launch_group<T, Map, R, Out, 2>(ctx, x, red, outer, map, out, accumulate);
         }
         // split long runs when there are too few of them; keep every split >= 16 KiB of input
-        size_t max_split = red * sizeof(T) / 16384;
-        if (max_split < 1) max_split = 1;
-        size_t want = outer >= target_ctas ? 1 : (target_ctas + outer - 1) / outer;
-        int nsplit = (int)(want < max_split ? want : max_split);
-        if (nsplit > 1024) nsplit = 1024;
+        const int nsplit = dim_nsplit(outer, target_ctas, red * sizeof(T) / 16384);
         A* partials = nullptr;
         if (nsplit > 1) {
-            int32_t st = ensure_scratch(ctx, outer * (size_t)nsplit * sizeof(A));
+            int32_t st = dab_scratch_grow(ctx, &ctx->dim_scratch, &ctx->dim_scratch_bytes, outer * (size_t)nsplit * sizeof(A), false);
             if (st != DAB_OK) return st;
             partials = (A*)ctx->dim_scratch;
         }
@@ -391,14 +374,10 @@ int32_t launch_rdim(dab_ctx* ctx, const T* x, size_t inner, size_t red, size_t o
     size_t base_ctas = vec ? (inner * outer / (16 / sizeof(T)) + RD_THREADS - 1) / RD_THREADS : (inner * outer + RD_THREADS - 1) / RD_THREADS;
     // split r so that the work items fill >= 4 waves of the persistent grid (a 1.08-wave launch loses ~45 % to the tail), while
     // every split keeps >= 256 rows so that the partial buffer stays < 1 % of the input
-    size_t max_split = red / 256;
-    if (max_split < 1) max_split = 1;
-    size_t want = base_ctas >= 4 * target_ctas ? 1 : (4 * target_ctas + base_ctas - 1) / base_ctas;
-    int nsplit = (int)(want < max_split ? want : max_split);
-    if (nsplit > 1024) nsplit = 1024;
+    const int nsplit = dim_nsplit(base_ctas, 4 * target_ctas, red / 256);
     A* partials = nullptr;
     if (nsplit > 1) {
-        int32_t st = ensure_scratch(ctx, inner * outer * (size_t)nsplit * sizeof(A));
+        int32_t st = dab_scratch_grow(ctx, &ctx->dim_scratch, &ctx->dim_scratch_bytes, inner * outer * (size_t)nsplit * sizeof(A), false);
         if (st != DAB_OK) return st;
         partials = (A*)ctx->dim_scratch;
     }

@@ -349,27 +349,13 @@ __global__ void fill_identity_kernel(typename S::A* __restrict__ out, size_t n) 
     for (size_t k = (size_t)blockIdx.x * SC_THREADS + threadIdx.x; k < n; k += (size_t)gridDim.x * SC_THREADS) out[k] = S::identity();
 }
 
-int32_t scan_grow(dab_ctx* ctx, void** buf, size_t* have, size_t bytes, bool zero) {
-    if (*have >= bytes) return DAB_OK;
-    if (*buf) {
-        DAB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        DAB_CUDA(ctx, cudaFree(*buf));
-        *buf = nullptr;
-        *have = 0;
-    }
-    DAB_CUDA(ctx, cudaMalloc(buf, bytes));
-    if (zero) DAB_CUDA(ctx, cudaMemsetAsync(*buf, 0, bytes, ctx->stream));
-    *have = bytes;
-    return DAB_OK;
-}
-
 template <typename T, typename Out, typename S>
 int32_t launch_flat(dab_ctx* ctx, const T* x, Out* y, size_t n, size_t len, const typename S::A* carry, typename S::A* totals) {
     const unsigned long long ntiles = (n + SC_TILE - 1) / SC_TILE;
     const size_t need = SC_HEAD_BYTES + (size_t)ntiles * sizeof(LookbackWord);
     if (ctx->scan_dev_bytes < need) {
         // fresh words are zero (never ready); the ticket counter restarts at 0
-        int32_t st = scan_grow(ctx, &ctx->scan_dev, &ctx->scan_dev_bytes, need + need / 4, true);
+        int32_t st = dab_scratch_grow(ctx, &ctx->scan_dev, &ctx->scan_dev_bytes, need + need / 4, true);
         if (st != DAB_OK) return st;
         ctx->scan_tickets = 0;
     }
@@ -416,7 +402,7 @@ int32_t launch_strided(dab_ctx* ctx, const T* x, Out* y, size_t inner, size_t le
         return DAB_OK;
     };
     if (nseg == 1) return run(y, carry, nullptr, totals);
-    int32_t st = scan_grow(ctx, &ctx->scan_scratch, &ctx->scan_scratch_bytes, nseg * nout * sizeof(A), false);
+    int32_t st = dab_scratch_grow(ctx, &ctx->scan_scratch, &ctx->scan_scratch_bytes, nseg * nout * sizeof(A), false);
     if (st != DAB_OK) return st;
     A* segs = (A*)ctx->scan_scratch;
     st = run(nullptr, nullptr, nullptr, segs);                           // pass 1: segment totals from the identity, [nout][nseg]

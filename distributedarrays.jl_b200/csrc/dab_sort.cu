@@ -476,19 +476,8 @@ __global__ void sort_small_kernel(const typename SortKey<T>::U* __restrict__ in,
 
 int32_t sort_scratch(dab_ctx* ctx, size_t dev_bytes) {
     if (!ctx->sort_host) DAB_CUDA(ctx, cudaMallocHost(&ctx->sort_host, 8 * 256 * sizeof(unsigned long long) + 4096));
-    if (ctx->sort_dev_bytes < dev_bytes) {
-        if (ctx->sort_dev) {
-            DAB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-            DAB_CUDA(ctx, cudaFree(ctx->sort_dev));
-            ctx->sort_dev = nullptr;
-            ctx->sort_dev_bytes = 0;
-        }
-        DAB_CUDA(ctx, cudaMalloc(&ctx->sort_dev, dev_bytes));
-        // the look-back words carry an epoch, so the scratch is cleared ONCE, here (epoch 0 is never used by a pass)
-        DAB_CUDA(ctx, cudaMemsetAsync(ctx->sort_dev, 0, dev_bytes, ctx->stream));
-        ctx->sort_dev_bytes = dev_bytes;
-    }
-    return DAB_OK;
+    // the look-back words carry an epoch, so the scratch is cleared ONCE, when it is allocated (epoch 0 is never used by a pass)
+    return dab_scratch_grow(ctx, &ctx->sort_dev, &ctx->sort_dev_bytes, dev_bytes, true);
 }
 
 constexpr size_t SORT_PLAN_BYTES = 65536;   // SortPlan + the staging areas of dab_sorted_split, ahead of the look-back words

@@ -217,3 +217,15 @@ def collapse_for_region(shape: Sequence[int], region: Sequence[int]):
         else:
             runs.append([red, int(s)])
     return [(r, e) for r, e in runs]
+
+
+def reduction_passes(shape: Sequence[int], region: Sequence[int]):
+    """Yield the ``(inner, reduce, outer)`` kernel passes of a reduction of a column-major chunk over ``region`` (1-based dims):
+    one per maximal run of reduced dims, last run first, so that ``inner`` is always the untouched prefix.  Each pass sees the
+    extents the passes before it left (their runs collapsed to 1)."""
+    runs = collapse_for_region(shape, set(region))
+    ext = [e for _, e in runs]
+    for ri in range(len(runs) - 1, -1, -1):
+        if runs[ri][0]:
+            yield int(np.prod(ext[:ri])), ext[ri], int(np.prod(ext[ri + 1:]))
+            ext[ri] = 1

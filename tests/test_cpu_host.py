@@ -120,6 +120,16 @@ def test_collapse_for_region(dab):
     assert c((4, 5, 6), {2}) == [(False, 4), (True, 5), (False, 6)]
 
 
+def test_reduction_passes(dab):
+    p = lambda shape, region: list(dab.layout.reduction_passes(shape, region))
+    assert p((32768, 16384), {1}) == [(1, 32768, 16384)]
+    assert p((32768, 16384), {2}) == [(32768, 16384, 1)]
+    assert p((4, 5, 6), {1, 2}) == [(1, 20, 6)]
+    assert p((4, 5, 6), {1, 3}) == [(20, 6, 1), (1, 4, 5)]      # last run first; the first pass leaves (4, 5, 1)
+    assert p((2, 3, 4, 5, 6), {2, 4}) == [(24, 5, 6), (2, 3, 24)]
+    assert p((4, 5), {3}) == []                                  # no reduced dim in the chunk
+
+
 # ------------------------------------------------------------------------------------------------ tracer / promotion / lowering
 def test_tracer_promotion_follows_julia():
     from darray_b200 import abs2, ifelse, sqrt
