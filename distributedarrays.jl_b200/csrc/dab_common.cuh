@@ -62,13 +62,6 @@ struct dab_ctx {
     void* scan_scratch;     // scan: segment totals of the split strided path
     size_t scan_scratch_bytes;
     long long opt_combine_timeout_ms;  // dab_set_option("combine_timeout_ms"): how long the fused combine waits for a peer (default 120 s)
-    long long opt_gemm_kc;  // dab_set_option("gemm_kc"): k extent summed inside tensor memory before a partial tile is drained (default 64)
-    int opt_gemm_rawhi;     // dab_set_option("gemm_rawhi"): 1 = raw fp32 tile as the tf32 "hi" operand (hardware truncation), 0 = RN split
-    int opt_gemm_simt;      // dab_set_option("gemm_simt"): 1 = force the SIMT tile kernel for Float32 (A/B measurements)
-    int opt_gemv_phase;     // dab_set_option("gemv_phase"): 1 (default) = phase-class kernel for A*x, 0 = the single-wave aligned / unit-wise pair
-    int opt_gemv_t_cols;    // dab_set_option("gemv_t_cols"): columns one thread of the A'*x kernel carries (4 or 8)
-    int opt_gemv_t_waves;   // dab_set_option("gemv_t_waves"): waves of CTAs the A'*x kernel is split into
-    int opt_spmv_group;     // dab_set_option("spmv_group"): lanes per row of dab_spmv (1, 2, 4, 8, 16 or 32); 0 (default) = from nnz / rows
     int opt_ew_tma;         // dab_set_option("ew_tma"): route aligned unary elementwise launches through the TMA-staged kernel
     dab_pending_affine pending;  // at most one deferred dab_affine; launched by the next entry or consumed by dab_reduce
     int defer_off;          // set by dab_stream: foreign work on the raw stream expects every call to be queued already

@@ -119,9 +119,6 @@ int32_t dab_init(int32_t device, dab_ctx** out) {
     ctx->nranks = 1;
     ctx->fuse_op = -1;
     ctx->opt_combine_timeout_ms = 120000;
-    ctx->opt_gemv_phase = 1;
-    ctx->opt_gemv_t_waves = 4;
-    ctx->opt_gemv_t_cols = 8;
     ctx->cache = new (std::nothrow) dab_alloc_cache();
 #define INIT_CUDA(call)                                                     \
     do {                                                                    \
@@ -228,8 +225,9 @@ int32_t dab_stream(dab_ctx* ctx, void** stream) {
     return DAB_OK;
 }
 
-// Tuning / experiment switches.  "ew_tma" = 1: unary elementwise kernels (dab_affine, dab_unary, dab_binary_scalar) use the
-// TMA-staged shared-memory ring instead of the default flat LDG/STG kernel (same results; measured slower, see dab_elementwise.cu).
+// Two switches.  "ew_tma" = 1: unary elementwise kernels (dab_affine, dab_unary, dab_binary_scalar) use the TMA-staged
+// shared-memory ring instead of the default flat LDG/STG kernel (same results; measured slower, see dab_elementwise.cu).
+// "combine_timeout_ms": how long the fused combine waits for a peer before it reports a dead rank.
 int32_t dab_set_option(dab_ctx* ctx, const char* key, int64_t value) {
     if (!ctx || !key) return dab_fail(ctx, DAB_ERR_ARG, "null argument");
     if (ctx->pending.active) {  // no DAB_ENTER here: a deferred dab_affine launches as it was called, before the switch changes
@@ -238,38 +236,6 @@ int32_t dab_set_option(dab_ctx* ctx, const char* key, int64_t value) {
     }
     if (strcmp(key, "ew_tma") == 0) {
         ctx->opt_ew_tma = value != 0;
-        return DAB_OK;
-    }
-    if (strcmp(key, "gemm_kc") == 0) {
-        ctx->opt_gemm_kc = value;
-        return DAB_OK;
-    }
-    if (strcmp(key, "gemm_rawhi") == 0) {
-        ctx->opt_gemm_rawhi = value != 0;
-        return DAB_OK;
-    }
-    if (strcmp(key, "gemv_phase") == 0) {
-        ctx->opt_gemv_phase = value != 0;
-        return DAB_OK;
-    }
-    if (strcmp(key, "gemv_t_cols") == 0) {
-        if (value != 4 && value != 8) return dab_fail(ctx, DAB_ERR_ARG, "gemv_t_cols must be 4 or 8");
-        ctx->opt_gemv_t_cols = (int)value;
-        return DAB_OK;
-    }
-    if (strcmp(key, "gemv_t_waves") == 0) {
-        if (value < 1 || value > 64) return dab_fail(ctx, DAB_ERR_ARG, "gemv_t_waves must be in 1..64");
-        ctx->opt_gemv_t_waves = (int)value;
-        return DAB_OK;
-    }
-    if (strcmp(key, "spmv_group") == 0) {
-        if (value != 0 && value != 1 && value != 2 && value != 4 && value != 8 && value != 16 && value != 32)
-            return dab_fail(ctx, DAB_ERR_ARG, "spmv_group must be 0 (automatic) or a power of two up to 32");
-        ctx->opt_spmv_group = (int)value;
-        return DAB_OK;
-    }
-    if (strcmp(key, "gemm_simt") == 0) {
-        ctx->opt_gemm_simt = value != 0;
         return DAB_OK;
     }
     if (strcmp(key, "combine_timeout_ms") == 0) {

@@ -14,7 +14,7 @@
 //     which wgmma does not accept for tf32 from shared memory, so every thread loads its fragment from the swizzled tile and splits it there.
 //   * two consumer warpgroups issue wgmma.mma_async m64n128k8 (a_hi x [b_hi | b_lo]) and m64n64k8 (a_lo x b_hi); CTA tile 128 x 64
 //   * two-level accumulation, because the tensor core does not round its fp32 accumulator to nearest (the error grows with the number of
-//     accumulating instructions): the register accumulators only sum KC consecutive k (default 64), then each finished partial tile is
+//     accumulating instructions): the register accumulators only sum TG_KC = 64 consecutive k, then each finished partial tile is
 //     added to fp32 registers with round-to-nearest
 // Everything else (Float64, Int32, Int64; Float32 operands whose base / leading dimension are not 16-byte aligned, which TMA cannot
 // address) -> gemm_simt_kernel: shared-memory tiled FMA kernel, fp64 with DFMA, integers wrap like Julia's.
@@ -111,6 +111,7 @@ int32_t launch_simt(dab_ctx* ctx, int transA, size_t m, size_t n, size_t k, cons
 
 // ======================================================================= wgmma 3xTF32 kernel ==========================================
 constexpr int TG_M = 128, TG_N = 64, TG_K = 32, TG_STAGES = 6;
+constexpr int TG_KC = 64;                                        // k extent of one register partial (a multiple of TG_K)
 constexpr int TG_A_BYTES = TG_M * TG_K * 4;                      // 16 KiB: one A tile (128 x 32 fp32)
 constexpr int TG_B_BYTES = TG_N * TG_K * 4;                      // 8 KiB: one B tile (32 x 64 fp32), K-major rows of 128 bytes
 constexpr int TG_STAGE_BYTES = TG_A_BYTES + 2 * TG_B_BYTES;      // A, B_hi, B_lo (B_lo right behind B_hi: [B_hi | B_lo] is one N = 128 operand)
@@ -205,7 +206,6 @@ __device__ __forceinline__ void fence_operand(float& r) { asm volatile("" : "+f"
 // the 13 dropped bits, clear them"; IADD / LOP3 / FSUB run at full rate, cvt.rna.tf32.f32 does not.  Both halves have their low 13 bits
 // cleared, so the products do not depend on how the tensor core treats the bits a tf32 operand drops.
 __device__ __forceinline__ float tf32_rn(float v) { return __uint_as_float((__float_as_uint(v) + 0x1000u) & 0xffffe000u); }
-__device__ __forceinline__ float tf32_trunc(float v) { return __uint_as_float(__float_as_uint(v) & 0xffffe000u); }
 __device__ __forceinline__ float4 split_tf32(float4& v) {   // v <- hi (tf32, round to nearest), returns lo = tf32_rn(v - hi)
     float4 lo;
     const float hx = tf32_rn(v.x), hy = tf32_rn(v.y), hz = tf32_rn(v.z), hw = tf32_rn(v.w);
@@ -217,20 +217,7 @@ __device__ __forceinline__ float4 split_tf32(float4& v) {   // v <- hi (tf32, ro
     return lo;
 }
 
-// RAWHI (opt-in, dab_set_option "gemm_rawhi"): the B tile stays in shared memory as it arrived and serves as the "hi" operand (the tensor
-// core reads an fp32 word as tf32 by ignoring its low 13 mantissa bits), so the converters only write "lo" = tf32_rn(v - trunc_tf32(v)) and
-// the shared-memory traffic of the conversion drops from 3 to 2 tile passes.  A is split in registers: hi = trunc_tf32(v), same remainder.
-// The always-positive remainder of a truncation makes the dropped a_lo*b_lo term a bias; the default keeps the round-to-nearest split.
-__device__ __forceinline__ float4 lo_of_trunc(const float4& v) {   // tf32_rn(v - trunc_tf32(v)), the remainder of the hardware's truncation
-    float4 lo;
-    lo.x = tf32_rn(__fsub_rn(v.x, tf32_trunc(v.x)));
-    lo.y = tf32_rn(__fsub_rn(v.y, tf32_trunc(v.y)));
-    lo.z = tf32_rn(__fsub_rn(v.z, tf32_trunc(v.z)));
-    lo.w = tf32_rn(__fsub_rn(v.w, tf32_trunc(v.w)));
-    return lo;
-}
-
-template <bool TA, bool RAWHI>
+template <bool TA>
 __global__ void __launch_bounds__(TG_THREADS, 1) gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
                                                                     float* __restrict__ C, size_t ldc, uint32_t m, uint32_t n, uint32_t k, uint32_t kc_blocks) {
     extern __shared__ unsigned char tg_raw[];
@@ -278,7 +265,7 @@ __global__ void __launch_bounds__(TG_THREADS, 1) gemm_tf32x3_kernel(const __grid
     // acc[0, 32): partial hi*hi product of the current k chunk; acc[32, 64) and acc2: the correction products a_hi*b_lo and a_lo*b_hi (kept
     // apart so that the two wgmmas of a k-step do not write the same registers, which would serialize them).  The tensor
     // core does not round its fp32 accumulator to nearest, and that error grows with the number of accumulating instructions: a partial only
-    // sums gemm_kc consecutive k before it is added to `sum` with round-to-nearest.
+    // sums TG_KC consecutive k before it is added to `sum` with round-to-nearest.
     float acc[64], acc2[32], sum[32];
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
@@ -296,13 +283,9 @@ __global__ void __launch_bounds__(TG_THREADS, 1) gemm_tf32x3_kernel(const __grid
         for (int q = 0; q < TG_B_BYTES / 16 / TG_CONSUMERS; ++q) {
             const int i = tid + q * TG_CONSUMERS;
             float4 v = bh[i];
-            if (RAWHI) {
-                bl[i] = lo_of_trunc(v);
-            } else {
-                const float4 lo = split_tf32(v);
-                bh[i] = v;
-                bl[i] = lo;
-            }
+            const float4 lo = split_tf32(v);
+            bh[i] = v;
+            bl[i] = lo;
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");                       // generic-proxy stores -> visible to wgmma
         asm volatile("bar.sync 1, %0;" ::"n"(TG_CONSUMERS) : "memory");
@@ -326,7 +309,7 @@ __global__ void __launch_bounds__(TG_THREADS, 1) gemm_tf32x3_kernel(const __grid
                 const uint32_t off = TA ? r * 32u + ((((kk >> 2) ^ (r & 7u))) << 2) + (kk & 3u)
                                         : (r >> 5) * 1024u + kk * 32u + (((((r & 31u) >> 2) ^ (kk & 7u))) << 2) + (r & 3u);
                 const float v = As[off];
-                const float hi = RAWHI ? tf32_trunc(v) : tf32_rn(v);
+                const float hi = tf32_rn(v);
                 ah[e] = __float_as_uint(hi);
                 al[e] = __float_as_uint(tf32_rn(__fsub_rn(v, hi)));
             }
@@ -402,10 +385,6 @@ int32_t launch_tf32x3(dab_ctx* ctx, int transA, size_t m, size_t n, size_t k, co
     if (st != DAB_OK) return st;
     const size_t gx = (m + TG_M - 1) / TG_M, gy = (n + TG_N - 1) / TG_N;
     if (gx > 0x7fffffffull || gy > 65535ull) return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_gemm: tile grid %zu x %zu too large", gx, gy);
-    long long kc = ctx->opt_gemm_kc > 0 ? ctx->opt_gemm_kc : 64;
-    uint32_t kc_blocks = (uint32_t)((kc + TG_K - 1) / TG_K);
-    if (kc_blocks < 1) kc_blocks = 1;
-    const bool raw = ctx->opt_gemm_rawhi != 0;
     auto launch = [&](auto kern) -> int32_t {
         static std::mutex mu;
         static std::map<std::pair<const void*, int>, bool> done;   // the >48 KiB opt-in is per (function, device)
@@ -418,12 +397,10 @@ int32_t launch_tf32x3(dab_ctx* ctx, int transA, size_t m, size_t n, size_t k, co
             }
         }
         dim3 grid((unsigned)gx, (unsigned)gy);
-        kern<<<grid, TG_THREADS, TG_SMEM_BYTES, ctx->stream>>>(mapA, mapB, C, ldc, (uint32_t)m, (uint32_t)n, (uint32_t)k, kc_blocks);
+        kern<<<grid, TG_THREADS, TG_SMEM_BYTES, ctx->stream>>>(mapA, mapB, C, ldc, (uint32_t)m, (uint32_t)n, (uint32_t)k, TG_KC / TG_K);
         return DAB_OK;
     };
-    int32_t rc;
-    if (transA) rc = raw ? launch(gemm_tf32x3_kernel<true, true>) : launch(gemm_tf32x3_kernel<true, false>);
-    else rc = raw ? launch(gemm_tf32x3_kernel<false, true>) : launch(gemm_tf32x3_kernel<false, false>);
+    const int32_t rc = transA ? launch(gemm_tf32x3_kernel<true>) : launch(gemm_tf32x3_kernel<false>);
     if (rc != DAB_OK) return rc;
     DAB_LAUNCHED(ctx);
     return DAB_OK;
@@ -447,7 +424,7 @@ int32_t dab_gemm(dab_ctx* ctx, int32_t dtype, int32_t transA, size_t m, size_t n
     switch (dtype) {
         case DAB_F32: {
             const bool big = m < ((size_t)1 << 31) && n < ((size_t)1 << 31) && k < ((size_t)1 << 31);
-            if (ctx->opt_gemm_simt == 0 && k > 0 && big && tma_ok(A, lda) && tma_ok(B, ldb))
+            if (k > 0 && big && tma_ok(A, lda) && tma_ok(B, ldb))
                 return launch_tf32x3(ctx, transA, m, n, k, (const float*)A, lda, (const float*)B, ldb, (float*)C, ldc);
             return launch_simt<float>(ctx, transA, m, n, k, (const float*)A, lda, (const float*)B, ldb, (float*)C, ldc);
         }

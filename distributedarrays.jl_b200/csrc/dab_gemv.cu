@@ -61,14 +61,17 @@ __device__ __forceinline__ GvVec<T, VEC> gv_load_cached(const T* p) {
 
 // ---- r = A x ----------------------------------------------------------------------------------------------------------------
 // grid (row tiles, column splits); lrt = log2(RT).  A thread owns R groups of VEC consecutive rows, RT*VEC rows apart, so a CTA covers
-// R*RT*VEC CONSECUTIVE rows of every column it touches: 4 KiB of contiguous DRAM per column in both variants -- R = 1 with 16-byte loads
-// when the columns are 16-byte aligned, R = 4 unit-wise loads otherwise (leading dimension not a multiple of 16 bytes, e.g. the 37/36-row
-// splits defaultdist produces; one row group per thread would read 1 KiB bursts scattered over many DRAM pages).
-template <typename T, int VEC, int U, int R>
+// R*RT*VEC CONSECUTIVE rows of every column it touches.
+// Loads in flight per thread: U = 4 columns x R = 1 row group, for 16-byte and unit-wise loads (leading dimension not a multiple of 16
+// bytes) alike.  For the unit-wise loads (U, R) = (4, 1) gave a steady rate in the design sweep; more loads in flight -- (8, 1), (16, 1),
+// (4, 2), (2, 4), (4, 4) -- swung widely with the column stride.
+constexpr int GV_N_U = 4, GV_N_R = 1;
+template <typename T, int VEC>
 __global__ void __launch_bounds__(GV_THREADS) gemv_n_kernel(const T* __restrict__ A, size_t m, size_t n, const T* __restrict__ x, int lrt,
                                                             size_t cols_per_split, typename GvAcc<T>::type* __restrict__ part,
                                                             T* __restrict__ y) {
     using Acc = typename GvAcc<T>::type;
+    constexpr int U = GV_N_U, R = GV_N_R;
     __shared__ Acc sh[GV_THREADS * VEC * R];
     const int RT = 1 << lrt, CL = GV_THREADS >> lrt;
     const int ri = threadIdx.x & (RT - 1), cl = threadIdx.x >> lrt;
@@ -475,16 +478,17 @@ int ceil_log2(size_t v) {
     return l;
 }
 
-template <typename T, int VEC, int U, int R>
-int32_t launch_n_cfg(dab_ctx* ctx, const T* A, size_t m, size_t n, const T* x, T* y) {
+template <typename T, int VEC>
+int32_t launch_n(dab_ctx* ctx, const T* A, size_t m, size_t n, const T* x, T* y) {
     using Acc = typename GvAcc<T>::type;
+    constexpr int U = GV_N_U, R = GV_N_R;
     const size_t rvecs = (m + (size_t)VEC * R - 1) / ((size_t)VEC * R);   // row groups-of-R
     int lrt = ceil_log2(rvecs);
     if (lrt > 8) lrt = 8;
     const int RT = 1 << lrt, CL = GV_THREADS >> lrt;
     const size_t gx = (rvecs + RT - 1) / RT;
     // one full wave of resident CTAs (no partial second wave), but every CTA keeps >= 16 column steps per lane
-    const size_t slots = (size_t)ctx->sm_count * (size_t)dab_resident_ctas((const void*)gemv_n_kernel<T, VEC, U, R>, GV_THREADS);
+    const size_t slots = (size_t)ctx->sm_count * (size_t)dab_resident_ctas((const void*)gemv_n_kernel<T, VEC>, GV_THREADS);
     const size_t want = slots / gx > 0 ? slots / gx : 1;
     size_t max_split = n / ((size_t)CL * U * 4);
     if (max_split < 1) max_split = 1;
@@ -500,21 +504,13 @@ int32_t launch_n_cfg(dab_ctx* ctx, const T* A, size_t m, size_t n, const T* x, T
     }
     DAB_REQUIRE(ctx, gx <= 0x7fffffffull, DAB_ERR_ARG, "dab_gemv: too many row tiles");
     dim3 grid((unsigned)gx, (unsigned)nsplit);
-    gemv_n_kernel<T, VEC, U, R><<<grid, GV_THREADS, 0, ctx->stream>>>(A, m, n, x, lrt, cps, part, y);
+    gemv_n_kernel<T, VEC><<<grid, GV_THREADS, 0, ctx->stream>>>(A, m, n, x, lrt, cps, part, y);
     DAB_LAUNCHED(ctx);
     if (part) {
         gemv_finish_kernel<T><<<(unsigned)((m + GV_THREADS - 1) / GV_THREADS), GV_THREADS, 0, ctx->stream>>>(part, m, (int)nsplit, y);
         DAB_LAUNCHED(ctx);
     }
     return DAB_OK;
-}
-
-// loads in flight per thread: U = 4 columns x R = 1 row group.  For the unit-wise variant (leading dimension not a multiple of 16 bytes)
-// (U, R) = (4, 1) gave a steady rate in the design sweep; more loads in flight -- (8, 1), (16, 1), (4, 2), (2, 4), (4, 4) -- swung
-// widely with the column stride, so the steady shape is kept.
-template <typename T, int VEC>
-int32_t launch_n(dab_ctx* ctx, const T* A, size_t m, size_t n, const T* x, T* y) {
-    return launch_n_cfg<T, VEC, 4, 1>(ctx, A, m, n, x, y);
 }
 
 // the phase-class variant (columns not 16-byte aligned): VEC classes x nsplit column splits in gridDim.y, always through the partials
@@ -570,7 +566,7 @@ int32_t launch_t(dab_ctx* ctx, const T* A, size_t m, size_t n, const T* x, T* y)
     const size_t cols_per_cta = (size_t)CB * COLS * G;
     const size_t gx = (n + cols_per_cta - 1) / cols_per_cta;
     const size_t slots = (size_t)ctx->sm_count * (size_t)dab_resident_ctas((const void*)gemv_t_kernel<T, VEC, COLS>, GV_THREADS);
-    const size_t waves = (ctx->opt_gemv_t_waves > 0 && n >= 64) ? (size_t)ctx->opt_gemv_t_waves : 1;
+    const size_t waves = n >= 64 ? 4 : 1;
     const size_t want = waves * slots / gx > 0 ? waves * slots / gx : 1;
     const size_t unit = (size_t)LI * VEC;  // rows one sweep step covers; splits start on a multiple of it (keeps 16-B alignment)
     size_t max_split = m / (unit * 16);
@@ -614,7 +610,7 @@ int32_t launch_t_phase(dab_ctx* ctx, const T* A, size_t m, size_t n, const T* x,
     const size_t cols_per_cta = (size_t)CB * COLS * G;
     const size_t gx = ((nk + cols_per_cta - 1) / cols_per_cta) * VEC;
     const size_t slots = (size_t)ctx->sm_count * (size_t)dab_resident_ctas((const void*)gemv_t_phase_kernel<T, VEC, COLS>, GV_THREADS);
-    const size_t waves = ctx->opt_gemv_t_waves > 0 ? (size_t)ctx->opt_gemv_t_waves : 1;
+    const size_t waves = 4;
     const size_t want = waves * slots / gx > 0 ? waves * slots / gx : 1;
     size_t max_split = words / ((size_t)LI * 16);
     if (max_split < 1) max_split = 1;
@@ -660,22 +656,22 @@ int32_t gemv_t(dab_ctx* ctx, int32_t trans, const T* A, size_t m, size_t n, cons
     // 16-byte loads need every column start 16-byte aligned: base aligned and m a multiple of VEC (x too for the A' x sweep)
     const bool vec = ((uintptr_t)A % 16 == 0) && (m % VEC == 0) && (!trans || (uintptr_t)x % 16 == 0);
     if (!trans) {
-        // The phase-class kernel is the default for every chunk big enough to matter: 16-byte loads whatever the alignment of the
-        // columns, and four waves of CTAs (faster than the single-wave kernel on aligned chunks and than unit-wise loads on misaligned
-        // ones when it was designed).  dab_set_option("gemv_phase", 0) restores the round-1 pair.
+        // The phase-class kernel serves every chunk big enough to matter: 16-byte loads whatever the alignment of the columns, and
+        // four waves of CTAs (faster than the single-wave kernel on aligned chunks and than unit-wise loads on misaligned ones when it
+        // was designed).
         // Where it pays: the VEC class partials cost 2*VEC*m carriers of traffic (16/n of the Float32 matrix bytes) and a short column
         // leaves row lanes idle -- an aligned chunk switches kernels only when that is below 2 % (measured 4194304 x 128: 5.8 vs 6.4
         // TB/s, 128 x 4194304: 3.0 vs 5.4), a misaligned one as soon as it beats the unit-wise loads' -35 %.
-        const bool phase_ok = ctx->opt_gemv_phase && (uintptr_t)A % sizeof(T) == 0;
+        const bool phase_ok = (uintptr_t)A % sizeof(T) == 0;
         if (phase_ok && (vec ? (m >= 4096 && n >= 1024) : (m >= 256 && n >= 64))) return launch_n_phase<T, VEC>(ctx, A, m, n, x, y);
         if (vec) return launch_n<T, VEC>(ctx, A, m, n, x, y);
         return launch_n<T, 1>(ctx, A, m, n, x, y);
     }
     // columns a thread carries (x is loaded once per COLS column elements): 8 with 16-byte loads (faster than 4 on a large Float32
-    // chunk when it was designed), dab_set_option("gemv_t_cols", 4) for the A/B measurement
-    if (ctx->opt_gemv_t_cols == 8 && vec && n >= 64) return launch_t<T, VEC, 8>(ctx, A, m, n, x, y);
-    // misaligned columns: the phase-class kernel keeps the 16-byte loads (gemv_phase = 0: unit-wise loads, the round-1 kernel)
-    if (!vec && ctx->opt_gemv_phase && (uintptr_t)A % sizeof(T) == 0 && (uintptr_t)x % sizeof(T) == 0 && m >= 256 && n >= 64)
+    // chunk when it was designed)
+    if (vec && n >= 64) return launch_t<T, VEC, 8>(ctx, A, m, n, x, y);
+    // misaligned columns: the phase-class kernel keeps the 16-byte loads
+    if (!vec && (uintptr_t)A % sizeof(T) == 0 && (uintptr_t)x % sizeof(T) == 0 && m >= 256 && n >= 64)
         return launch_t_phase<T, VEC, 4>(ctx, A, m, n, x, y);   // 4 columns per thread: 8 cost 128 registers here (6.4-6.8 vs 5.4-6.1 TB/s)
     return vec ? launch_t<T, VEC, 4>(ctx, A, m, n, x, y) : launch_t<T, 1, 4>(ctx, A, m, n, x, y);
 }

@@ -102,9 +102,8 @@ int32_t launch_spmv(dab_ctx* ctx, size_t nrows, const long long* ptr, const int3
     return DAB_OK;
 }
 
-// G: the smallest power of two >= the mean row length, 1..32 (dab_set_option("spmv_group", G) pins it)
-int spmv_group(const dab_ctx* ctx, size_t nrows, size_t nnz) {
-    if (ctx->opt_spmv_group) return ctx->opt_spmv_group;
+// G: the smallest power of two >= the mean row length, 1..32
+int spmv_group(size_t nrows, size_t nnz) {
     const size_t mean = nrows ? (nnz + nrows - 1) / nrows : 0;
     int g = 1;
     while (g < 32 && (size_t)g < mean) g <<= 1;
@@ -113,7 +112,7 @@ int spmv_group(const dab_ctx* ctx, size_t nrows, size_t nnz) {
 
 template <typename T>
 int32_t spmv_t(dab_ctx* ctx, size_t nrows, size_t nnz, const long long* ptr, const int32_t* idx, const void* val, const void* x, void* out) {
-    switch (spmv_group(ctx, nrows, nnz)) {
+    switch (spmv_group(nrows, nnz)) {
         case 1: return launch_spmv<T, 1>(ctx, nrows, ptr, idx, val, x, out);
         case 2: return launch_spmv<T, 2>(ctx, nrows, ptr, idx, val, x, out);
         case 4: return launch_spmv<T, 4>(ctx, nrows, ptr, idx, val, x, out);

@@ -138,9 +138,8 @@ int32_t dab_device_info(dab_ctx* ctx, int32_t* device, int32_t* sm_count, size_t
 /* the ctx's cudaStream_t (as void*), so a host runtime can order its own work after ours.  Queues a held-back
  * dab_affine and stops holding any back on this ctx from then on. */
 int32_t dab_stream(dab_ctx* ctx, void** stream);
-/* tuning switches; "combine_timeout_ms" = wall-clock bound of the fused combine's wait for a peer; "ew_tma" = 1 routes aligned unary elementwise launches through the TMA-staged (cp.async.bulk + mbarrier
- * ring) kernel instead of the default flat LDG/STG kernel -- identical results, measured slower (DESIGN.md section 3); "spmv_group" = lanes per row of
- * dab_spmv (1, 2, 4, 8, 16 or 32; 0 = chosen from nnz / rows) -- identical results, every group size folds in storage order. */
+/* two switches; "combine_timeout_ms" = wall-clock bound of the fused combine's wait for a peer; "ew_tma" = 1 routes aligned unary elementwise launches through the TMA-staged (cp.async.bulk + mbarrier
+ * ring) kernel instead of the default flat LDG/STG kernel -- identical results, measured slower (DESIGN.md section 3).  Any other key is DAB_ERR_ARG. */
 int32_t dab_set_option(dab_ctx* ctx, const char* key, int64_t value);
 /* number of kernels this ctx has launched so far (bench.py's gpu_launches claim). */
 int32_t dab_launch_count(dab_ctx* ctx, uint64_t* launches);
@@ -359,7 +358,7 @@ int32_t dab_csc_to_csr(dab_ctx* ctx, int32_t dtype, size_t m, size_t n, size_t n
  * stored k x m (lda); B is k x n (ldb).  Replaces  localpart(A) * convert(localtype(B), Bjk)  and the transpose / adjoint forms of
  * _matmatmul! (src/linalg.jl:218-226); the caller scales C by beta and adds alpha * R per tile exactly as the reference (:232-252).
  * Float32 with 16-byte aligned bases and leading dimensions: TMA-fed wgmma (3xTF32 error-compensated, register partials drained
- * every "gemm_kc" k for fp32 round-to-nearest accumulation); otherwise and for Float64 / Int32 / Int64: shared-memory tiled FMA kernel
+ * every 64 k for fp32 round-to-nearest accumulation); otherwise and for Float64 / Int32 / Int64: shared-memory tiled FMA kernel
  * (integers wrap like Julia's).  n == 1 with a dense A (lda == its row count) IS a matrix-vector product and is served by K9
  * (dab_gemv: one read of A at the HBM roofline).  R is overwritten. */
 int32_t dab_gemm(dab_ctx* ctx, int32_t dtype, int32_t transA, size_t m, size_t n, size_t k, const void* A, size_t lda, const void* B,

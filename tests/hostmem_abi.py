@@ -306,7 +306,7 @@ class HostMemABI:
 
     # -- linear algebra tiles (NumPy stand-ins: only the HOST logic around them is under test) and small utilities
     def dab_set_option(self, ctx, key, value):
-        return 0
+        return 0 if key in (b"ew_tma", b"combine_timeout_ms") else 2     # DAB_ERR_ARG: an unknown key, as the library
 
     def dab_h2d_2d(self, ctx, dptr, dpitch, hptr, hpitch, row_bytes, cols):
         for c in range(int(cols)):

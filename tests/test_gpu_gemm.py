@@ -55,7 +55,7 @@ SHAPES = [(128, 128, 32), (128, 128, 256), (256, 384, 512), (100, 60, 44), (37, 
 
 @pytest.mark.parametrize("m,n,k", SHAPES)
 @pytest.mark.parametrize("transA", [False, True])
-def test_gemm_f32(dab, rt1, m, n, k, transA):
+def test_gemm_f32_tma_and_simt_kernels(dab, rt1, m, n, k, transA):
     rng = np.random.default_rng(m * 7 + n * 3 + k)
     for kind in ("uniform", "normal"):
         A = (rng.random((k, m) if transA else (m, k)) if kind == "uniform" else rng.standard_normal((k, m) if transA else (m, k))).astype(F32)
@@ -67,18 +67,15 @@ def test_gemm_f32(dab, rt1, m, n, k, transA):
             ldb = (k + 3) // 4 * 4 if pad else k
             R = gemm(dab, rt1, A, B, transA, lda, ldb)
             check_float(R, A, B, transA, 2e-6)
-    # the SIMT kernel on the same data
-    rt1.set_option("gemm_simt", 1)
-    try:
-        R2 = gemm(dab, rt1, A, B, transA)
-        check_float(R2, A, B, transA, 2e-6 * max(1.0, k / 512))
-    finally:
-        rt1.set_option("gemm_simt", 0)
+    # the SIMT kernel on the same data: a leading dimension of A that is not a multiple of 4 is one TMA cannot address
+    ra = A.shape[0]
+    R2 = gemm(dab, rt1, A, B, transA, ra if ra % 4 else ra + 1)
+    check_float(R2, A, B, transA, 2e-6 * max(1.0, k / 512))
 
 
 def test_gemm_f32_relative_1e6_on_positive_data(dab, rt1):
     """Uniform [0,1) data (the bench's distribution): every entry of the tensor-core product within 1e-6 RELATIVE of the fp64 product,
-    for a long contraction, thanks to the two-level accumulation (register partials of gemm_kc k, fp32 round-to-nearest between them)."""
+    for a long contraction, thanks to the two-level accumulation (register partials of 64 k, fp32 round-to-nearest between them)."""
     rng = np.random.default_rng(5)
     m, n, k = 256, 256, 8192
     A, B = rng.random((m, k)).astype(F32), rng.random((k, n)).astype(F32)
@@ -106,27 +103,3 @@ def test_gemm_other_types(dab, rt1, dtype, transA):
                 want = (A.T if transA else A) @ B                       # NumPy integer matmul wraps too
             assert R.dtype == np.dtype(dtype) and np.array_equal(R, want)
 
-
-@pytest.mark.parametrize("transA", [False, True])
-def test_gemm_f32_raw_hi_operand(dab, rt1, transA):
-    """``gemm_rawhi`` = 1: the raw fp32 tile is the tf32 "hi" operand (the tensor core ignores the low 13 mantissa bits) and only the
-    remainder tile is written by the converters.  Same accuracy contract as the round-to-nearest split."""
-    rng = np.random.default_rng(77)
-    m, n, k = 384, 256, 4096
-    A = rng.random((k, m) if transA else (m, k)).astype(F32)
-    B = rng.random((k, n)).astype(F32)
-    rt1.set_option("gemm_rawhi", 1)
-    try:
-        R = gemm(dab, rt1, A, B, transA)
-    finally:
-        rt1.set_option("gemm_rawhi", 0)
-    want = (A.T if transA else A).astype(np.float64) @ B.astype(np.float64)
-    assert float(np.abs(R - want).max() / np.abs(want).min()) <= 1e-6
-    An = rng.standard_normal(A.shape).astype(F32)
-    Bn = rng.standard_normal(B.shape).astype(F32)
-    rt1.set_option("gemm_rawhi", 1)
-    try:
-        R = gemm(dab, rt1, An, Bn, transA)
-    finally:
-        rt1.set_option("gemm_rawhi", 0)
-    check_float(R, An, Bn, transA, 2e-6)

@@ -108,6 +108,15 @@ def test_affine_tma_variant(dab, rt1, n, dtype):
         rt1.set_option("ew_tma", 0)
 
 
+@pytest.mark.parametrize("key,value", [("gemm_rawhi", 0), ("gemm_simt", 0), ("gemm_kc", 64), ("gemv_phase", 1), ("gemv_t_cols", 8),
+                                       ("gemv_t_waves", 4), ("spmv_group", 0)])
+def test_set_option_refuses_kernel_choices(dab, rt1, key, value):
+    """dab_set_option knows "ew_tma" and "combine_timeout_ms" only.  The GEMM, GEMV and SpMV kernels are chosen from the operands,
+    so naming one of those choices, even with the value they are chosen with, is an unknown key."""
+    with pytest.raises(dab.ArgumentError):
+        rt1.set_option(key, value)
+
+
 def test_affine_is_not_fma(dab, rt1):
     """a*x+b must be two roundings (Julia never contracts): pick values where fma(a,x,b) != (a*x)+b."""
     n = 1 << 16

@@ -18,7 +18,7 @@ if HOSTMEM:                                                     # the emulated C
     import sparse_hostmem
     sparse_hostmem.install()
 DTYPES = [np.float32, np.float64, np.int32, np.int64]
-GROUPS = (0,) if HOSTMEM else (0, 1, 2, 4, 8, 16, 32)      # 0: chosen from nnz / rows; the emulation has no group sizes
+GROUPS = (0,) if HOSTMEM else (0, 1, 2, 4, 8, 16, 32)      # 0: the mix as it is; the emulation has no group sizes
 
 
 def _values(rng, dtype, k, special=True):
@@ -79,24 +79,41 @@ def _spmv(dab, rt, ptr, idx, val, x):
     return got
 
 
+def _spmv_group(nrows, nnz):
+    """Lanes per row that ``spmv_group()`` (dab_sparse.cu) picks: the smallest power of two >= the mean row length, 1..32."""
+    mean = -(-nnz // nrows) if nrows else 0
+    return min(32, 1 << max(mean - 1, 0).bit_length())
+
+
+def _pad_to_group(lengths, g):
+    """The row-length mix followed by empty rows (to lower the mean) or rows of 32 entries (to raise it) until it selects G = g."""
+    nrows, nnz = len(lengths), int(sum(lengths))
+    empty = full = 0
+    while (G := _spmv_group(nrows, nnz)) != g:
+        if G > g:
+            empty += 1
+        else:
+            full += 1
+            nnz += 32
+        nrows += 1
+    return list(lengths) + [0] * empty + [32] * full
+
+
 @pytest.mark.parametrize("dtype", DTYPES)
-def test_spmv_kernel_every_group_size(dab, rt1, dtype):
-    """K18 on rows of 0, 1, 31, 33, 1024 and 10^5 entries mixed with short rows, under every lanes-per-row choice: the ordered fold, bit for
-    bit."""
+def test_spmv_kernel_padded_to_every_group_size(dab, rt1, dtype):
+    """K18 on rows of 0, 1, 31, 33, 1024 and 10^5 entries mixed with short rows, each mix as it is and padded until its mean row length
+    selects each lanes-per-row choice: the ordered fold, bit for bit."""
     rng = np.random.default_rng(101)
     ncols = 120000
     x = _values(rng, dtype, ncols)
-    for lengths in ([1] * 300, [31] * 70 + [0] * 5, [33] * 64, [1024] * 9 + [0, 1, 2], [100000, 3, 0, 31, 33, 1024], [0] * 17,
-                    list(rng.integers(0, 40, 2000))):
-        ptr, idx, val = _rows_csr(rng, dtype, lengths, ncols)
-        want = so.fold_rows(ptr, idx, val, x)
+    for mix in ([1] * 300, [31] * 70 + [0] * 5, [33] * 64, [1024] * 9 + [0, 1, 2], [100000, 3, 0, 31, 33, 1024], [0] * 17,
+                list(rng.integers(0, 40, 2000))):
         for g in GROUPS:
-            rt1.set_option("spmv_group", g)
-            try:
-                got = _spmv(dab, rt1, ptr, idx, val, x)
-            finally:
-                rt1.set_option("spmv_group", 0)
-            assert so.same_bits(got, want), (np.dtype(dtype), lengths[:4], g)
+            lengths = _pad_to_group(mix, g) if g else mix
+            ptr, idx, val = _rows_csr(rng, dtype, lengths, ncols)
+            assert g == 0 or _spmv_group(len(lengths), int(ptr[-1])) == g
+            got = _spmv(dab, rt1, ptr, idx, val, x)
+            assert so.same_bits(got, so.fold_rows(ptr, idx, val, x)), (np.dtype(dtype), mix[:4], g)
 
 
 @pytest.mark.parametrize("dtype", DTYPES)
