@@ -779,8 +779,13 @@ int32_t launch_transpose(dab_ctx* ctx, void* dst, size_t dst_ld, const void* src
     return DAB_OK;
 }
 
-// conj(transpose) of one box of Complex{T}: transpose_box_kernel's tile walk with 8- / 16-byte elements, the imaginary component negated
-// (its sign bit flipped, as Julia's conj) between the shared-memory tile and the store.
+// Julia's conj negates the imaginary part by flipping its sign bit, so a NaN keeps its payload; an arithmetic negation would give the
+// canonical NaN on the GPU.
+__device__ __forceinline__ float flip_sign(float x) { return __uint_as_float(__float_as_uint(x) ^ 0x80000000u); }
+__device__ __forceinline__ double flip_sign(double x) { return __longlong_as_double(__double_as_longlong(x) ^ (long long)0x8000000000000000ull); }
+
+// conj(transpose) of one box of Complex{T}: transpose_box_kernel's tile walk with 8- / 16-byte elements, the imaginary component's
+// sign bit flipped between the shared-memory tile and the store.
 template <typename T, int TR_TILE>
 __global__ void __launch_bounds__(256) adjoint_box_kernel(Cplx<T>* __restrict__ dst, size_t dst_ld, const Cplx<T>* __restrict__ src,
                                                           size_t src_ld, size_t rows, size_t cols, unsigned tiles_r) {
@@ -804,7 +809,7 @@ __global__ void __launch_bounds__(256) adjoint_box_kernel(Cplx<T>* __restrict__ 
         const size_t c = c0 + tx, r = r0 + k;
         if (r < rows && c < cols) {
             Cplx<T> z = tile[tx][k];
-            z.im = -z.im;
+            z.im = flip_sign(z.im);
             dst[c + r * dst_ld] = z;
         }
     }

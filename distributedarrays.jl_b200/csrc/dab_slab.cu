@@ -11,8 +11,6 @@
 // source geometry allows (16 B when source base / pitches / row length are 16-byte multiples); when the destination is less
 // aligned than the source the value is stored in smaller pieces (local HBM stores are cheap).  A contiguous slab whose source
 // start is not 16-byte aligned is split on the host into head (< 16 B) + 16-byte-aligned body + tail.
-#include <cstdlib>
-
 #include "dab_common.cuh"
 
 namespace {
@@ -65,35 +63,18 @@ __global__ void __launch_bounds__(256) copy_box_kernel(char* __restrict__ dst, c
         if (ok[u]) store_as<U, S>(dst + doff[u], v[u]);
 }
 
-int copy_unroll() {
-    static int u = 0;
-    if (!u) {
-        const char* e = getenv("DAB_COPY_UNROLL");
-        u = (e && atoi(e) == 4) ? 4 : 8;
-    }
-    return u;
-}
+constexpr int COPY_UNROLL = 8;
 
 template <typename U, typename S>
 int32_t launch_copy(dab_ctx* ctx, char* dst, const char* src, const BoxGeom& g) {
     unsigned long long total = g.upr * g.e1 * g.e2 * g.e3;
     if (total == 0) return DAB_OK;
-    const bool small = total < (1ull << 31);
-    const int un = copy_unroll();
-    const size_t work = (size_t)((total + 256ull * un - 1) / (256ull * un));
-#define LAUNCH(I, UN)                                                                                          \
-    do {                                                                                                       \
-        if (work > 0x7fffffffull) return dab_fail(ctx, DAB_ERR_ARG, "box too large for one launch");           \
-        copy_box_kernel<U, S, I, UN><<<(unsigned)work, 256, 0, ctx->stream>>>(dst, src, g, (I)total);          \
-    } while (0)
-    if (small) {
-        if (un == 4) LAUNCH(unsigned int, 4);
-        else LAUNCH(unsigned int, 8);
-    } else {
-        if (un == 4) LAUNCH(unsigned long long, 4);
-        else LAUNCH(unsigned long long, 8);
-    }
-#undef LAUNCH
+    const size_t work = (size_t)((total + 256ull * COPY_UNROLL - 1) / (256ull * COPY_UNROLL));
+    if (work > 0x7fffffffull) return dab_fail(ctx, DAB_ERR_ARG, "box too large for one launch");
+    if (total < (1ull << 31))
+        copy_box_kernel<U, S, unsigned int, COPY_UNROLL><<<(unsigned)work, 256, 0, ctx->stream>>>(dst, src, g, (unsigned int)total);
+    else
+        copy_box_kernel<U, S, unsigned long long, COPY_UNROLL><<<(unsigned)work, 256, 0, ctx->stream>>>(dst, src, g, total);
     DAB_LAUNCHED(ctx);
     return DAB_OK;
 }

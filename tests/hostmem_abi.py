@@ -10,7 +10,7 @@ missing.  Nothing here says anything about the CUDA kernels; those are checked b
 
 Emulated entry points: lifecycle and buffers (alloc / free / h2d / d2h / d2d / fill / rand_u01), the elementwise family the real
 ``run_local`` routes to (``dab_affine``, ``dab_unary``, ``dab_binary``, ``dab_binary_scalar``, ``dab_broadcast_expr`` as the strided 4-D
-box walk of the NVRTC kernel), ``dab_copy_box`` / ``dab_gather_box`` (halo and view copies), ``dab_reduce`` / ``dab_mapreduce_all`` /
+box walk of the NVRTC kernel), ``dab_copy_box`` / ``dab_gather_box`` (halo and view copies, 1- to 16-byte elements), ``dab_transpose_box`` / ``dab_adjoint_box``, ``dab_reduce`` / ``dab_mapreduce_all`` /
 ``dab_reducedim`` / ``dab_mapreduce_expr`` (sums in a wide carrier: an order-free stand-in for the kernels' trees, compared at tolerance),
 ``dab_sort`` / ``dab_sort_by_key`` / ``dab_sorted_split``.  The host-only entry points (``dab_reduce_result_dtype``,
 ``dab_combine_ordered``) are the real library's.
@@ -35,6 +35,7 @@ import julia_scalar as jl
 F32, F64, I32, I64, U8 = range(5)
 _NP = {F32: np.dtype(np.float32), F64: np.dtype(np.float64), I32: np.dtype(np.int32), I64: np.dtype(np.int64), U8: np.dtype(np.uint8)}
 SIGN64 = np.uint64(0x8000000000000000)
+_UNIT = {1: np.dtype(np.uint8), 2: np.dtype(np.uint16), 4: np.dtype(np.uint32), 8: np.dtype(np.uint64), 16: np.dtype("V16")}   # data-movement units
 
 
 # ---- dab_sort_key.cuh in NumPy ------------------------------------------------------------------------------------------------
@@ -292,12 +293,17 @@ class HostMemABI:
         self.launches += 1
         return 0
 
-    # -- dab_copy_box (4-D box, column-major)
+    # -- dab_copy_box (4-D box, column-major); refusals as the library's: an element width it has no unit for, a box past either array
     def dab_copy_box(self, ctx, elem_bytes, dst, dst_shape, dst_off, src, src_shape, src_off, extent):
         dsh, dof, ssh, sof, ext = map(_sz4, (dst_shape, dst_off, src_shape, src_off, extent))
-        dt = {1: np.uint8, 2: np.uint16, 4: np.uint32, 8: np.uint64}[int(elem_bytes)]
-        if min(ext) == 0:
-            return 0
+        if int(elem_bytes) not in _UNIT:
+            return 2                                               # DAB_ERR_ARG
+        dt = _UNIT[int(elem_bytes)]
+        for d in range(4):
+            if ext[d] == 0:
+                return 0
+            if sof[d] + ext[d] > ssh[d] or dof[d] + ext[d] > dsh[d]:
+                return 4                                           # DAB_ERR_DIM_MISMATCH
         d = _view(dst, int(np.prod(dsh)), dt).reshape(dsh, order="F")
         s = _view(src, int(np.prod(ssh)), dt).reshape(ssh, order="F")
         d[tuple(slice(o, o + e) for o, e in zip(dof, ext))] = s[tuple(slice(o, o + e) for o, e in zip(sof, ext))]
@@ -339,18 +345,32 @@ class HostMemABI:
         self.launches += 1
         return 0
 
-    def dab_transpose_box(self, ctx, elem_bytes, dst, dst_ld, src, src_ld, rows, cols):
-        dt = {1: np.uint8, 2: np.uint16, 4: np.uint32, 8: np.uint64}[int(elem_bytes)]
+    def dab_transpose_box(self, ctx, elem_bytes, dst, dst_ld, src, src_ld, rows, cols, conj=False):
         rows, cols, dst_ld, src_ld = int(rows), int(cols), int(dst_ld), int(src_ld)
-        if rows and cols:
-            s_ = _view(src, src_ld * (cols - 1) + rows, dt)
-            d_ = _view(dst, dst_ld * (rows - 1) + cols, dt)
-            from numpy.lib.stride_tricks import as_strided
-            sv = as_strided(s_, shape=(rows, cols), strides=(dt().itemsize, src_ld * dt().itemsize))
-            dv = as_strided(d_, shape=(cols, rows), strides=(dt().itemsize, dst_ld * dt().itemsize))
-            dv[...] = sv.T
+        if rows == 0 or cols == 0:
+            return 0
+        if src_ld < rows or dst_ld < cols:
+            return 4                                               # DAB_ERR_DIM_MISMATCH
+        if int(elem_bytes) not in _UNIT:
+            return 2
+        dt = _UNIT[int(elem_bytes)]
+        es = dt.itemsize
+        s_ = _view(src, src_ld * (cols - 1) + rows, dt)
+        d_ = _view(dst, dst_ld * (rows - 1) + cols, dt)
+        from numpy.lib.stride_tricks import as_strided
+        sv = as_strided(s_, shape=(rows, cols), strides=(es, src_ld * es))
+        dv = as_strided(d_, shape=(cols, rows), strides=(es, dst_ld * es))
+        dv[...] = sv.T
+        if conj:                                                   # Julia's conj: the imaginary part's sign bit flipped, NaN payloads kept
+            top = as_strided(_view(dst, (dst_ld * (rows - 1) + cols) * es, np.uint8)[es - 1:], shape=(cols, rows), strides=(es, dst_ld * es))
+            top ^= np.uint8(0x80)
         self.launches += 1
         return 0
+
+    def dab_adjoint_box(self, ctx, dtype, dst, dst_ld, src, src_ld, rows, cols):
+        if int(dtype) not in (6, 7):
+            return 6                                               # DAB_ERR_UNSUPPORTED: not a complex dtype
+        return self.dab_transpose_box(ctx, 8 if int(dtype) == 6 else 16, dst, dst_ld, src, src_ld, rows, cols, conj=True)
 
     def dab_accumulate_stack(self, ctx, dtype, y, n, beta, alpha, stack, stride, count):
         dt, n = _NP[int(dtype)], int(n)
@@ -370,10 +390,14 @@ class HostMemABI:
     # -- dab_gather_box: per dimension the element offset of coordinate t is t * stride (possibly negative) or table[t]
     def dab_gather_box(self, ctx, elem_bytes, ndim, dst, dst_strides, dst_index, src, src_strides, src_index, extent):
         nd = int(ndim)
+        if not 1 <= nd <= 8:
+            return 6                                               # DAB_ERR_UNSUPPORTED
         ext = [int(extent[k]) for k in range(nd)]
         if min(ext) == 0:
             return 0
-        dt = {1: np.uint8, 2: np.uint16, 4: np.uint32, 8: np.uint64}[int(elem_bytes)]
+        if int(elem_bytes) not in _UNIT:
+            return 2
+        dt = _UNIT[int(elem_bytes)]
 
         def offsets(strides, index):
             total = np.zeros((), dtype=np.int64)
