@@ -5,7 +5,8 @@ loader shim).  The public names mirror DistributedArrays.jl's for this path: ``D
 ``localindices``, ``locate``, ``makelocal``, ``procs``, ``dzeros/dones/dfill/drand``, ``map`` (``map_``), ``map!``
 (``map_inplace``), broadcast (``broadcast`` / ``broadcast_into``), ``reduce``, ``mapreduce``, ``sum``, ``prod``,
 ``maximum``, ``minimum``, ``all``, ``any``, ``count``, ``extrema``, ``findmax`` / ``findmin`` / ``argmax`` / ``argmin`` (with and without
-``dims``), ``mapslices`` (with ``sort``, ``svdvals``, ``eigvals``, reductions,
+``dims``), ``sort`` and ``sortperm`` of a DVector (``sortperm(d; sample, by)``: stable, 1-based, the layout of ``sort``),
+``mapslices`` (with ``sort``, ``svdvals``, ``eigvals``, reductions,
 elementwise and constant slice functions), ``ppeval`` (batched slice products ``ppeval(operator.matmul, A, B)``, ``eigvals`` of symmetric
 slices, and every ``mapslices`` slice function), ``cumsum`` / ``cumprod`` / ``accumulate`` and their ``!`` forms
 (``cumsum_`` ...), ``Array(d)`` (``to_array``), range ``getindex``; sparse DArrays (``distribute`` of a scipy.sparse matrix: CSC
@@ -31,7 +32,7 @@ from ._mapreduce import (all, any, axpy_, count, dot, extrema, isequal, mapreduc
                          prod, reduce, rmul_, sum)
 from ._linalg import Adjoint, Transpose, adjoint, copy_transposed, lmul_diag, matmat, matmul, mul_, mul_mat_, rmul_diag, transpose
 from ._findmax import argmax, argmin, findmax, findmin
-from ._sort import sort, sort_with_boundaries
+from ._sort import sort, sort_with_boundaries, sortperm
 from ._scan import accumulate, accumulate_, cumprod, cumprod_, cumsum, cumsum_
 from ._slices import eigvals, mapslices, svdvals
 from ._ppeval import ppeval

@@ -118,6 +118,8 @@ _SIGS = {
     "dab_sorted_split": (_i32, [_vp, _i32, _vp, _sz, _vp, _i32, C.POINTER(C.c_ulonglong)]),
     "dab_sort_by_key": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _sz, _sz]),
     "dab_sort_by_key_scratch_bytes": (_i32, [_i32, _sz, C.POINTER(_sz)]),
+    "dab_sort_pairs": (_i32, [_vp, _i32, _vp, _vp, _vp, C.c_int64, _vp, _vp, _sz, _sz]),
+    "dab_sort_pairs_scratch_bytes": (_i32, [_i32, _sz, C.POINTER(_sz)]),
     "dab_sort_slices": (_i32, [_vp, _i32, _vp, _vp, _sz, _sz, _sz]),
     "dab_svdvals_batched": (_i32, [_vp, _i32, _vp, _sz, _sz, _sz, _vp, _vp]),
     "dab_matmul_batched": (_i32, [_vp, _i32, _sz, _sz, _sz, _vp, _sz, _vp, _sz, _vp, _sz]),

@@ -19,6 +19,10 @@ sort of the gathered samples, :77; the split compares ``by(x) > by(boundaries[i+
 closure, ``keys = f.(chunk)`` is ONE fused elementwise kernel, ``dab_sort_by_key`` orders the values stably by those keys (K11 on
 packed key|position words), the split runs on ``f.(sorted chunk)``, and the few hundred samples / boundaries get their keys from the
 same kernel so that host and device agree bit for bit on ``f``.
+
+``sortperm(d; sample, by)`` (no reference method) runs the same samplesort (``_samplesort``) with K21 ``dab_sort_pairs`` as both local
+sorts: every key carries its 1-based global index, the Int64 index plane travels with the keys by the same exchange plan, and the result
+holds the indices.  Stable (equal keys and all NaNs keep ascending index order), in ``sort``'s layout.
 """
 from __future__ import annotations
 
@@ -204,42 +208,112 @@ def sort(d: DArray, sample=True, by=None, alg=None, **kwargs) -> DArray:  # noqa
 
 def sort_with_boundaries(d: DArray, sample=True, by=None, alg=None, **kwargs):
     """``sort`` plus the ``boundaries`` vector it partitioned with (what compute_boundaries returns, src/sort.jl:66-88)."""
+    kf, pids = _check_args(d, sample, by, kwargs, "sort")
+    presample = _presample(d, sample, len(pids), d.dtype)
+    return _samplesort(d, d.chunks, d.dtype, presample, kf, perm=False)
+
+
+def sortperm(d: DArray, sample=True, by=None, alg=None, **kwargs) -> DArray:
+    """``sortperm(d::DVector; sample=true, by)``: the DVector of Int64 with ``d[p]`` sorted -- Julia's ``sortperm(Array(d))``, 1-based
+    global indices in ``isless`` order, STABLE (equal keys, and all NaNs, keep ascending index order).  The samplesort of ``sort``
+    with K21 (``dab_sort_pairs``) carrying every key's global index: chunk j of the result indexes the elements in chunk j of
+    ``sort(d; sample)``, the layout is the same.  (Only when the reference's scan would leave NaNs ahead of larger keys, so that
+    ``sort(d)`` itself is out of ``isless`` order, are the NaNs moved to the last receiving piece and the chunk sizes differ.)
+    ``by = f``: ``sortperm(f.(d))``, with ``sample`` in key space.  ``alg`` is accepted and ignored (one stable result)."""
+    from ._sparse import SparseDArray, refuse
+    if isinstance(d, SparseDArray):
+        refuse("sortperm")
+    if isinstance(d, DArray) and d.dtype.kind == "c" and by is None:
+        raise TypeError(f"MethodError: no method matching isless(::{d.dtype}, ::{d.dtype}) -- complex numbers are not ordered")
+    kf, pids = _check_args(d, sample, by, kwargs, "sortperm")
+    if d.size == 0:
+        raise _lib.ArgumentError(_lib.ERR_EMPTY, "sortperm: empty DVector")
+    kdt = d.dtype if kf is None else kf.kdt
+    if kf is None:
+        return _samplesort(d, d.chunks, kdt, _presample(d, sample, len(pids), kdt), None, perm=True)[0]
+    if sample is not False:
+        presample = _presample(None, sample, len(pids), kdt)   # a bad sample raises before the keys are computed
+    keys = DArray(d.layout, kdt, {pid: kf.keys_of(ch) for pid, ch in d.chunks.items()}, d.rt)
+    try:
+        if sample is False:
+            presample = _presample(keys, False, len(pids), kdt)
+        return _samplesort(keys, keys.chunks, kdt, presample, None, perm=True)[0]
+    finally:
+        keys.close()
+
+
+def _check_args(d: DArray, sample, by, kwargs, what: str):
+    """The argument checks of ``sort`` / ``sortperm``, all before any launch: (traced key function or None, pids)."""
     if kwargs:
         raise _lib.ArgumentError(_lib.ERR_ARG, "Only `alg`, `by` and `sample` are supported as keyword arguments")
     if d.ndim != 1:
-        raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, "sort is defined for a DVector")
+        raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, f"{what} is defined for a DVector")
     dt = d.dtype
     if dt not in _SORT_DTYPES:
-        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"sort: eltype {dt} (served: Float32 Float64 Int32 Int64)")
-    rt = d.rt
-    kf = _KeyFn(rt, by, dt) if by is not None else None         # traced before any launch: an untraceable `by` raises here
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what}: eltype {dt} (served: Float32 Float64 Int32 Int64)")
+    kf = _KeyFn(d.rt, by, dt) if by is not None else None      # traced before any launch: an untraceable `by` raises here
     pids = list(d.layout.pids)
-    nparts = len(pids)
-    if nparts > 256:
-        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "sort over more than 256 workers")
-    isz = dt.itemsize
+    if len(pids) > 256:
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what} over more than 256 workers")
     if sample is True and any(hi < lo for ((lo, hi),) in d.layout.indices):
         raise ZeroDivisionError("DivideError: integer division error")            # div(llp, 0) on an empty localpart, src/sort.jl:9
+    return kf, pids
 
-    # ---- boundaries that do not need the sorted chunks (src/sort.jl:118-155)
-    presample = None
+
+def _presample(d, sample, nparts: int, dt: np.dtype):
+    """The sample of the boundaries that do not need the sorted chunks (src/sort.jl:118-155), or None for ``sample = true``.
+    ``sample = false`` reads minimum(d) and maximum(d); the other forms launch nothing."""
     if sample is False:
         from ._mapreduce import maximum, minimum
         sample = (minimum(d), maximum(d))
     if isinstance(sample, tuple):
         if len(sample) != 2:
             raise _lib.ArgumentError(_lib.ERR_ARG, "keyword arg `sample` must be Boolean, Tuple(Min,Max) or an actual sample of data")
-        presample = uniform_sample(sample[0], sample[1], nparts, dt)
-    elif isinstance(sample, (np.ndarray, list)):
-        presample = np.asarray(sample)
-    elif sample is not True:
+        return uniform_sample(sample[0], sample[1], nparts, dt)
+    if isinstance(sample, (np.ndarray, list)):
+        return np.asarray(sample)
+    if sample is not True:
         raise _lib.ArgumentError(_lib.ERR_ARG, f"keyword arg `sample` must be Boolean, Tuple(Min,Max) or an actual sample of data : {sample}")
+    return None
 
-    # ---- sort(localpart(d)) on every worker
+
+def _sort_pairs(rt, keys_ptr: int, keys_out: B200Array, vals_ptr, base: int, vals_out: B200Array, n: int, dt: np.dtype):
+    """K21 on one chunk: keys_out / vals_out = keys / vals (``vals_ptr`` None: base + i) in the stable isless order of the keys."""
+    need = C.c_size_t()
+    _lib.check(_lib.lib().dab_sort_pairs_scratch_bytes(dab_dtype(dt), n, C.byref(need)))
+    scratch = B200Array.empty(rt, (need.value,), np.uint8, temp=True)
+    _lib.call("dab_sort_pairs", rt.ctx, dab_dtype(dt), C.c_void_p(keys_ptr), C.c_void_p(keys_out.ptr), C.c_void_p(vals_ptr), base,
+              C.c_void_p(vals_out.ptr), C.c_void_p(scratch.ptr), need.value, n)
+    scratch.free()
+
+
+def _nan_count(rt, s: B200Array) -> int:
+    """count(isnan, s) on the device (one reduce launch)."""
+    slot = B200Array.empty(rt, (16,), np.uint8, temp=True)
+    _lib.call("dab_reduce", rt.ctx, dab_dtype(s.dtype), _lib.COUNT, _lib.MAP_ISNAN, None, C.c_void_p(s.ptr), s.size, C.c_void_p(slot.ptr))
+    n = int(slot.to_numpy()[:8].view(np.int64)[0])
+    slot.free()
+    return n
+
+
+def _samplesort(d: DArray, src: Dict[int, B200Array], dt: np.dtype, presample, kf, perm: bool):
+    """The samplesort of ``d``'s layout over the chunks ``src`` (keys of dtype ``dt``).  ``perm``: every key carries its 1-based
+    global index (K21) and the result holds the indices instead of the keys."""
+    rt = d.rt
+    pids = list(d.layout.pids)
+    nparts = len(pids)
+    isz = dt.itemsize
+
+    # ---- sort(localpart(d)) on every worker (sortperm: with the chunk's global indices)
     srt: Dict[int, B200Array] = {}
-    for pid, ch in d.chunks.items():
+    idx: Dict[int, B200Array] = {}
+    for pid, ch in src.items():
         out = B200Array.empty(rt, (ch.size,), dt, temp=True)
-        if kf is None:
+        if perm:
+            idx[pid] = B200Array.empty(rt, (ch.size,), np.int64, temp=True)
+            ((lo, _),) = d.layout.indices[pids.index(pid)]
+            _sort_pairs(rt, ch.ptr, out, None, lo, idx[pid], ch.size, dt)
+        elif kf is None:
             _sort_chunk(rt, ch.ptr, ch.size, dt, out)
         else:
             kf.sort_chunk(ch, out)
@@ -296,34 +370,56 @@ def sort_with_boundaries(d: DArray, sample=True, by=None, alg=None, **kwargs):
             e.append(prev)
         ends[pid] = e
         sizes_mine[pid] = [e[0]] + [e[i] - e[i - 1] for i in range(1, nparts)]
+        if perm:                                                # sortperm: the chunk's NaN count rides along as one more column
+            sizes_mine[pid].append(_nan_count(rt, s) if dt.kind == "f" and s.size else 0)
     # the size matrix (source worker x destination) on every rank: one small all-gather through the exchange arena
     wpr = rt.workers_per_rank
-    mine_arr = np.zeros((wpr, nparts), dtype=np.int64)
+    ncol = nparts + 1 if perm else nparts
+    mine_arr = np.zeros((wpr, ncol), dtype=np.int64)
     for pid, row in sizes_mine.items():
         mine_arr[(pid - 1) % wpr] = row
     allrows = rt.allgather_small(mine_arr.reshape(-1))
     sizes: Dict[int, List[int]] = {}
     for pid in pids:
         r, w = rt.rank_of(pid), (pid - 1) % wpr
-        sizes[pid] = [int(v) for v in allrows[r].reshape(wpr, nparts)[w]]
+        sizes[pid] = [int(v) for v in allrows[r].reshape(wpr, ncol)[w]]
+    if perm:
+        # The reference scan leaves a chunk's NaNs (the tail of its sorted keys) in its last non-empty piece, which can lie ahead of
+        # larger keys of other chunks.  sortperm moves them to the last piece that receives anything, J: the result stays in isless
+        # order, and when sort's result is (every NaN chunk already ends in J) nothing moves and the layout is sort's.
+        nan = {p: sizes[p].pop() for p in pids}
+        J = max((max(j for j in range(nparts) if sizes[p][j]) for p in pids if any(sizes[p])), default=0)
+        for p in pids:
+            if nan[p]:
+                last = max(j for j in range(nparts) if sizes[p][j])
+                sizes[p][last] -= nan[p]
+                sizes[p][J] += nan[p]
+                if p in ends:
+                    ends[p] = [int(x) for x in np.cumsum(sizes[p])]
 
-    # ---- ship piece i to worker i
+    # ---- ship piece i to worker i (sortperm: the index plane travels with the keys, by the same plan)
     totals = [sum(sizes[p][j] for p in pids) for j in range(nparts)]
     # a worker that receives ONE non-empty piece already holds its sorted result: the piece lands straight in the result chunk and the
     # second sort (``sort!(lp_sorting)``, src/sort.jl:61) has nothing to do; several pieces are concatenated and sorted again
     recv: Dict[int, B200Array] = {}
+    recv_idx: Dict[int, B200Array] = {}
     single_run: Dict[int, bool] = {}
     for j, pid in enumerate(pids):
         if rt.is_local(pid) and totals[j]:
             single_run[j] = sum(1 for p in pids if sizes[p][j]) == 1
-            recv[j] = B200Array.empty(rt, (totals[j],), dt, temp=not single_run[j])
+            recv[j] = B200Array.empty(rt, (totals[j],), dt, temp=perm or not single_run[j])
+            if perm:
+                recv_idx[j] = B200Array.empty(rt, (totals[j],), np.int64, temp=not single_run[j])
     plan = sort_exchange_plan(pids, sizes, rt.rank_of, rt.rank)
-    for j, p, off, n in plan["local"]:
-        _lib.call("dab_d2d", rt.ctx, C.c_void_p(recv[j].ptr + off * isz), C.c_void_p(srt[p].ptr + (ends[p][j] - n) * isz), n * isz)
-    sends = [(srt[p].ptr + (ends[p][j] - n) * isz, n * isz, peer) for j, p, n, peer in plan["sends"]]
-    recvs = [(recv[j].ptr + off * isz, n * isz, peer) for j, p, off, n, peer in plan["recvs"]]
+    planes = [(srt, recv, isz)] + ([(idx, recv_idx, 8)] if perm else [])
+    sends, recvs = [], []
+    for sbufs, rbufs, es in planes:
+        for j, p, off, n in plan["local"]:
+            _lib.call("dab_d2d", rt.ctx, C.c_void_p(rbufs[j].ptr + off * es), C.c_void_p(sbufs[p].ptr + (ends[p][j] - n) * es), n * es)
+        sends += [(sbufs[p].ptr + (ends[p][j] - n) * es, n * es, peer) for j, p, n, peer in plan["sends"]]
+        recvs += [(rbufs[j].ptr + off * es, n * es, peer) for j, p, off, n, peer in plan["recvs"]]
     grouped_exchange(rt, sends, recvs)
-    for s in srt.values():
+    for s in list(srt.values()) + list(idx.values()):
         s.free()
 
     # ---- sort!(lp_sorting) on every receiver and DArray(local_sorted_refs) without the empty parts (src/sort.jl:52-61, 163-169)
@@ -332,6 +428,16 @@ def sort_with_boundaries(d: DArray, sample=True, by=None, alg=None, **kwargs):
         raise _lib.ArgumentError(_lib.ERR_EMPTY, "sort: empty DVector")
     chunks: Dict[int, B200Array] = {}
     for j, buf in recv.items():
+        if perm:
+            # pieces arrive in source-worker order, which is global index order: the stable pair sort keeps equal keys in index order
+            if single_run[j]:
+                chunks[pids[j]] = recv_idx[j]
+            else:
+                chunks[pids[j]] = B200Array.empty(rt, (totals[j],), np.int64)
+                _sort_pairs(rt, buf.ptr, buf, recv_idx[j].ptr, 0, chunks[pids[j]], totals[j], dt)
+                recv_idx[j].free()
+            buf.free()
+            continue
         if single_run[j]:
             chunks[pids[j]] = buf
             continue
@@ -343,4 +449,4 @@ def sort_with_boundaries(d: DArray, sample=True, by=None, alg=None, **kwargs):
         buf.free()
         chunks[pids[j]] = out
     layout = layout_from_chunk_shapes([(totals[j],) for j in keep], (len(keep),), [pids[j] for j in keep])
-    return DArray(layout, dt, chunks, rt), boundaries
+    return DArray(layout, np.int64 if perm else dt, chunks, rt), boundaries

@@ -12,6 +12,12 @@
 //                         stable), resolve the tile's bucket offsets by decoupled look-back over the earlier tiles, reorder the tile by digit
 //                         in shared memory and write it out in runs
 // Algorithmic bytes: elem * (1 + 2 * passes) per key.
+//
+// K21, the pair sort (dab_sort_pairs, the kernel under sortperm): the same kernels with the payload parameter P = uint32_t.  Every key
+// carries its 32-bit position in the chunk through the passes: the reorder step writes it to the same shared-memory slot as its key and
+// the write-out moves both.  The first pass reads no payload (it generates the tile position), the last one writes the Int64 value
+// (base + position, or vals[position]).  The radix key is sortby_radix_key: every NaN collapses to the top key, so NaNs are ties and
+// LSD stability keeps them, like every other run of equal keys, in input order.  P = void is the keys-only K11, unchanged.
 #include <map>
 #include <mutex>
 #include <type_traits>
@@ -19,8 +25,27 @@
 
 #include "dab_common.cuh"
 #include "dab_sort_key.cuh"
+#include "dab_sortby_core.cuh"
 
 namespace {
+
+// What the pair instances need beyond the keys; empty for the keys-only ones.
+template <typename P> struct PairIO {};
+template <> struct PairIO<uint32_t> {
+    uint32_t* pos_out;       // positions between passes, beside the keys in `out`
+    uint32_t* pos_tmp;       // ... beside the keys in `tmp`
+    const int64_t* vals;     // NULL: the value of position i is base + i
+    int64_t base;
+    int64_t* vals_out;
+    __device__ __forceinline__ int64_t value(uint32_t pos) const { return vals ? vals[pos] : base + (int64_t)pos; }
+};
+
+// Radix key of a raw key: the keys-only bijection, or (pairs) the same with every NaN collapsed to the top key.
+template <typename T, typename P>
+__device__ __forceinline__ typename SortKey<T>::U radix_of(typename SortKey<T>::U raw) {
+    if constexpr (std::is_void<P>::value) return SortKey<T>::enc(raw);
+    else return sortby_radix_key<T>(raw);
+}
 
 constexpr int ST_THREADS = 256;
 constexpr int ST_KPT = 8;                        // keys per thread (16 left the scatter at 111 registers = 2 CTAs per SM, latency-bound)
@@ -84,7 +109,7 @@ __device__ __forceinline__ int load_blocked(const U* __restrict__ in, size_t fir
 }
 
 // ---- all-digit histogram ------------------------------------------------------------------------------------------------------------
-template <typename T>
+template <typename T, typename P>
 __global__ void __launch_bounds__(ST_THREADS) sort_hist_kernel(const typename SortKey<T>::U* __restrict__ in, size_t n,
                                                                unsigned long long* __restrict__ ghist) {
     using K = SortKey<T>;
@@ -98,7 +123,7 @@ __global__ void __launch_bounds__(ST_THREADS) sort_hist_kernel(const typename So
         const int cnt = load_blocked<U>(in, base + (size_t)threadIdx.x * ST_KPT, n, key);
         if (cnt > 0) {
             unsigned int cur[K::DIGITS], run[K::DIGITS];
-            const U k0 = K::enc(key[0]);
+            const U k0 = radix_of<T, P>(key[0]);
 #pragma unroll
             for (int d = 0; d < K::DIGITS; ++d) {
                 cur[d] = (unsigned)(k0 >> (8 * d)) & 255u;
@@ -107,7 +132,7 @@ __global__ void __launch_bounds__(ST_THREADS) sort_hist_kernel(const typename So
 #pragma unroll
             for (int k = 1; k < ST_KPT; ++k)
                 if (k < cnt) {
-                    const U kk = K::enc(key[k]);
+                    const U kk = radix_of<T, P>(key[k]);
 #pragma unroll
                     for (int d = 0; d < K::DIGITS; ++d) {
                         const unsigned int dg = (unsigned)(kk >> (8 * d)) & 255u;
@@ -195,12 +220,20 @@ __global__ void __launch_bounds__(256) sort_plan_kernel(SortPlan* plan, unsigned
     }
 }
 
-// mode 0: copy in -> tmp when the plan asks for the staging copy; mode 1: copy in -> out when NO pass runs (all keys equal)
-template <typename U>
+// mode 0: copy in -> tmp when the plan asks for the staging copy; mode 1: copy in -> out when NO pass runs (all keys equal; pairs: the
+// permutation is the identity, so vals_out gets the values in input order, and an in-place sort copies no key)
+template <typename U, typename P>
 __global__ void __launch_bounds__(256) sort_copy_if_kernel(const SortPlan* __restrict__ plan, const U* __restrict__ src, U* __restrict__ dst,
-                                                           size_t n, int mode) {
+                                                           size_t n, int mode, PairIO<P> io) {
     if (mode == 0 ? !plan->precopy : plan->n_active != 0) return;
-    for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (size_t)gridDim.x * 256) dst[i] = src[i];
+    for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (size_t)gridDim.x * 256) {
+        if constexpr (std::is_void<P>::value) {
+            dst[i] = src[i];
+        } else {
+            if (src != dst) dst[i] = src[i];
+            if (mode == 1) io.vals_out[i] = io.value((uint32_t)i);
+        }
+    }
 }
 
 // ---- one digit pass, "onesweep": count + look-back + stable scatter in ONE sweep over the keys ------------------------------------------
@@ -251,9 +284,11 @@ __device__ __forceinline__ void onesweep_rank(const typename SortKey<T>::U* __re
 }
 
 // The tile, sorted by the digit, into the second shared-memory buffer: local slot = start of the digit's run for this warp + rank.
-template <typename T, int KPT, bool FULL>
+// Pairs: the key's position goes to the same slot of the position buffer -- pstage[li], or tbase + li when the pass generates it.
+template <typename T, typename P, int KPT, bool FULL>
 __device__ __forceinline__ void onesweep_reorder(const typename SortKey<T>::U* __restrict__ stage, uint32_t sorted_s, unsigned int wofs, int lane,
-                                                 unsigned int nvalid, int shift, uint32_t wc_row, const unsigned short (&rank)[KPT]) {
+                                                 unsigned int nvalid, int shift, uint32_t wc_row, const unsigned short (&rank)[KPT],
+                                                 const uint32_t* __restrict__ pstage, uint32_t psorted_s, bool gen_pos, unsigned int tbase) {
     using U = typename SortKey<T>::U;
 #pragma unroll
     for (int k = 0; k < KPT; ++k) {
@@ -266,6 +301,10 @@ __device__ __forceinline__ void onesweep_reorder(const typename SortKey<T>::U* _
             const uint32_t a = sorted_s + (base + rank[k]) * (unsigned)sizeof(U);
             if constexpr (sizeof(U) == 8) asm volatile("st.shared.b64 [%0], %1;" ::"r"(a), "l"(key) : "memory");
             else asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(key) : "memory");
+            if constexpr (!std::is_void<P>::value) {
+                const uint32_t pos = gen_pos ? tbase + li : pstage[li];
+                asm volatile("st.shared.b32 [%0], %1;" ::"r"(psorted_s + (base + rank[k]) * 4u), "r"(pos) : "memory");
+            }
         }
     }
 }
@@ -279,13 +318,15 @@ __device__ __forceinline__ void onesweep_reorder(const typename SortKey<T>::U* _
 //   publish thread d sends the tile's count of digit d (PARTIAL) at once; decoupled look-back resolves the exclusive prefix later
 //   reorder the tile is written, sorted by digit, into a second shared-memory buffer
 //   write   consecutive threads -> consecutive addresses inside each bucket run
-template <typename T, int THREADS, int KPT, int MINB>
+// Pairs (P = uint32_t): the positions travel in two more shared buffers beside the keys, by a second bulk copy on the same mbarrier.
+template <typename T, typename P, int THREADS, int KPT, int MINB>
 __global__ void __launch_bounds__(THREADS, MINB) sort_onesweep_kernel(const typename SortKey<T>::U* __restrict__ in, typename SortKey<T>::U* __restrict__ out,
                                                                       typename SortKey<T>::U* __restrict__ tmp, size_t n, int d, SortPlan* __restrict__ plan,
                                                                       unsigned long long* __restrict__ lookback, unsigned int ntiles,
-                                                                      unsigned long long epoch) {
+                                                                      unsigned long long epoch, PairIO<P> io) {
     using K = SortKey<T>;
     using U = typename K::U;
+    constexpr bool PAIRS = !std::is_void<P>::value;
     constexpr int WARPS = THREADS / 32;
     constexpr int TILE = THREADS * KPT;
     static_assert(THREADS >= 256 && THREADS % 32 == 0, "thread d serves digit d");
@@ -293,7 +334,9 @@ __global__ void __launch_bounds__(THREADS, MINB) sort_onesweep_kernel(const type
     extern __shared__ __align__(128) unsigned char os_smem[];
     U* stage = reinterpret_cast<U*>(os_smem);                                   // [TILE] the tile as it sits in memory
     U* sorted = stage + TILE;                                                   // [TILE] the tile sorted by the digit
-    unsigned int (*wc)[256] = reinterpret_cast<unsigned int (*)[256]>(sorted + TILE);   // [WARPS][256]
+    uint32_t* pstage = reinterpret_cast<uint32_t*>(sorted + TILE);              // pairs: [TILE] positions of `stage`
+    uint32_t* psorted = pstage + TILE;                                          // pairs: [TILE] positions of `sorted`
+    unsigned int (*wc)[256] = reinterpret_cast<unsigned int (*)[256]>(PAIRS ? psorted + TILE : pstage);   // [WARPS][256]
     unsigned int* dbase = &wc[WARPS][0];                                        // [256]
     unsigned int* wtot = dbase + 256;                                           // [8]
     __shared__ unsigned int s_next;
@@ -302,6 +345,14 @@ __global__ void __launch_bounds__(THREADS, MINB) sort_onesweep_kernel(const type
     const U* __restrict__ src = ssel == SEL_IN ? in : (ssel == SEL_OUT ? out : tmp);
     U* __restrict__ dst = dsel == SEL_OUT ? out : tmp;
     const bool raw_in = plan->raw_in[d] != 0, raw_out = plan->raw_out[d] != 0;   // buffers between passes hold ENCODED keys
+    // pairs: positions come from the buffer beside the source keys (none on the first pass: it generates them) and go beside the
+    // destination keys (the last pass writes the Int64 values instead)
+    const uint32_t* __restrict__ psrc = nullptr;
+    uint32_t* __restrict__ pdst = nullptr;
+    if constexpr (PAIRS) {
+        psrc = raw_in ? nullptr : (ssel == SEL_OUT ? io.pos_out : io.pos_tmp);
+        pdst = dsel == SEL_OUT ? io.pos_out : io.pos_tmp;
+    }
     const unsigned int* gbase = plan->base[d];
     const int shift = 8 * d;
     const unsigned long long ep = (epoch << 32) & LB_EPOCH_MASK;
@@ -310,17 +361,29 @@ __global__ void __launch_bounds__(THREADS, MINB) sort_onesweep_kernel(const type
     const bool src_aligned = (reinterpret_cast<uintptr_t>(src) & 15u) == 0;
     const uint32_t bar = sort_smem_u32(&s_bar), stage_s = sort_smem_u32(stage), sorted_s = sort_smem_u32(sorted);
     const uint32_t wc_row = sort_smem_u32(&wc[warp][0]);
-    // a tile can come by bulk copy when its bytes are a multiple of 16 from a 16-byte aligned address
+    const uint32_t pstage_s = sort_smem_u32(pstage), psorted_s = sort_smem_u32(psorted);
+    // a tile can come by bulk copy when its bytes are a multiple of 16 from a 16-byte aligned address (pairs: its positions too)
     auto bulk_ok = [&](unsigned int t) -> bool {
         if (!src_aligned) return false;
         const size_t tb = (size_t)t * TILE;
         const size_t cnt = (tb + TILE <= n) ? (size_t)TILE : n - tb;
+        if constexpr (PAIRS)
+            if (psrc && (cnt % 4 != 0 || (reinterpret_cast<uintptr_t>(psrc) & 15u) != 0)) return false;
         return (cnt * sizeof(U)) % 16 == 0;
     };
     auto issue_bulk = [&](unsigned int t) {   // one thread
         const size_t tb = (size_t)t * TILE;
         const uint32_t bytes = (uint32_t)(((tb + TILE <= n) ? (size_t)TILE : n - tb) * sizeof(U));
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+        if constexpr (PAIRS) {
+            const uint32_t pbytes = psrc ? bytes / (uint32_t)sizeof(U) * 4u : 0u;
+            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes + pbytes) : "memory");
+            if (pbytes)
+                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                             ::"r"(pstage_s), "l"(psrc + tb), "r"(pbytes), "r"(bar)
+                             : "memory");
+        } else {
+            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+        }
         asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                      ::"r"(stage_s), "l"(src + tb), "r"(bytes), "r"(bar)
                      : "memory");
@@ -352,6 +415,9 @@ __global__ void __launch_bounds__(THREADS, MINB) sort_onesweep_kernel(const type
             phase ^= 1u;
         } else {                                                // misaligned source or ragged byte count: plain loads by everybody
             for (unsigned int i = threadIdx.x; i < nvalid; i += THREADS) stage[i] = __ldcs(src + tbase + i);
+            if constexpr (PAIRS)
+                if (psrc)
+                    for (unsigned int i = threadIdx.x; i < nvalid; i += THREADS) pstage[i] = __ldcs(psrc + tbase + i);
             __syncthreads();
         }
         const unsigned int wofs = (unsigned)warp * (KPT * 32);
@@ -359,7 +425,7 @@ __global__ void __launch_bounds__(THREADS, MINB) sort_onesweep_kernel(const type
 #pragma unroll
             for (int k = 0; k < KPT; ++k) {
                 const unsigned int li = wofs + (unsigned)k * 32 + lane;
-                if (full || li < nvalid) stage[li] = K::enc(stage[li]);
+                if (full || li < nvalid) stage[li] = radix_of<T, P>(stage[li]);
             }
         }
         unsigned short rank[KPT];
@@ -397,8 +463,8 @@ __global__ void __launch_bounds__(THREADS, MINB) sort_onesweep_kernel(const type
             for (int w = 0; w < WARPS; ++w) wc[w][dd] += tstart;
         }
         __syncthreads();
-        if (full) onesweep_reorder<T, KPT, true>(stage, sorted_s, wofs, lane, nvalid, shift, wc_row, rank);
-        else onesweep_reorder<T, KPT, false>(stage, sorted_s, wofs, lane, nvalid, shift, wc_row, rank);
+        if (full) onesweep_reorder<T, P, KPT, true>(stage, sorted_s, wofs, lane, nvalid, shift, wc_row, rank, pstage, psorted_s, raw_in, (unsigned)tbase);
+        else onesweep_reorder<T, P, KPT, false>(stage, sorted_s, wofs, lane, nvalid, shift, wc_row, rank, pstage, psorted_s, raw_in, (unsigned)tbase);
         __syncthreads();                                        // `stage` is free again, `sorted` is complete
         if (threadIdx.x == 0) {                                 // next tile: ticket + bulk copy, in flight during look-back and write-out
             const unsigned int t1 = atomicAdd(&plan->tile_ticket[d], 1u);
@@ -430,7 +496,26 @@ __global__ void __launch_bounds__(THREADS, MINB) sort_onesweep_kernel(const type
             dbase[dd] = gbase[dd] + excl - tstart;
         }
         __syncthreads();
-        if (full && !raw_out) {
+        if constexpr (PAIRS) {   // key and position leave together; the last pass turns the position into its Int64 value
+            auto put = [&](unsigned int i) {
+                const U kk = sorted[i];
+                const unsigned int o = dbase[(unsigned)(kk >> shift) & 255u] + i;
+                const uint32_t pos = psorted[i];
+                if (raw_out) {
+                    dst[o] = K::dec(kk);
+                    io.vals_out[o] = io.value(pos);
+                } else {
+                    dst[o] = kk;
+                    pdst[o] = pos;
+                }
+            };
+            if (full) {
+#pragma unroll
+                for (int k = 0; k < KPT; ++k) put((unsigned)k * THREADS + threadIdx.x);
+            } else {
+                for (unsigned int i = threadIdx.x; i < nvalid; i += THREADS) put(i);
+            }
+        } else if (full && !raw_out) {
 #pragma unroll
             for (int k = 0; k < KPT; ++k) {
                 const unsigned int i = (unsigned)k * THREADS + threadIdx.x;
@@ -455,13 +540,14 @@ __global__ void __launch_bounds__(THREADS, MINB) sort_onesweep_kernel(const type
 }
 
 // encode / decode a whole buffer (only when no digit pass runs at all, or as the odd-parity fix-up never needed: kept for n small)
-template <typename T>
-__global__ void sort_small_kernel(const typename SortKey<T>::U* __restrict__ in, typename SortKey<T>::U* __restrict__ out, unsigned int n) {
+template <typename T, typename P>
+__global__ void sort_small_kernel(const typename SortKey<T>::U* __restrict__ in, typename SortKey<T>::U* __restrict__ out, unsigned int n,
+                                  PairIO<P> io) {
     // n <= 1024: rank sort in shared memory by one CTA (stable: ties broken by index)
     using K = SortKey<T>;
     using U = typename K::U;
     __shared__ U sk[1024];
-    for (unsigned int i = threadIdx.x; i < n; i += blockDim.x) sk[i] = K::enc(in[i]);
+    for (unsigned int i = threadIdx.x; i < n; i += blockDim.x) sk[i] = radix_of<T, P>(in[i]);
     __syncthreads();
     for (unsigned int i = threadIdx.x; i < n; i += blockDim.x) {
         const U me = sk[i];
@@ -471,6 +557,7 @@ __global__ void sort_small_kernel(const typename SortKey<T>::U* __restrict__ in,
             r += (o < me) || (o == me && j < i);
         }
         out[r] = K::dec(me);
+        if constexpr (!std::is_void<P>::value) io.vals_out[r] = io.value(i);
     }
 }
 
@@ -483,10 +570,12 @@ int32_t sort_scratch(dab_ctx* ctx, size_t dev_bytes) {
 constexpr size_t SORT_PLAN_BYTES = 65536;   // SortPlan + the staging areas of dab_sorted_split, ahead of the look-back words
 static_assert(sizeof(SortPlan) + 8192 <= SORT_PLAN_BYTES, "plan area");
 
-template <typename T, int THREADS, int KPT, int MINB>
-int32_t sort_passes(dab_ctx* ctx, const typename SortKey<T>::U* in, typename SortKey<T>::U* out, typename SortKey<T>::U* tmp, size_t n) {
+template <typename T, typename P, int THREADS, int KPT, int MINB>
+int32_t sort_passes(dab_ctx* ctx, const typename SortKey<T>::U* in, typename SortKey<T>::U* out, typename SortKey<T>::U* tmp, size_t n,
+                    PairIO<P> io) {
     using K = SortKey<T>;
     using U = typename K::U;
+    constexpr bool PAIRS = !std::is_void<P>::value;
     constexpr int TILE = THREADS * KPT;
     const unsigned int ntiles = (unsigned int)((n + TILE - 1) / TILE);
     {
@@ -499,7 +588,7 @@ int32_t sort_passes(dab_ctx* ctx, const typename SortKey<T>::U* in, typename Sor
     {
         const unsigned int htiles = (unsigned int)((n + ST_TILE - 1) / ST_TILE);
         const unsigned int hgrid = htiles < (unsigned)ctx->sm_count * 4u ? htiles : (unsigned)ctx->sm_count * 4u;
-        sort_hist_kernel<T><<<hgrid, ST_THREADS, 0, ctx->stream>>>(in, n, &plan->hist[0][0]);
+        sort_hist_kernel<T, P><<<hgrid, ST_THREADS, 0, ctx->stream>>>(in, n, &plan->hist[0][0]);
         DAB_LAUNCHED(ctx);
     }
     const int inplace = (const void*)in == (const void*)out;
@@ -507,14 +596,15 @@ int32_t sort_passes(dab_ctx* ctx, const typename SortKey<T>::U* in, typename Sor
     DAB_LAUNCHED(ctx);
     const int cgrid = dab_grid_for(ctx, (n + 1023) / 1024, 8);
     if (inplace) {
-        sort_copy_if_kernel<U><<<cgrid, 256, 0, ctx->stream>>>(plan, in, tmp, n, 0);
-        DAB_LAUNCHED(ctx);
-    } else {
-        sort_copy_if_kernel<U><<<cgrid, 256, 0, ctx->stream>>>(plan, in, out, n, 1);   // acts only when every key is equal
+        sort_copy_if_kernel<U, P><<<cgrid, 256, 0, ctx->stream>>>(plan, in, tmp, n, 0, io);
         DAB_LAUNCHED(ctx);
     }
-    auto kern = sort_onesweep_kernel<T, THREADS, KPT, MINB>;
-    constexpr size_t smem = 2 * (size_t)TILE * sizeof(U) + (size_t)(THREADS / 32) * 1024 + 1024 + 32;
+    if (!inplace || PAIRS) {   // acts only when every key is equal (pairs: vals_out is written even when the keys stay in place)
+        sort_copy_if_kernel<U, P><<<cgrid, 256, 0, ctx->stream>>>(plan, in, out, n, 1, io);
+        DAB_LAUNCHED(ctx);
+    }
+    auto kern = sort_onesweep_kernel<T, P, THREADS, KPT, MINB>;
+    constexpr size_t smem = 2 * (size_t)TILE * (sizeof(U) + (PAIRS ? 4 : 0)) + (size_t)(THREADS / 32) * 1024 + 1024 + 32;
     int per_sm = 0;
     {   // >48 KiB of dynamic shared memory is an opt-in attribute of the (kernel, device) pair; the occupancy query needs it set
         static std::mutex mu;
@@ -538,14 +628,14 @@ int32_t sort_passes(dab_ctx* ctx, const typename SortKey<T>::U* in, typename Sor
             --d;
             continue;
         }
-        kern<<<grid, THREADS, smem, ctx->stream>>>(in, out, tmp, n, d, plan, lookback, ntiles, epoch);
+        kern<<<grid, THREADS, smem, ctx->stream>>>(in, out, tmp, n, d, plan, lookback, ntiles, epoch, io);
         DAB_LAUNCHED(ctx);
     }
     return DAB_OK;
 }
 
-template <typename T>
-int32_t sort_t(dab_ctx* ctx, const void* in_v, void* out_v, void* tmp_v, size_t n) {
+template <typename T, typename P = void>
+int32_t sort_t(dab_ctx* ctx, const void* in_v, void* out_v, void* tmp_v, size_t n, PairIO<P> io = {}) {
     using K = SortKey<T>;
     using U = typename K::U;
     const U* in = (const U*)in_v;
@@ -559,7 +649,7 @@ int32_t sort_t(dab_ctx* ctx, const void* in_v, void* out_v, void* tmp_v, size_t 
             DAB_CUDA(ctx, cudaMemcpyAsync(tmp, in, n * sizeof(U), cudaMemcpyDeviceToDevice, ctx->stream));
             src = tmp;
         }
-        sort_small_kernel<T><<<1, 256, 0, ctx->stream>>>(src, out, (unsigned)n);
+        sort_small_kernel<T, P><<<1, 256, 0, ctx->stream>>>(src, out, (unsigned)n, io);
         DAB_LAUNCHED(ctx);
         return DAB_OK;
     }
@@ -568,8 +658,16 @@ int32_t sort_t(dab_ctx* ctx, const void* in_v, void* out_v, void* tmp_v, size_t 
     // tile shape: 32 KiB of keys per CTA in shared memory -> ~128-byte bucket runs per tile on random digits
     // tile shape (tools/sort_vs_cub.cu sweeps it: larger tiles and 3 resident CTAs per SM won over smaller tiles at 4 CTAs
     // and over 128-register CTAs at 2): 256 threads x 16 keys (64-bit) / x 32 keys (32-bit) = 32 KiB of keys per tile, twice in shared memory
-    if constexpr (sizeof(U) == 8) return sort_passes<T, 256, 16, 3>(ctx, in, out, tmp, n);
-    else return sort_passes<T, 256, 32, 3>(ctx, in, out, tmp, n);
+    // Pairs hold a 4-byte position beside every key, twice: the tiles shrink so that 3 CTAs per SM still fit (4096 pairs of 32-bit
+    // keys = 64 KiB, 2560 pairs of 64-bit keys = 60 KiB, plus 9 KiB of counters each; 72 registers, no spills, -Xptxas -v)
+    if constexpr (!std::is_void<P>::value) {
+        if constexpr (sizeof(U) == 8) return sort_passes<T, P, 256, 10, 3>(ctx, in, out, tmp, n, io);
+        else return sort_passes<T, P, 256, 16, 3>(ctx, in, out, tmp, n, io);
+    } else if constexpr (sizeof(U) == 8) {
+        return sort_passes<T, P, 256, 16, 3>(ctx, in, out, tmp, n, io);
+    } else {
+        return sort_passes<T, P, 256, 32, 3>(ctx, in, out, tmp, n, io);
+    }
 }
 
 // ---- split points in a sorted chunk ----------------------------------------------------------------------------------------------------
@@ -636,9 +734,53 @@ int32_t bounds_t(dab_ctx* ctx, const void* sorted, size_t n, const void* bounds_
     return DAB_OK;
 }
 
+// dab_sort_pairs scratch: the keys' ping-pong buffer, then the two position buffers, each 256-byte aligned
+inline size_t pairs_stride(size_t bytes) { return (bytes + 255) & ~(size_t)255; }
+
+inline int pairs_key_bytes(int32_t key_dtype) {
+    return (key_dtype == DAB_F64 || key_dtype == DAB_I64) ? 8 : (key_dtype == DAB_F32 || key_dtype == DAB_I32) ? 4 : 0;
+}
+
+template <typename T>
+int32_t pairs_t(dab_ctx* ctx, const void* keys, void* keys_out, const int64_t* vals, int64_t base, int64_t* vals_out, void* scratch, size_t n) {
+    using U = typename SortKey<T>::U;
+    char* s = (char*)scratch;
+    const size_t ks = pairs_stride(n * sizeof(U)), ps = pairs_stride(n * 4);
+    PairIO<uint32_t> io{(uint32_t*)(s + ks), (uint32_t*)(s + ks + ps), vals, base, vals_out};
+    return sort_t<T, uint32_t>(ctx, keys, keys_out, s, n, io);
+}
+
 }  // namespace
 
 extern "C" {
+
+int32_t dab_sort_pairs_scratch_bytes(int32_t key_dtype, size_t n, size_t* bytes) {
+    if (bytes == nullptr) return dab_fail(nullptr, DAB_ERR_ARG, "dab_sort_pairs_scratch_bytes: null pointer");
+    const int kb = pairs_key_bytes(key_dtype);
+    if (kb == 0) return dab_fail(nullptr, DAB_ERR_UNSUPPORTED, "dab_sort_pairs: key dtype %d", key_dtype);
+    *bytes = pairs_stride(n * kb) + 2 * pairs_stride(n * 4);
+    return DAB_OK;
+}
+
+int32_t dab_sort_pairs(dab_ctx* ctx, int32_t key_dtype, const void* keys, void* keys_out, const int64_t* vals, int64_t base, int64_t* vals_out,
+                       void* scratch, size_t scratch_bytes, size_t n) {
+    DAB_ENTER(ctx);
+    if (n == 0) return DAB_OK;
+    DAB_REQUIRE(ctx, keys && keys_out && vals_out && scratch, DAB_ERR_ARG, "dab_sort_pairs: null pointer");
+    DAB_REQUIRE(ctx, (const void*)vals != (const void*)vals_out, DAB_ERR_ARG, "dab_sort_pairs: vals_out must not alias vals");
+    DAB_REQUIRE(ctx, n < 0xFFFFF000ull, DAB_ERR_UNSUPPORTED, "dab_sort_pairs: chunks of 2^32 - 4096 or more elements are not served");
+    size_t need = 0;
+    int32_t st = dab_sort_pairs_scratch_bytes(key_dtype, n, &need);
+    if (st != DAB_OK) return dab_fail(ctx, st, "dab_sort_pairs: key dtype %d", key_dtype);
+    DAB_REQUIRE(ctx, scratch_bytes >= need, DAB_ERR_ARG, "dab_sort_pairs: scratch of %zu bytes, %zu needed", scratch_bytes, need);
+    DAB_REQUIRE(ctx, ((uintptr_t)scratch & 15) == 0, DAB_ERR_ARG, "dab_sort_pairs: scratch must be 16-byte aligned");
+    switch (key_dtype) {
+        case DAB_F32: return pairs_t<float>(ctx, keys, keys_out, vals, base, vals_out, scratch, n);
+        case DAB_F64: return pairs_t<double>(ctx, keys, keys_out, vals, base, vals_out, scratch, n);
+        case DAB_I32: return pairs_t<int32_t>(ctx, keys, keys_out, vals, base, vals_out, scratch, n);
+        default: return pairs_t<int64_t>(ctx, keys, keys_out, vals, base, vals_out, scratch, n);
+    }
+}
 
 int32_t dab_sort(dab_ctx* ctx, int32_t dtype, const void* in, void* out, void* tmp, size_t n) {
     DAB_ENTER(ctx);

@@ -396,6 +396,20 @@ int32_t dab_sort_by_key(dab_ctx* ctx, int32_t key_dtype, const void* keys, int32
                         void* scratch, size_t scratch_bytes, size_t n);
 int32_t dab_sort_by_key_scratch_bytes(int32_t key_dtype, size_t n, size_t* bytes);
 
+/* ==== pair sort K21 (row f11) ================================================================
+ * keys_out / vals_out = keys / vals in the stable isless order of keys (all NaNs equal); vals == NULL means vals[i] = base + i.
+ * The per-chunk step of sortperm: with vals == NULL and base = the chunk's first global index, vals_out is the chunk's permutation.
+ * Key order is Julia's isless (-0.0 < 0.0, NaNs last); every NaN key is equal to every other, so elements with equal keys -- NaNs
+ * included -- keep their input order.  K11's onesweep passes with a 4-byte position carried beside every key; the last pass writes
+ * the Int64 value (base + position, or vals[position]).  The sorted keys are bit-identical to dab_sort's except that every NaN comes
+ * out as one canonical NaN.  key dtypes F32 F64 I32 I64; n < 2^32 - 4096 (otherwise DAB_ERR_UNSUPPORTED).  Aliasing: keys_out may
+ * equal keys (in-place); vals_out must not overlap vals, keys or keys_out; no other overlap is allowed.  scratch: device memory of
+ * at least dab_sort_pairs_scratch_bytes() bytes, 16-byte aligned.  Asynchronous on the ctx stream (the pass plan is made on the
+ * device, as in dab_sort). */
+int32_t dab_sort_pairs_scratch_bytes(int32_t key_dtype, size_t n, size_t* bytes);
+int32_t dab_sort_pairs(dab_ctx* ctx, int32_t key_dtype, const void* keys, void* keys_out, const int64_t* vals, int64_t base,
+                       int64_t* vals_out, void* scratch, size_t scratch_bytes, size_t n);
+
 /* Split points of a sorted chunk for the boundaries of the samplesort (src/sort.jl:28-40): for each of the
  * nb (<= 256) host values bounds[i] (dtype elements), counts_host[i] = the number of leading elements the
  * reference's scan would pass before the first x > bounds[i] had it started at element 1 -- the count of

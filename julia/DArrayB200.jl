@@ -22,6 +22,7 @@
 #   src/linalg.jl:1-17   adjoint!(lp, rp), complex T      LinearAlgebra.adjoint!                     dab_adjoint_box
 #   src/sort.jl:8,22,61  sort(localpart(d)), sort!(lp)    Base.sort / Base.sort!                     dab_sort
 #   src/sort.jl:8,22,61  sort(localpart(d); by = f)       sort_by (keys = f.(a) by broadcast)        dab_sort_by_key
+#   (Base.sortperm: scalar getindex)  sortperm(localpart(d)), sortperm(d)   Base.sortperm (chunk and DVector methods)   dab_sort_pairs
 #   src/mapreduce.jl:205 mapslices(f, localpart(y), dims) mapslices_sort / svdvals_batched       dab_sort_slices / dab_svdvals_batched
 #   src/mapreduce.jl:315 _ppeval(f, localparts...; dim)   matmul_batched / eigvals_sym_batched  dab_matmul_batched / dab_eigvals_sym_batched
 #   (no reference method)  accumulate!(op, lp, lp; dims)   Base.accumulate! (cumsum! / cumprod!)   dab_scan
@@ -393,6 +394,34 @@ function sort_by(a::B200Array{T,1}, keys::B200Array{K,1}) where {T,K}
 end
 # keyword arguments do not take part in dispatch: ONE method serves both spellings
 Base.sort(a::B200Array{T,1}; by = identity, kw...) where {T} = by === identity ? sort_keys(a) : sort_by(a, by.(a))
+
+# K21: keys and Int64 values in the stable isless order of the keys (every NaN equal); vals === nothing means vals[i] = base + i.
+# Returns (sorted keys, values).  keys and vals are not written.
+function sort_pairs(keys::B200Array{K,1}, vals::Union{Nothing,B200Array{Int64,1}}, base::Int64) where {K}
+    n = length(keys); need = Ref{Csize_t}(0)
+    check(ccall((:dab_sort_pairs_scratch_bytes, libdab), Int32, (Int32, Csize_t, Ref{Csize_t}), dab_dtype(K), n, need), ctx())
+    kout = B200Array{K,1}(undef, size(keys)); vout = B200Array{Int64,1}(undef, size(keys))
+    scratch = B200Array{UInt8,1}(undef, (Int(need[]),))
+    check(ccall((:dab_sort_pairs, libdab), Int32,
+                (Ptr{Cvoid}, Int32, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Int64, Ptr{Cvoid}, Ptr{Cvoid}, Csize_t, Csize_t),
+                ctx(), dab_dtype(K), keys.ptr, kout.ptr, vals === nothing ? C_NULL : vals.ptr, base, vout.ptr, scratch.ptr, need[], n), ctx())
+    kout, vout
+end
+# sortperm(localpart(d)): 1-based, stable; by = f orders by the keys f.(a) (one fused broadcast kernel)
+Base.sortperm(a::B200Array{T,1}; by = identity, kw...) where {T} = sort_pairs(by === identity ? a : by.(a), nothing, Int64(1))[2]
+
+# sortperm(d::DVector): K21 on every chunk with base = the chunk's first global index, then the sorted runs are merged on the caller
+# in worker order (a stable merge: equal keys keep ascending global index) and the permutation is distributed over procs(d).  The
+# Python runtime instead runs sort's samplesort with the index plane (the layout of sort(d)); this method keeps the binding small.
+function Base.sortperm(d::DArray{T,1,B200Array{T,1}}; by = identity, kw...) where {T}
+    runs = [remotecall_fetch(p) do
+                a = localpart(d)
+                k, v = sort_pairs(by === identity ? a : by.(a), nothing, Int64(first(localindices(d)[1])))
+                Array(k), Array(v)
+            end for p in procs(d)]
+    keys = reduce(vcat, first.(runs)); idx = reduce(vcat, last.(runs))
+    distribute(idx[sortperm(keys; alg = Base.Sort.DEFAULT_STABLE)]; procs = procs(d))
+end
 
 # mapslices(f, localpart(y), dims=z)  (src/mapreduce.jl:205) for f = sort (one dim) and f = svdvals (two dims, slices already packed as
 # `batch` column-major m x n matrices: the Python runtime packs them with dab_gather_box).  Julia's LAPACK wrapper rejects non-finite

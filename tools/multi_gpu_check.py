@@ -5,7 +5,7 @@
 
 Checks, against the CPU oracle regenerated on every rank: sum / maximum with the NCCL all-gather + ordered left fold,
 mapreducedim with the grouped send/recv between-phase, findmax / findmin with dims and cumsum / accumulate along a dim cut
-across ranks, one-sided halo reads over CUDA IPC peer mappings, broadcast across mismatched layouts; then times the C5 halo
+across ranks, sort and sortperm of a DVector, one-sided halo reads over CUDA IPC peer mappings, broadcast across mismatched layouts; then times the C5 halo
 read (256 MiB slab from the next rank) and prints one JSON line per metric (rank 0).
 """
 import ctypes as C
@@ -200,6 +200,21 @@ def main():
             d2.close()
     rt.barrier()
     log("ok: sort(d::DVector) across ranks")
+
+    # ---- sortperm across ranks: keys and the Int64 index plane travel by the same grouped send/recv; exact against the model
+    for T in (np.int64, np.float64):
+        rs = np.random.default_rng(78)
+        av = rs.integers(-50, 50, 300007).astype(T)                    # heavy ties: stability across ranks is the whole answer
+        dv = dab.distribute(av)
+        for sample in (True, False, av[:400]):
+            p = dab.sortperm(dv, sample=sample)
+            s = dab.sort(dv, sample=sample)
+            assert np.array_equal(dab.to_array(p), orc.jl_sortperm_stable(av) + 1)
+            assert list(p.layout.pids) == list(s.layout.pids) and list(p.layout.indices) == list(s.layout.indices)
+            p.close()
+            s.close()
+    rt.barrier()
+    log("ok: sortperm(d::DVector) across ranks")
 
     # ---- C5: 256 MiB slab owned by the next rank, contiguous and 2-D strided, bandwidth vs NVLink
     m = 1 << 26
