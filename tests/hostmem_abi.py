@@ -534,46 +534,71 @@ class HostMemABI:
         self.launches += 1
         return 0
 
-    # -- fused map + reduce of a traced expression, Int128 values only (the other value types need dab_combine_ordered etc.)
+    # -- fused map + reduce of a traced expression: the refusals of dab_mapreduce_expr with its status codes, then the result slot as
+    #    mr_spec lays it out (word 0 the result, word 1 the carrier; a 16-byte carrier fills the slot)
     def dab_mapreduce_expr(self, ctx, src, val_dtype, op, n, nargs, dts, ptrs, scal, out):
+        val, op, n, nargs = int(val_dtype), int(op), int(n), int(nargs)
+        if not src or not _addr(out) or not 1 <= nargs <= 8 or dts is None or ptrs is None or scal is None:
+            return 2                                               # DAB_ERR_ARG
+        if val not in range(8):
+            return 2
+        if n == 0:
+            return 3                                               # DAB_ERR_EMPTY
+        if not _mr_served(val, op):
+            return 6                                               # DAB_ERR_UNSUPPORTED
+        for k in range(nargs):
+            if int(dts[k]) not in _ELEM or (not ptrs[k] and int(dts[k]) == 7):
+                return 2                                           # no such element type; a ComplexF64 scalar does not fit 8 bytes
+        if any(ptrs[k] and _addr(ptrs[k]) % (4 * _ELEM[int(dts[k])].itemsize) for k in range(nargs)):
+            return 6                                               # arrays must be aligned to 4 elements
         expr = self.exprs[src]
-        n = int(n)
         args = []
-        for k in range(int(nargs)):
-            p = ptrs[k]
-            if p:
-                args.append(_view(p, n, _NP[int(dts[k])] if int(dts[k]) != U8 else np.bool_).copy())
+        for k in range(nargs):
+            dt = _ELEM[int(dts[k])]
+            if ptrs[k]:
+                args.append(_view(ptrs[k], n, dt).copy())
             else:
-                args.append(np.frombuffer(int(scal[k]).to_bytes(8, "little"), dtype=_NP[int(dts[k])])[0])
-        if int(val_dtype) == U8:                                 # Bool values: all / any / count
-            v = np.broadcast_to(np.asarray(eval_expr(expr, args)), (n,)).astype(bool)
-            acc = {4: int(np.all(v)), 5: int(np.any(v)), 6: int(np.count_nonzero(v))}[int(op)]
-            C.memmove(_addr(out), np.asarray([acc, acc], dtype=np.int64).ctypes.data, 16)
-            self.launches += 2
-            return 0
-        if int(val_dtype) != 5:                                  # array element types: sum in the wide carrier, max / min exact
-            assert int(op) in (0, 1, 2, 3) and int(val_dtype) in (F32, F64, I32, I64), "hostmem_abi: SUM / PROD / MAX / MIN of numeric values only"
-            v = np.broadcast_to(np.asarray(eval_expr(expr, args)), (n,))
-            isf = v.dtype.kind == "f"
-            wide = np.float64 if isf else np.int64
-            with np.errstate(all="ignore"):
-                acc = {0: lambda: v.astype(wide).sum(), 1: lambda: v.astype(wide).prod(), 2: v.max, 3: v.min}[int(op)]()
-            rdt = (v.dtype if isf else np.dtype(np.int64)) if int(op) in (0, 1) else v.dtype
-            slot = np.zeros(16, dtype=np.uint8)
-            slot[:rdt.itemsize] = np.asarray([acc], dtype=rdt).view(np.uint8)
-            slot[8:8 + np.dtype(wide).itemsize] = np.asarray([acc], dtype=wide).view(np.uint8)
-            C.memmove(_addr(out), slot.ctypes.data, 16)
-            self.launches += 2
-            return 0
-        vals = [int(v) for v in np.broadcast_to(eval_expr(expr, args), (n,))]
-        mask = (1 << 128) - 1
-        acc = vals[0]
-        for v in vals[1:]:
-            acc = {0: acc + v, 1: acc * v, 2: max(acc, v), 3: min(acc, v)}[int(op)]
-            acc &= mask
-            acc = acc - (1 << 128) if acc >> 127 else acc
-        C.memmove(_addr(out), (acc & mask).to_bytes(16, "little"), 16)
+                args.append(np.frombuffer(int(scal[k]).to_bytes(8, "little")[:dt.itemsize], dtype=dt)[0])
         self.launches += 2
+        if val == 5:                                               # Int128: Python integers wrapped to 128 bits
+            vals = [int(v) for v in np.broadcast_to(eval_expr(expr, args), (n,))]
+            mask = (1 << 128) - 1
+            acc = vals[0]
+            for v in vals[1:]:
+                acc = {0: acc + v, 1: acc * v, 2: max(acc, v), 3: min(acc, v)}[op]
+                acc &= mask
+                acc = acc - (1 << 128) if acc >> 127 else acc
+            C.memmove(_addr(out), (acc & mask).to_bytes(16, "little"), 16)
+            return 0
+        v = np.broadcast_to(np.asarray(eval_expr(expr, args)), (n,)).astype(_ELEM[val])
+        slot = np.zeros(16, dtype=np.uint8)
+        with np.errstate(all="ignore"):
+            if val == U8:                                          # Bool values: sum / count / all / any, the count is the carrier
+                c = int(np.count_nonzero(v))
+                res = {0: c, 6: c, 4: int(c == n), 5: int(c != 0)}[op]
+                slot.view(np.int64)[:] = [res, c]
+            elif val in (6, 7):                                    # complex: the sum or product in ComplexF64, rounded once
+                w = v.astype(np.complex128)
+                acc = complex(w.real.sum(), w.imag.sum()) if op == 0 else complex(np.prod(w))
+                R = np.float32 if val == 6 else np.float64
+                pair = np.asarray([acc.real, acc.imag], dtype=np.float64).astype(R)
+                slot[:pair.nbytes] = pair.view(np.uint8)
+            elif v.dtype.kind == "f":
+                if op in (0, 1):                                   # exact fp64 carrier, the result rounded once
+                    acc = v.astype(np.float64).sum() if op == 0 else v.astype(np.float64).prod()
+                    slot[:v.itemsize] = np.asarray([acc], dtype=v.dtype).view(np.uint8)
+                    slot[8:] = np.asarray([acc], dtype=np.float64).view(np.uint8)
+                else:                                              # Julia's max / min; the carrier is the value type
+                    r = np.asarray([jl_extreme(v, 0, op == 2)], dtype=v.dtype).view(np.uint8)
+                    slot[:v.itemsize] = slot[8:8 + v.itemsize] = r
+            else:
+                if op in (0, 1):                                   # Int32 widened, Int64 wrapping mod 2^64
+                    w = v.astype(np.int64)
+                    slot.view(np.int64)[:] = w.sum(dtype=np.int64) if op == 0 else w.prod(dtype=np.int64)
+                else:
+                    r = np.asarray([v.max() if op == 2 else v.min()], dtype=v.dtype).view(np.uint8)
+                    slot[:v.itemsize] = slot[8:8 + v.itemsize] = r
+        C.memmove(_addr(out), slot.ctypes.data, 16)
         return 0
 
     def dab_sorted_split(self, ctx, dtype, sorted_p, n, bounds_host, nb, counts):
@@ -597,6 +622,20 @@ class HostMemABI:
             counts[t] = n if rest_nan else lo
         self.launches += 1
         return 0
+
+
+_ELEM = {**_NP, U8: np.dtype(np.bool_), 6: np.dtype(np.complex64), 7: np.dtype(np.complex128)}   # array element types
+
+
+def _mr_served(val: int, op: int) -> bool:
+    """mr_spec of dab_jit.cu: which (value type, op) dab_mapreduce_expr serves."""
+    if val == 5:
+        return op in (0, 1, 2, 3)
+    if val in (6, 7):
+        return op in (0, 1)
+    if val == U8:
+        return op in (0, 4, 5, 6)
+    return op in (0, 1, 2, 3)
 
 
 def jl_extreme(m, axis, is_max):
@@ -628,6 +667,12 @@ def eval_expr(e, args):
         return np.asarray(eval_expr(e.args[0], args)).astype(npt[e.jt])
     a = [eval_expr(x, args) for x in e.args]
     with np.errstate(all="ignore"):
+        if e.op == "complex":
+            return _pack(np.asarray(a[0]), np.asarray(a[1])).astype(npt[e.jt])
+        if e.op in ("conj", "real", "imag"):
+            return {"conj": np.conj, "real": np.real, "imag": np.imag}[e.op](np.asarray(a[0])).astype(npt[e.jt])
+        if e.op in ("add", "sub", "mul", "div") and len({np.iscomplexobj(v) for v in a}) == 2:
+            return _mixed_complex(e.op, a[0], a[1]).astype(npt[e.jt])
         if e.op == "ifelse":
             return np.where(a[0], a[1], a[2])
         if e.op in ("add", "sub", "mul", "div", "rem", "mod", "max", "min", "and", "or", "xor", "lt", "le", "gt", "ge", "eq", "ne", "idiv"):
@@ -658,6 +703,25 @@ def eval_expr(e, args):
                             "x_gamma": sp.gamma, "x_loggamma": sp.gammaln})
             r = one[e.op](np.asarray(a[0]))
         return np.asarray(r).astype(npt[e.jt])
+
+
+def _mixed_complex(op, a, b):
+    """Julia's methods between a real and a complex operand: the real one is not promoted to complex (x*z = Complex(x*zr, x*zi), ...)."""
+    a, b = np.asarray(a), np.asarray(b)
+    if np.iscomplexobj(a):
+        zr, zi, x = a.real, a.imag, b
+        re, im = {"add": (zr + x, zi), "sub": (zr - x, zi), "mul": (zr * x, zi * x), "div": (zr / x, zi / x)}[op]
+    else:
+        x, zr, zi = a, b.real, b.imag
+        re, im = {"add": (x + zr, zi), "sub": (x - zr, -zi), "mul": (x * zr, x * zi)}[op]
+    return _pack(re, im)
+
+
+def _pack(re, im):
+    """Complex values from their components (re + 1j*im would turn an infinite component into NaNs)."""
+    out = np.empty(np.broadcast(re, im).shape, dtype=np.result_type(re, im, np.complex64))
+    out.real, out.imag = re, im
+    return out
 
 
 def jl_shift(x: int, n: int, bits: int, left: bool) -> int:
