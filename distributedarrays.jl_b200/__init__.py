@@ -9,7 +9,8 @@ loader shim).  The public names mirror DistributedArrays.jl's for this path: ``D
 ``mapslices`` (with ``sort``, ``svdvals``, ``eigvals``, reductions,
 elementwise and constant slice functions), ``ppeval`` (batched slice products ``ppeval(operator.matmul, A, B)``, ``eigvals`` of symmetric
 slices, and every ``mapslices`` slice function), ``cumsum`` / ``cumprod`` / ``accumulate`` and their ``!`` forms
-(``cumsum_`` ...), ``Array(d)`` (``to_array``), range ``getindex``; sparse DArrays (``distribute`` of a scipy.sparse matrix: CSC
+(``cumsum_`` ...), ``Array(d)`` (``to_array``), range ``getindex``, ``d[I]`` with ``I`` a DArray of Int32 / Int64 (a gather on the GPU:
+``v[sortperm(v)]``, ``A[findmax(A; dims)[2]]``; a DArray key holds Julia's 1-based linear indices, host Python indices stay 0-based); sparse DArrays (``distribute`` of a scipy.sparse matrix: CSC
 localparts, ``nnz``, ``A*x`` / ``A'*x`` / ``mul!``).
 
 Everything computes on the GPU through ``csrc/libdab200.so`` (C ABI: ``include/dab200.h``).  There is no CPU fallback:

@@ -260,6 +260,10 @@ class DArray:
 
     # ---- indexing (src/darray.jl:642-661) ---------------------------------------------------------------------------------
     def __getitem__(self, key):
+        from ._sparse import SparseDArray
+        if isinstance(key, (DArray, SparseDArray)):
+            from ._take import take                              # d[I]: 1-based linear indices held on the devices (_take.py)
+            return take(self, key)
         if not isinstance(key, tuple):
             key = (key,)
         if len(key) == 1 and self.ndim > 1 and isinstance(key[0], (int, np.integer)):

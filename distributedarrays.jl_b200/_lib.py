@@ -108,6 +108,7 @@ _SIGS = {
     "dab_scan_carrier_dtype": (_i32, [_i32, _i32, _i32, C.POINTER(_i32)]),
     "dab_copy_box": (_i32, [_vp, _i32, _vp, C.POINTER(_sz), C.POINTER(_sz), _vp, C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz)]),
     "dab_gather_box": (_i32, [_vp, _i32, _i32, _vp, C.POINTER(C.c_longlong), _pvp, _vp, C.POINTER(C.c_longlong), _pvp, C.POINTER(_sz)]),
+    "dab_index_gather": (_i32, [_vp, _i32, _vp, _vp, _i32, _sz, _i32, C.POINTER(_sz), C.POINTER(_i32), C.POINTER(_sz), _pvp, _vp]),
     "dab_gemv": (_i32, [_vp, _i32, _i32, _vp, _sz, _sz, _vp, _vp]),
     "dab_spmv": (_i32, [_vp, _i32, _sz, _sz, _vp, _vp, _vp, _vp, _vp]),
     "dab_csc_to_csr": (_i32, [_vp, _i32, _sz, _sz, _sz, _vp, _vp, _vp, _vp, _vp, _vp]),

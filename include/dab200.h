@@ -329,6 +329,22 @@ int32_t dab_copy_box(dab_ctx* ctx, int32_t elem_bytes, void* dst, const size_t d
 int32_t dab_gather_box(dab_ctx* ctx, int32_t elem_bytes, int32_t ndim, void* dst, const long long* dst_strides, const void* const* dst_index,
                        const void* src, const long long* src_strides, const void* const* src_index, const size_t* extent);
 
+/* ==== indexed gather K22 (row f12) ==========================================================
+ * out[k] = d[idx[k]] for k < n: one localpart of R = d[I::DArray{<:Integer}], which Base's generic getindex computes as
+ * similar(d, axes(I)) (src/darray.jl:238) filled by scalar reads.  idx holds the matching block of I: 1-based column-major LINEAR
+ * indices into the whole source d (Julia's A[I::AbstractArray{<:Integer}]); idx_dtype DAB_I32 (widened to 64 bits in the kernel)
+ * or DAB_I64.  Duplicates are allowed.  The source is described by its ndim (1..8) dims, its grid (chunks per dim) and, per dim,
+ * grid[k] + 1 cuts (0-based first element of each chunk along the dim, then dims[k]; empty chunks repeat a cut), concatenated dim
+ * by dim, and one pointer per chunk in column-major grid order: local or a CUDA-IPC peer mapping, NULL allowed for an empty chunk.
+ * At most 1024 chunks (otherwise DAB_ERR_UNSUPPORTED); the table travels by value in the kernel's parameter block.  elem_bytes
+ * 1, 4, 8 or 16: the kernel moves bytes, so NaN payloads and -0.0 are kept.  out aligned to elem_bytes, idx to its element size;
+ * 16-byte aligned idx and out take the 16-byte index loads.  Bounds: an index outside [1, prod(dims)] writes nothing for that
+ * element and atomicMin's its position k into *bad_pos (device, 8 bytes), which the caller initialises to ULLONG_MAX.  n == 0
+ * launches nothing.  Asynchronous on the ctx stream. */
+int32_t dab_index_gather(dab_ctx* ctx, int32_t elem_bytes, void* out, const void* idx, int32_t idx_dtype, size_t n, int32_t ndim,
+                         const size_t* dims, const int32_t* grid, const size_t* cuts, const void* const* chunk_ptrs,
+                         unsigned long long* bad_pos);
+
 /* ==== Level-2 linear algebra K9 (widening row f4; HBM-bound) ==============================
  * r = op(A) * x on ONE column-major chunk A (m x n, leading dimension m): trans = 0 -> r[m] = A x[n];
  * trans = 1 -> r[n] = A' x[m].  Replaces  localpart(A)*convert(localtype(x), xj)  (src/linalg.jl:95-97)

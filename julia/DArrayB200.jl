@@ -28,6 +28,8 @@
 #   (no reference method)  accumulate!(op, lp, lp; dims)   Base.accumulate! (cumsum! / cumprod!)   dab_scan
 #   src/linalg.jl:95-97,141 localpart(A)*xj, SparseMatrixCSC chunks   Base.:* (SparseB200Chunk)   dab_spmv / dab_csc_to_csr
 #   (Base._findmax: scalar getindex)  findmax(f, d) / findmin(f, d)   (DArray methods below)   dab_findminmax / dab_combine_findminmax
+#   (Base getindex(A, I::AbstractArray): similar(d, axes(I)), src/darray.jl:238, scalar reads)  d[I::DArray{<:Integer}]
+#                                                         Base.getindex(::DArray, ::DArray{<:Integer})   dab_index_gather
 module DArrayB200
 
 using Distributed, DistributedArrays, LinearAlgebra
@@ -498,6 +500,57 @@ function Base.getindex(a::B200Array{T,N}, I::Vararg{Union{AbstractRange{Int},Vec
                 ctx(), sizeof(T), N, out.ptr, Clonglong[dstr...], C_NULL, src, zeros(Clonglong, N), Ptr{Cvoid}[t.ptr for t in tabs],
                 Csize_t[length.(I)...]), ctx())
     out
+end
+
+# d[I::DArray{<:Integer}] (Base's generic getindex: similar(d, axes(I)), src/darray.jl:238, filled by scalar reads): K22 on every
+# localpart of R = similar(d, size(I)).  I[k] is a 1-based column-major linear index into d.  Every worker of R maps the other
+# workers' localparts of d over CUDA IPC and reads its block of I with the reference's halo getindex (src/darray.jl:798-820), which
+# brings the block through the host (the Python runtime copies it device to device); bad positions come back by remotecall_fetch.
+# Peer mappings are cached per handle on each worker, as in the Python runtime, and released by ipc_close_all() (call it before
+# the owners free their localparts, e.g. when the worker shuts down).
+const IPC_MAPS = Dict{Vector{UInt8},Ptr{Cvoid}}()
+function ipc_handle(a::B200Array)
+    h = zeros(UInt8, 64)
+    length(a) == 0 || check(ccall((:dab_ipc_get_handle, libdab), Int32, (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{UInt8}), ctx(), a.ptr, h), ctx())
+    h
+end
+ipc_open(h::Vector{UInt8}) = get!(IPC_MAPS, h) do
+    p = Ref{Ptr{Cvoid}}(C_NULL)
+    check(ccall((:dab_ipc_open, libdab), Int32, (Ptr{Cvoid}, Ptr{UInt8}, Ref{Ptr{Cvoid}}), ctx(), h, p), ctx())
+    p[]
+end
+function ipc_close_all()
+    for p in values(IPC_MAPS)
+        check(ccall((:dab_ipc_close, libdab), Int32, (Ptr{Cvoid}, Ptr{Cvoid}), ctx(), p), ctx())
+    end
+    empty!(IPC_MAPS)
+end
+function Base.getindex(d::DArray{T,N,B200Array{T,N}}, I::DArray{<:Integer}) where {T,N}
+    eltype(I) <: Union{Int32,Int64} || throw(ArgumentError("index element type $(eltype(I)) is not served (Int32, Int64)"))
+    R = similar(d, size(I))
+    owners = vec(d.pids)
+    handles = Dict(p => remotecall_fetch(() -> ipc_handle(localpart(d)), p) for p in owners)
+    # 0-based chunk starts from the chunk extents (an empty chunk repeats a cut), then size(d, k)
+    cuts = reduce(vcat, [cumsum([0; [length(d.indices[ntuple(j -> j == k ? c : 1, N)...][k]) for c in 1:size(d.pids, k)]]) for k in 1:N])
+    bad = asyncmap(procs(R)) do p
+        remotecall_fetch(p) do
+            J = localindices(R)
+            ptrs = Ptr{Cvoid}[any(isempty, d.indices[c]) ? C_NULL : q == myid() ? localpart(d).ptr : ipc_open(handles[q])
+                              for (c, q) in enumerate(owners)]
+            blk = B200Array(Array(I[J...]))                                   # the halo read of I's block, uploaded
+            pos = B200Array(fill(typemax(UInt64), 1))
+            check(ccall((:dab_index_gather, libdab), Int32,
+                        (Ptr{Cvoid}, Int32, Ptr{Cvoid}, Ptr{Cvoid}, Int32, Csize_t, Int32, Ptr{Csize_t}, Ptr{Int32}, Ptr{Csize_t},
+                         Ptr{Ptr{Cvoid}}, Ptr{Cvoid}),
+                        ctx(), sizeof(T), localpart(R).ptr, blk.ptr, dab_dtype(eltype(I)), length(blk), N, Csize_t[size(d)...],
+                        Int32[size(d.pids)...], Csize_t[cuts...], ptrs, pos.ptr), ctx())
+            b = Array(pos)[1]
+            b == typemax(UInt64) ? nothing : (LinearIndices(size(I))[CartesianIndex(Tuple(CartesianIndices(map(length, J))[b + 1]) .+ first.(J) .- 1)])
+        end
+    end
+    found = filter(!isnothing, bad)
+    isempty(found) || (close(R); throw(BoundsError(d, I[minimum(found)])))
+    R
 end
 
 # user code is then unchanged:
