@@ -10,7 +10,9 @@ loader shim).  The public names mirror DistributedArrays.jl's for this path: ``D
 elementwise and constant slice functions), ``ppeval`` (batched slice products ``ppeval(operator.matmul, A, B)``, ``eigvals`` of symmetric
 slices, and every ``mapslices`` slice function), ``cumsum`` / ``cumprod`` / ``accumulate`` and their ``!`` forms
 (``cumsum_`` ...), ``Array(d)`` (``to_array``), range ``getindex``, ``d[I]`` with ``I`` a DArray of Int32 / Int64 (a gather on the GPU:
-``v[sortperm(v)]``, ``A[findmax(A; dims)[2]]``; a DArray key holds Julia's 1-based linear indices, host Python indices stay 0-based); sparse DArrays (``distribute`` of a scipy.sparse matrix: CSC
+``v[sortperm(v)]``, ``A[findmax(A; dims)[2]]``; a DArray key holds Julia's 1-based linear indices, host Python indices stay 0-based),
+logical indexing ``d[mask]`` with a Bool DArray of ``d``'s dims, ``findall(mask)`` / ``findall(f, d)`` (1-based linear indices as a
+``DArray{Int64}``) and ``filter(f, d)`` (stream compaction on the GPU; results are DVectors in column-major order); sparse DArrays (``distribute`` of a scipy.sparse matrix: CSC
 localparts, ``nnz``, ``A*x`` / ``A'*x`` / ``mul!``).
 
 Everything computes on the GPU through ``csrc/libdab200.so`` (C ABI: ``include/dab200.h``).  There is no CPU fallback:
@@ -33,6 +35,7 @@ from ._mapreduce import (all, any, axpy_, count, dot, extrema, isequal, mapreduc
                          prod, reduce, rmul_, sum)
 from ._linalg import Adjoint, Transpose, adjoint, copy_transposed, lmul_diag, matmat, matmul, mul_, mul_mat_, rmul_diag, transpose
 from ._findmax import argmax, argmin, findmax, findmin
+from ._compact import filter, findall  # noqa: A004
 from ._sort import sort, sort_with_boundaries, sortperm
 from ._scan import accumulate, accumulate_, cumprod, cumprod_, cumsum, cumsum_
 from ._slices import eigvals, mapslices, svdvals

@@ -261,6 +261,9 @@ class DArray:
     # ---- indexing (src/darray.jl:642-661) ---------------------------------------------------------------------------------
     def __getitem__(self, key):
         from ._sparse import SparseDArray
+        if isinstance(key, DArray) and key.dtype == np.bool_ and key.dims == self.dims:
+            from ._compact import getindex_mask                  # d[mask]: stream compaction on the devices (_compact.py)
+            return getindex_mask(self, key)
         if isinstance(key, (DArray, SparseDArray)):
             from ._take import take                              # d[I]: 1-based linear indices held on the devices (_take.py)
             return take(self, key)

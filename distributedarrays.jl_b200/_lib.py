@@ -23,6 +23,7 @@ ADD, SUB, MUL, DIV, REM, BMAX, BMIN, MOD, IDIV, AND, OR, XOR = range(12)
 SORT_SLICES_SMEM_LEN = 8192                   # longest fibre dab_sort_slices sorts in shared memory
 SVDVALS_MAX_K, SVDVALS_MAX_ELEMS = 32, 4096   # dab_svdvals_batched serves min(m, n) <= 32 and m * n <= 4096
 EIGVALS_SYM_MAX_N = 64                        # dab_eigvals_sym_batched serves n <= 64
+COMPACT_TILE, COMPACT_INDEX = 4096, 0          # dab_compact_count / dab_compact: tile length, index mode
 
 
 class DabError(RuntimeError):
@@ -109,6 +110,8 @@ _SIGS = {
     "dab_copy_box": (_i32, [_vp, _i32, _vp, C.POINTER(_sz), C.POINTER(_sz), _vp, C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz)]),
     "dab_gather_box": (_i32, [_vp, _i32, _i32, _vp, C.POINTER(C.c_longlong), _pvp, _vp, C.POINTER(C.c_longlong), _pvp, C.POINTER(_sz)]),
     "dab_index_gather": (_i32, [_vp, _i32, _vp, _vp, _i32, _sz, _i32, C.POINTER(_sz), C.POINTER(_i32), C.POINTER(_sz), _pvp, _vp]),
+    "dab_compact_count": (_i32, [_vp, _vp, _sz, _sz, _vp]),
+    "dab_compact": (_i32, [_vp, _i32, _vp, _vp, _sz, _sz, _vp, _vp, _i32, C.POINTER(_sz), _pvp]),
     "dab_gemv": (_i32, [_vp, _i32, _i32, _vp, _sz, _sz, _vp, _vp]),
     "dab_spmv": (_i32, [_vp, _i32, _sz, _sz, _vp, _vp, _vp, _vp, _vp]),
     "dab_csc_to_csr": (_i32, [_vp, _i32, _sz, _sz, _sz, _vp, _vp, _vp, _vp, _vp, _vp]),

@@ -300,7 +300,9 @@ def fence(rt, kind: str):
 def open_remote_reads(rt, arrays: Sequence, kind: str) -> bool:
     """Opening half of a one-sided read of other ranks' chunks of the DArrays ``arrays``: shares the CUDA-IPC handles not
     shared yet and fences the producers, so that every earlier write to those chunks has landed before a peer reads them.
-    Nothing happens on one rank or for an empty list.  Returns whether it fenced; pass that to ``close_remote_reads``."""
+    It opens one-sided WRITES the same way (``d[mask]`` stores into other ranks' chunks of its result): every owner has
+    allocated the chunk and finished with it before a peer stores into it.  Nothing happens on one rank or for an empty
+    list.  Returns whether it fenced; pass that to ``close_remote_reads``."""
     if rt.world == 1 or not arrays:
         return False
     for a in arrays:
@@ -313,7 +315,8 @@ def open_remote_reads(rt, arrays: Sequence, kind: str) -> bool:
 def close_remote_reads(rt, fenced: bool, kind: str):
     """Closing half of ``open_remote_reads``, with the same fence kind: the owners of the chunks that were read may not
     overwrite or free them before every reader's copy has run (freed blocks go straight back to the allocator cache).  The
-    reference's ``remotecall_fetch`` is synchronous for the same reason."""
+    reference's ``remotecall_fetch`` is synchronous for the same reason.  After one-sided writes the closing fence is what
+    makes the peers' stores visible to the chunks' owners."""
     if fenced:
         if kind == "host":
             rt.sync()

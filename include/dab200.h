@@ -345,6 +345,29 @@ int32_t dab_index_gather(dab_ctx* ctx, int32_t elem_bytes, void* out, const void
                          const size_t* dims, const int32_t* grid, const size_t* cuts, const void* const* chunk_ptrs,
                          unsigned long long* bad_pos);
 
+/* ==== stream compaction K23 (row f13) ========================================================
+ * The kernels of d[mask::DArray{Bool}], findall(mask) and filter(f, d), which Base computes by scalar iteration.  One call serves
+ * one chunk, cut into `runs` RUNS of run_len elements that lie back to back in the chunk's storage and are each contiguous in the
+ * global column-major order (the host derives them from the layout: DESIGN.md section 3.10).  Each run is cut into
+ * tiles_per_run = ceil(run_len / DAB_COMPACT_TILE) tiles; tile b = r * tiles_per_run + t covers chunk elements
+ * [r * run_len + t * DAB_COMPACT_TILE, r * run_len + min((t + 1) * DAB_COMPACT_TILE, run_len)).  A mask byte is true when nonzero.
+ * The mask may have any alignment (16-byte loads where a tile starts 16-byte aligned).  Asynchronous on the ctx stream;
+ * run_len == 0 or runs == 0 launches nothing.  More than 2^31 - 1 tiles: DAB_ERR_UNSUPPORTED. */
+#define DAB_COMPACT_TILE 4096
+#define DAB_COMPACT_INDEX 0
+/* counts[b] (Int32) = the number of true bytes of mask tile b. */
+int32_t dab_compact_count(dab_ctx* ctx, const void* mask, size_t run_len, size_t runs, int32_t* counts);
+/* Writes the selected elements of the chunk, in order, to a 1-D output of nchunks (1..1024) chunks: the element at run position i
+ * of run r that is the p-th true of its run goes to output position run_info[2r] + p.  tile_incl: the Int64 inclusive scan of
+ * counts along each run (dab_scan DAB_I32 -> DAB_I64, SUM, inner 1, len tiles_per_run, outer runs).  The output is described by
+ * nchunks + 1 cuts (0-based first position of each chunk, then its length; empty chunks repeat a cut) and one pointer per chunk,
+ * local or a CUDA-IPC peer mapping (NULL allowed for an empty chunk), passed by value.  elem_bytes 1, 4, 8 or 16: src[element] is
+ * copied as bytes (NaN payloads and -0.0 kept); elem_bytes == DAB_COMPACT_INDEX: the Int64 run_info[2r + 1] + i + 1 is written
+ * (run_info[2r + 1] is the 0-based global linear index of the run's first element; src unused).  Positions at or past the output
+ * length are not written. */
+int32_t dab_compact(dab_ctx* ctx, int32_t elem_bytes, const void* mask, const void* src, size_t run_len, size_t runs, const int64_t* tile_incl,
+                    const int64_t* run_info, int32_t nchunks, const size_t* cuts, void* const* chunk_ptrs);
+
 /* ==== Level-2 linear algebra K9 (widening row f4; HBM-bound) ==============================
  * r = op(A) * x on ONE column-major chunk A (m x n, leading dimension m): trans = 0 -> r[m] = A x[n];
  * trans = 1 -> r[n] = A' x[m].  Replaces  localpart(A)*convert(localtype(x), xj)  (src/linalg.jl:95-97)

@@ -30,6 +30,8 @@
 #   (Base._findmax: scalar getindex)  findmax(f, d) / findmin(f, d)   (DArray methods below)   dab_findminmax / dab_combine_findminmax
 #   (Base getindex(A, I::AbstractArray): similar(d, axes(I)), src/darray.jl:238, scalar reads)  d[I::DArray{<:Integer}]
 #                                                         Base.getindex(::DArray, ::DArray{<:Integer})   dab_index_gather
+#   (Base getindex(A, I::AbstractArray{Bool}) / findall: scalar iteration)  d[m::DArray{Bool}], findall(m)
+#                                                         Base.getindex(::DArray, ::DArray{Bool}), Base.findall   dab_compact_count / dab_compact
 module DArrayB200
 
 using Distributed, DistributedArrays, LinearAlgebra
@@ -552,6 +554,74 @@ function Base.getindex(d::DArray{T,N,B200Array{T,N}}, I::DArray{<:Integer}) wher
     isempty(found) || (close(R); throw(BoundsError(d, I[minimum(found)])))
     R
 end
+
+# d[m::DArray{Bool}] and findall(m) (Base's generic methods iterate element by element): K23 on every localpart of d, DESIGN.md §3.10.
+# A run of a chunk is contiguous in the global column-major order; with k the first split dimension, chunk c has runs of
+# prod(size(d)[1:k-1]) * ext[k] elements, run ids b + grid[k] * o and first linear indices inner * (start_k + size(d, k) * o).  Phase
+# 1 counts tiles and scans them on each owner (the tables wait in COMPACT_PLANS), the host lays out the run offsets, phase 2 writes
+# the selected elements into R's localparts through peer mappings.
+const COMPACT_PLANS = Dict{Tuple{UInt,Int},Any}()
+function compact_runs(d::DArray)
+    dims, grid = size(d), size(d.pids)
+    k = something(findfirst(>(1), grid), length(dims))
+    inner, outer = prod(dims[1:k-1]), dims[k+1:end]
+    runs = map(enumerate(d.indices)) do (c, I)
+        ext = map(length, I)
+        os = Int64[LinearIndices(outer)[CartesianIndex(Tuple(o) .+ first.(I[k+1:end]) .- 1)] - 1 for o in CartesianIndices(ext[k+1:end])]
+        (inner * ext[k], ((c - 1) % grid[k]) .+ grid[k] .* os, inner .* (first(I[k]) - 1) .+ inner * dims[k] .* os)
+    end
+    runs, grid[k] * prod(outer)
+end
+function compact(d::DArray{T,N,B200Array{T,N}}, m::DArray{Bool,N}, index::Bool) where {T,N}
+    size(m) == size(d) || throw(ArgumentError("logical indexing with a DArray{Bool} of other dims is not served"))
+    runs, nruns = compact_runs(d)
+    owners, key = vec(d.pids), objectid(d)
+    tots = asyncmap(enumerate(owners)) do (c, p)
+        remotecall_fetch(p) do
+            run_len, ids, _ = runs[c]
+            run_len * length(ids) == 0 && return zeros(Int64, length(ids))
+            blk = B200Array(Array(m[d.indices[c]...]))                        # the halo read of the mask block, uploaded
+            tiles = cld(run_len, 4096) * length(ids)
+            counts, incl, tot = B200Array(zeros(Int32, tiles)), B200Array(zeros(Int64, tiles)), B200Array(zeros(Int64, length(ids)))
+            check(ccall((:dab_compact_count, libdab), Int32, (Ptr{Cvoid}, Ptr{Cvoid}, Csize_t, Csize_t, Ptr{Cvoid}), ctx(), blk.ptr, run_len,
+                        length(ids), counts.ptr), ctx())
+            tpr, nr = tiles ÷ length(ids), length(ids)                         # Int32 SUM -> Int64 along each run of the tile table
+            check(ccall((:dab_scan, libdab), Int32, (Ptr{Cvoid}, Int32, Int32, Int32, Ptr{Cvoid}, Csize_t, Csize_t, Csize_t, Ptr{Cvoid}, Ptr{Cvoid}),
+                        ctx(), dab_dtype(Int32), Int32(0), dab_dtype(Int64), counts.ptr, 1, tpr, nr, C_NULL, incl.ptr), ctx())
+            check(ccall((:dab_scan_totals, libdab), Int32, (Ptr{Cvoid}, Int32, Int32, Int32, Ptr{Cvoid}, Csize_t, Csize_t, Csize_t, Ptr{Cvoid}),
+                        ctx(), dab_dtype(Int32), Int32(0), dab_dtype(Int64), counts.ptr, 1, tpr, nr, tot.ptr), ctx())
+            COMPACT_PLANS[(key, c)] = (blk, incl)
+            Array(tot)
+        end
+    end
+    totals = zeros(Int64, nruns)
+    for (c, t) in enumerate(tots)
+        totals[runs[c][2] .+ 1] .= t
+    end
+    offsets = [0; cumsum(totals)]
+    R = similar(d, index ? Int64 : T, (offsets[end],))
+    offsets[end] == 0 && return R
+    handles = Dict(p => remotecall_fetch(() -> ipc_handle(localpart(R)), p) for p in procs(R))
+    cuts = Csize_t[0; cumsum([length(I[1]) for I in vec(R.indices)])]
+    asyncmap(enumerate(owners)) do (c, p)
+        remotecall_fetch(p) do
+            plan = pop!(COMPACT_PLANS, (key, c), nothing)
+            plan === nothing && return nothing
+            run_len, ids, lin = runs[c]
+            info = B200Array(vec(permutedims([offsets[ids .+ 1] lin])))
+            ptrs = Ptr{Cvoid}[isempty(R.indices[j][1]) ? C_NULL : q == myid() ? localpart(R).ptr : ipc_open(handles[q])
+                              for (j, q) in enumerate(vec(R.pids))]
+            check(ccall((:dab_compact, libdab), Int32, (Ptr{Cvoid}, Int32, Ptr{Cvoid}, Ptr{Cvoid}, Csize_t, Csize_t, Ptr{Cvoid}, Ptr{Cvoid},
+                        Int32, Ptr{Csize_t}, Ptr{Ptr{Cvoid}}), ctx(), index ? 0 : sizeof(T), plan[1].ptr, index ? C_NULL : localpart(d).ptr,
+                        run_len, length(ids), plan[2].ptr, info.ptr, length(ptrs), cuts, ptrs), ctx())
+            check(ccall((:dab_sync, libdab), Int32, (Ptr{Cvoid},), ctx()), ctx())   # the peer stores have landed before R is read
+            nothing
+        end
+    end
+    R
+end
+Base.getindex(d::DArray{T,N,B200Array{T,N}}, m::DArray{Bool,N}) where {T,N} = compact(d, m, false)
+Base.findall(m::DArray{Bool,N,B200Array{Bool,N}}) where {N} = compact(m, m, true)   # linear indices, on the devices (DESIGN.md §3.10)
 
 # user code is then unchanged:
 #   d = DArray(I -> B200Array(rand(Float32, map(length, I))), (8 * 2^30,))
