@@ -12,7 +12,9 @@ slices, and every ``mapslices`` slice function), ``cumsum`` / ``cumprod`` / ``ac
 (``cumsum_`` ...), ``Array(d)`` (``to_array``), range ``getindex``, ``d[I]`` with ``I`` a DArray of Int32 / Int64 (a gather on the GPU:
 ``v[sortperm(v)]``, ``A[findmax(A; dims)[2]]``; a DArray key holds Julia's 1-based linear indices, host Python indices stay 0-based),
 logical indexing ``d[mask]`` with a Bool DArray of ``d``'s dims, ``findall(mask)`` / ``findall(f, d)`` (1-based linear indices as a
-``DArray{Int64}``) and ``filter(f, d)`` (stream compaction on the GPU; results are DVectors in column-major order); sparse DArrays (``distribute`` of a scipy.sparse matrix: CSC
+``DArray{Int64}``) and ``filter(f, d)`` (stream compaction on the GPU; results are DVectors in column-major order); ``d[key] = v`` for
+every key ``d[key]`` takes, and ``copyto(view, src)`` (a scatter on the GPU for a DArray key, the last occurrence of a repeated index
+winning as in Julia's sequential ``setindex!``; ``d[mask] = v`` as the inverse of compaction; a scalar, host array or DArray value); sparse DArrays (``distribute`` of a scipy.sparse matrix: CSC
 localparts, ``nnz``, ``A*x`` / ``A'*x`` / ``mul!``).
 
 Everything computes on the GPU through ``csrc/libdab200.so`` (C ABI: ``include/dab200.h``).  There is no CPU fallback:

@@ -71,60 +71,72 @@ def _check(d, m):
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"a result over {len(procs(d))} workers (served: up to {MAX_CHUNKS})")
 
 
-def _compact(d: DArray, m: DArray, index: bool) -> DArray:
-    """The selected elements of ``d`` (``index``: their 1-based linear indices, Int64) where the Bool DArray ``m`` of ``d``'s dims is
-    true, in column-major order, as a DVector with the layout of ``similar(d, T, (count,))``.  Collective."""
+def plan(d: DArray, m: DArray, temps: list):
+    """Phases 1 and 2 of ``d[m]`` (and of ``d[m] = v``) for a non-empty ``d`` and a Bool DArray ``m`` of its dims: per local non-empty
+    chunk the mask block in ``d``'s chunk shape and the scans of its tile counts, then the global output offset of every run.  Returns
+    ``(runs, work, plans, offsets)``: ``run_plan(d.layout)``'s runs, the ``(chunk, pid)`` pairs served here, ``plans[chunk] = (mask
+    block, inclusive tile scan, run totals)``, and the ``nruns + 1`` offsets whose last entry is ``count(m)``.  Every device block it
+    allocates goes to ``temps``, which the caller frees.  Collective."""
     rt = d.rt
     lay = d.layout
-    dt = np.dtype(np.int64) if index else d.dtype
-    if d.size == 0:
-        return similar(d, dt, (0,))
     runs, nruns = run_plan(lay)
     mine = [(c, pid) for c, pid in enumerate(lay.pids) if pid in d.chunks]
     work = [(c, pid) for c, pid in mine if d.chunks[pid].size]
     same = m.layout.same_as(lay)
-    temps, plans, R = [], {}, None
-    try:
-        fenced = open_remote_reads(rt, [] if same else [m], "device")
-        for c, pid in work:
-            run_len, ids, _ = runs[c]
-            if same:
-                blk = m.chunks[pid]
-            else:                                              # the mask block in d's chunk shape: a halo read of 1-byte elements
-                blk = B200Array.empty(rt, d.chunks[pid].shape, np.bool_, temp=True)
-                temps.append(blk)
-                SubDArray(m, lay.indices[c], tuple(False for _ in lay.indices[c])).copy_to(blk)
-            tiles = -(-run_len // _lib.COMPACT_TILE) * ids.size
-            counts = B200Array.empty(rt, (tiles,), np.int32, temp=True)
-            incl = B200Array.empty(rt, (tiles,), np.int64, temp=True)
-            tot = B200Array.empty(rt, (ids.size,), np.int64, temp=True)
-            temps += [counts, incl, tot]
-            _lib.call("dab_compact_count", rt.ctx, C.c_void_p(blk.ptr), run_len, ids.size, C.c_void_p(counts.ptr))
-            tpr = tiles // ids.size
-            _lib.call("dab_scan", rt.ctx, _lib.I32, _lib.SUM, _lib.I64, C.c_void_p(counts.ptr), 1, tpr, ids.size, None, C.c_void_p(incl.ptr))
-            _lib.call("dab_scan_totals", rt.ctx, _lib.I32, _lib.SUM, _lib.I64, C.c_void_p(counts.ptr), 1, tpr, ids.size, C.c_void_p(tot.ptr))
-            plans[c] = (blk, incl, tot)
-        close_remote_reads(rt, fenced, "device")
+    plans = {}
+    fenced = open_remote_reads(rt, [] if same else [m], "device")
+    for c, pid in work:
+        run_len, ids, _ = runs[c]
+        if same:
+            blk = m.chunks[pid]
+        else:                                              # the mask block in d's chunk shape: a halo read of 1-byte elements
+            blk = B200Array.empty(rt, d.chunks[pid].shape, np.bool_, temp=True)
+            temps.append(blk)
+            SubDArray(m, lay.indices[c], tuple(False for _ in lay.indices[c])).copy_to(blk)
+        tiles = -(-run_len // _lib.COMPACT_TILE) * ids.size
+        counts = B200Array.empty(rt, (tiles,), np.int32, temp=True)
+        incl = B200Array.empty(rt, (tiles,), np.int64, temp=True)
+        tot = B200Array.empty(rt, (ids.size,), np.int64, temp=True)
+        temps += [counts, incl, tot]
+        _lib.call("dab_compact_count", rt.ctx, C.c_void_p(blk.ptr), run_len, ids.size, C.c_void_p(counts.ptr))
+        tpr = tiles // ids.size
+        _lib.call("dab_scan", rt.ctx, _lib.I32, _lib.SUM, _lib.I64, C.c_void_p(counts.ptr), 1, tpr, ids.size, None, C.c_void_p(incl.ptr))
+        _lib.call("dab_scan_totals", rt.ctx, _lib.I32, _lib.SUM, _lib.I64, C.c_void_p(counts.ptr), 1, tpr, ids.size, C.c_void_p(tot.ptr))
+        plans[c] = (blk, incl, tot)
+    close_remote_reads(rt, fenced, "device")
 
-        # every rank sends the run totals of its chunks in layout order, padded to the longest payload of any rank
-        per_rank = [0] * rt.world
-        for c, pid in enumerate(lay.pids):
-            per_rank[rt.rank_of(pid)] += runs[c][1].size
-        payload = np.zeros(max(max(per_rank), 1), dtype=np.int64)
-        o = 0
-        for c, _ in mine:
-            n = runs[c][1].size
-            if c in plans:
-                payload[o:o + n] = plans[c][2].to_numpy()
-            o += n
-        totals = np.zeros(nruns, dtype=np.int64)
-        cursor = [0] * rt.world
-        gathered = rt.allgather_small(payload)
-        for c, pid in enumerate(lay.pids):
-            r, n = rt.rank_of(pid), runs[c][1].size
-            totals[runs[c][1]] = gathered[r][cursor[r]:cursor[r] + n]
-            cursor[r] += n
-        offsets = np.concatenate([[0], np.cumsum(totals)]).astype(np.int64)
+    # every rank sends the run totals of its chunks in layout order, padded to the longest payload of any rank
+    per_rank = [0] * rt.world
+    for c, pid in enumerate(lay.pids):
+        per_rank[rt.rank_of(pid)] += runs[c][1].size
+    payload = np.zeros(max(max(per_rank), 1), dtype=np.int64)
+    o = 0
+    for c, _ in mine:
+        n = runs[c][1].size
+        if c in plans:
+            payload[o:o + n] = plans[c][2].to_numpy()
+        o += n
+    totals = np.zeros(nruns, dtype=np.int64)
+    cursor = [0] * rt.world
+    gathered = rt.allgather_small(payload)
+    for c, pid in enumerate(lay.pids):
+        r, n = rt.rank_of(pid), runs[c][1].size
+        totals[runs[c][1]] = gathered[r][cursor[r]:cursor[r] + n]
+        cursor[r] += n
+    offsets = np.concatenate([[0], np.cumsum(totals)]).astype(np.int64)
+    return runs, work, plans, offsets
+
+
+def _compact(d: DArray, m: DArray, index: bool) -> DArray:
+    """The selected elements of ``d`` (``index``: their 1-based linear indices, Int64) where the Bool DArray ``m`` of ``d``'s dims is
+    true, in column-major order, as a DVector with the layout of ``similar(d, T, (count,))``.  Collective."""
+    rt = d.rt
+    dt = np.dtype(np.int64) if index else d.dtype
+    if d.size == 0:
+        return similar(d, dt, (0,))
+    temps, R = [], None
+    try:
+        runs, work, plans, offsets = plan(d, m, temps)
         count = int(offsets[-1])
 
         R = similar(d, dt, (count,))

@@ -267,6 +267,17 @@ class DArray:
         if isinstance(key, (DArray, SparseDArray)):
             from ._take import take                              # d[I]: 1-based linear indices held on the devices (_take.py)
             return take(self, key)
+        S = self._view(key)
+        return S.to_numpy()[()] if S.scalar else S
+
+    def __setitem__(self, key, v):
+        """``d[key] = v``: ``setindex!`` for every key ``__getitem__`` takes (_setindex.py).  Collective."""
+        from ._setindex import setindex
+        setindex(self, key, v)
+
+    def _view(self, key) -> "SubDArray":
+        """The view ``d[key]`` selects, for host keys (ints, slices, int lists and arrays; 0-based).  All ints: the one element, a view
+        whose ``scalar`` is true."""
         if not isinstance(key, tuple):
             key = (key,)
         if len(key) == 1 and self.ndim > 1 and isinstance(key[0], (int, np.integer)):
@@ -277,7 +288,7 @@ class DArray:
             if not _allowscalar[0]:
                 raise RuntimeError("ErrorException: scalar indexing disabled")  # src/darray.jl:640
             J = tuple((int(k) % s + 1, int(k) % s + 1) if -s <= int(k) < s else _oob(k, s) for k, s in zip(key, self.dims))
-            return SubDArray(self, J, tuple(True for _ in key)).to_numpy()[()]
+            return SubDArray(self, J, tuple(True for _ in key))
         J, drop, idx = [], [], []
         for k, s in zip(key, self.dims):
             if isinstance(k, (int, np.integer)):
@@ -364,6 +375,11 @@ class SubDArray:
     def __init__(self, parent: DArray, J: Tuple[Range, ...], drop: Tuple[bool, ...], idx: Optional[Tuple] = None):
         self.parent, self.J, self.drop = parent, J, drop
         self.idx = idx if idx is not None else tuple(None for _ in J)
+
+    @property
+    def scalar(self) -> bool:
+        """Every index is an Int: the view holds one element (``d[i, j]``)."""
+        return all(self.drop)
 
     @property
     def unit(self) -> bool:
@@ -514,6 +530,14 @@ class SubDArray:
 
     def __getitem__(self, key):
         """``view(s, I...)`` of a view composes into a view of the parent (Base.reindex)."""
+        return self.parent[self._parent_key(key)]
+
+    def __setitem__(self, key, v):
+        """``s[key] = v`` writes through to the parent, as a Julia view does (Base.reindex).  Collective."""
+        self.parent[self._parent_key(key)] = v
+
+    def _parent_key(self, key) -> tuple:
+        """The parent key (0-based) that ``key`` selects in this view."""
         if not isinstance(key, tuple):
             key = (key,)
         kept = [k for k, dr in enumerate(self.drop) if not dr]
@@ -535,7 +559,7 @@ class SubDArray:
                     pkey[k] = slice(int(w[0]), int(w[0]) + int(w.size))
                 else:
                     pkey[k] = np.asarray(w, dtype=np.int64)
-        return self.parent[tuple(pkey)]
+        return tuple(pkey)
 
 
 # ---- constructors --------------------------------------------------------------------------------------------------------
@@ -768,9 +792,13 @@ def to_array(d: DArray) -> np.ndarray:
 
 
 def copyto(dest: DArray, src: np.ndarray) -> DArray:
-    """``copyto!(dest::DArray, src::AbstractArray)`` (src/darray.jl:679-687): per worker ``copyto!(localpart(dest), view(src,
-    localindices(dest)...))``.  A host array is uploaded slice by slice; a DArray / SubDArray source (test/darray.jl:225-234) stays on the
-    devices -- one identity broadcast per localpart, the view of a differently laid out source being the usual halo fetch."""
+    """``copyto!(dest::SubOrDArray, src::AbstractArray)`` (src/darray.jl:679-687): per worker ``copyto!(localpart(dest), view(src,
+    localindices(dest)...))``; a view ``dest`` takes the writes of ``view[:] = src`` (_setindex.py).  A host array is uploaded slice by
+    slice; a DArray / SubDArray source (test/darray.jl:225-234) stays on the devices -- one identity broadcast per localpart, the view of
+    a differently laid out source being the usual halo fetch."""
+    if isinstance(dest, SubDArray):                            # copyto!(view, src): the same writes as view[:] = src
+        from ._setindex import copyto_view
+        return copyto_view(dest, src)
     if isinstance(src, (DArray, SubDArray)):
         from ._broadcast import broadcast_into
         if tuple(src.dims) != dest.dims:

@@ -112,6 +112,10 @@ _SIGS = {
     "dab_index_gather": (_i32, [_vp, _i32, _vp, _vp, _i32, _sz, _i32, C.POINTER(_sz), C.POINTER(_i32), C.POINTER(_sz), _pvp, _vp]),
     "dab_compact_count": (_i32, [_vp, _vp, _sz, _sz, _vp]),
     "dab_compact": (_i32, [_vp, _i32, _vp, _vp, _sz, _sz, _vp, _vp, _i32, C.POINTER(_sz), _pvp]),
+    "dab_scatter_check": (_i32, [_vp, _vp, _i32, _sz, _i32, C.POINTER(_sz), C.POINTER(_i32), C.POINTER(_sz), _pvp, _vp]),
+    "dab_scatter_winners": (_i32, [_vp, _vp, _i32, _sz, _sz, _vp, _i32, _i32, C.POINTER(_sz), C.POINTER(_i32), C.POINTER(_sz), _pvp]),
+    "dab_scatter": (_i32, [_vp, _i32, _vp, _i32, _sz, _vp, _vp, _sz, _vp, _i32, _i32, C.POINTER(_sz), C.POINTER(_i32), C.POINTER(_sz), _pvp, _pvp]),
+    "dab_expand": (_i32, [_vp, _i32, _vp, _vp, _sz, _sz, _vp, _vp, _i32, C.POINTER(_sz), _pvp, _vp]),
     "dab_gemv": (_i32, [_vp, _i32, _i32, _vp, _sz, _sz, _vp, _vp]),
     "dab_spmv": (_i32, [_vp, _i32, _sz, _sz, _vp, _vp, _vp, _vp, _vp]),
     "dab_csc_to_csr": (_i32, [_vp, _i32, _sz, _sz, _sz, _vp, _vp, _vp, _vp, _vp, _vp]),

@@ -13,89 +13,12 @@
 // 2 * elem_bytes) -- read the index, read the element, write the element.  The kernel only moves bytes (NaN payloads, -0.0 intact).
 //
 // Bounds: an index outside [1, length(d)] stores nothing and atomicMin's its position k (0-based, in the block) into *bad_pos.
-#include "dab_common.cuh"
+#include "dab_take_core.cuh"
 
 namespace {
 
 constexpr int TK_THREADS = 256;
 constexpr int TK_ITEMS = 8;                     // indices per thread, all loads issued before the first store
-constexpr int TK_MAXD = 8;
-constexpr int TK_MAX_CHUNKS = 1024;
-// sum over dims of grid[k] + 1: for integers g >= 1, g1 + g2 <= g1 * g2 + 1, so sum(grid) <= prod(grid) + ndim - 1 and the cuts of
-// any grid of at most TK_MAX_CHUNKS chunks fit (1039 for grid (1024, 1, ..., 1) over 8 dims)
-constexpr int TK_MAX_CUTS = TK_MAX_CHUNKS + 2 * TK_MAXD - 1;
-
-struct TakeSrc {
-    unsigned long long dims[TK_MAXD];
-    unsigned long long inv[TK_MAXD];             // floor((2^64 - 1) / dims[k]): division by a multiply-high (tk_divmod)
-    unsigned long long len;                      // prod(dims)
-    int ndim, nchunks, ncuts;
-    int grid[TK_MAXD];
-    int cut_off[TK_MAXD];                        // dim k's grid[k] + 1 cuts start at cuts[cut_off[k]]
-    unsigned long long cuts[TK_MAX_CUTS];        // 0-based first element of each chunk along the dim, then dims[k]
-    const char* chunks[TK_MAX_CHUNKS];           // column-major grid order; NULL for an empty chunk
-};
-static_assert(sizeof(TakeSrc) <= 32764, "kernel parameter block exceeds the 32764-byte limit");
-
-// largest c in [0, n) with cuts[c] <= x (cuts[0] == 0 <= x): skips empty chunks, whose cut equals the next one
-__device__ __forceinline__ int tk_search(const unsigned long long* cuts, int n, unsigned long long x) {
-    int lo = 0;
-    while (n > 1) {
-        const int half = n >> 1;
-        if (cuts[lo + half] <= x) {
-            lo += half;
-            n -= half;
-        } else {
-            n = half;
-        }
-    }
-    return lo;
-}
-
-// q = x / d, x -= q * d, inline (the 64-bit division subroutine would spill around its call).  inv = floor((2^64 - 1) / d)
-// makes x * inv / 2^64 exceed x / d - 1, so the estimate is at most 1 short.
-__device__ __forceinline__ unsigned long long tk_divmod(unsigned long long& x, unsigned long long d, unsigned long long inv) {
-    unsigned long long q = __umul64hi(x, inv);
-    x -= q * d;
-    while (x >= d) {
-        x -= d;
-        ++q;
-    }
-    return q;
-}
-
-// Address of source element g (0-based linear, < len).  ND == false: the 1-D source, no division.
-template <bool ND>
-__device__ __forceinline__ const char* tk_addr(const TakeSrc& s, const unsigned long long* cuts, const char* const* chunks,
-                                               unsigned long long g, int es) {
-    if (!ND) {
-        const int c = tk_search(cuts, s.grid[0], g);
-        return chunks[c] + (size_t)(g - cuts[c]) * es;
-    }
-    unsigned long long rem = g, off = 0, mult = 1;
-    int chunk = 0, cstride = 1;
-#pragma unroll
-    for (int k = 0; k < TK_MAXD; ++k) {
-        if (k < s.ndim) {
-            unsigned long long x = rem;
-            if (k + 1 < s.ndim) rem = tk_divmod(x, s.dims[k], s.inv[k]);
-            const unsigned long long* ck = cuts + s.cut_off[k];
-            const int c = tk_search(ck, s.grid[k], x);
-            off += (x - ck[c]) * mult;
-            mult *= ck[c + 1] - ck[c];
-            chunk += c * cstride;
-            cstride *= s.grid[k];
-        }
-    }
-    return chunks[chunk] + (size_t)off * es;
-}
-
-template <int W> struct Word;
-template <> struct Word<1> { using T = uint8_t; };
-template <> struct Word<2> { using T = uint16_t; };
-template <> struct Word<4> { using T = uint32_t; };
-template <> struct Word<8> { using T = unsigned long long; };
-template <> struct Word<16> { using T = int4; };
 
 // V consecutive elements at a (V * sizeof(U))-aligned address (capped at 16 bytes per store)
 template <typename U, int V>
@@ -214,44 +137,8 @@ int32_t dab_index_gather(dab_ctx* ctx, int32_t elem_bytes, void* out, const void
     DAB_REQUIRE(ctx, (uintptr_t)out % elem_bytes == 0 && (uintptr_t)idx % ib == 0 && (uintptr_t)bad_pos % 8 == 0, DAB_ERR_ARG,
                 "dab_index_gather: misaligned out / idx / bad_pos");
     TakeSrc s;
-    memset(&s, 0, sizeof(s));
-    s.ndim = ndim;
-    s.len = 1;
-    int nchunks = 1, ncuts = 0;
-    for (int k = 0; k < ndim; ++k) {
-        DAB_REQUIRE(ctx, grid[k] >= 1, DAB_ERR_ARG, "dab_index_gather: grid[%d] = %d", k, grid[k]);
-        DAB_REQUIRE(ctx, nchunks <= TK_MAX_CHUNKS / grid[k], DAB_ERR_UNSUPPORTED, "dab_index_gather: more than %d source chunks", TK_MAX_CHUNKS);
-        nchunks *= grid[k];
-        s.dims[k] = dims[k];
-        s.inv[k] = dims[k] ? ~0ull / dims[k] : 0;
-        s.grid[k] = grid[k];
-        s.cut_off[k] = ncuts;
-        DAB_REQUIRE(ctx, ncuts + grid[k] + 1 <= TK_MAX_CUTS, DAB_ERR_UNSUPPORTED, "dab_index_gather: more than %d cuts", TK_MAX_CUTS);
-        const size_t* ck = cuts + ncuts;
-        DAB_REQUIRE(ctx, ck[0] == 0 && ck[grid[k]] == dims[k], DAB_ERR_ARG, "dab_index_gather: cuts of dim %d do not span 0..%zu", k, dims[k]);
-        for (int c = 0; c <= grid[k]; ++c) {
-            DAB_REQUIRE(ctx, c == 0 || ck[c] >= ck[c - 1], DAB_ERR_ARG, "dab_index_gather: cuts of dim %d decrease", k);
-            s.cuts[ncuts + c] = ck[c];
-        }
-        ncuts += grid[k] + 1;
-        DAB_REQUIRE(ctx, dims[k] == 0 || s.len <= ~0ull / dims[k], DAB_ERR_ARG, "dab_index_gather: source length overflows");
-        s.len *= dims[k];
-    }
-    s.nchunks = nchunks;
-    s.ncuts = ncuts;
-    // a non-empty chunk must have a pointer (an empty one is never addressed: the cut search skips it)
-    for (int c = 0; c < nchunks; ++c) {
-        int r = c;
-        bool empty = false;
-        for (int k = 0; k < ndim; ++k) {
-            const int ci = r % grid[k];
-            r /= grid[k];
-            empty = empty || s.cuts[s.cut_off[k] + ci + 1] == s.cuts[s.cut_off[k] + ci];
-        }
-        DAB_REQUIRE(ctx, empty || chunk_ptrs[c], DAB_ERR_ARG, "dab_index_gather: null pointer for non-empty chunk %d", c);
-        DAB_REQUIRE(ctx, (uintptr_t)chunk_ptrs[c] % elem_bytes == 0, DAB_ERR_ARG, "dab_index_gather: chunk %d misaligned", c);
-        s.chunks[c] = (const char*)chunk_ptrs[c];
-    }
+    const int32_t st = tk_fill_src(ctx, "dab_index_gather", ndim, dims, grid, cuts, chunk_ptrs, (size_t)elem_bytes, &s);
+    if (st != DAB_OK) return st;
     switch (elem_bytes) {
         case 1: return take_idx<uint8_t>(ctx, idx_dtype, out, idx, n, s, bad_pos);
         case 4: return take_idx<uint32_t>(ctx, idx_dtype, out, idx, n, s, bad_pos);

@@ -368,6 +368,42 @@ int32_t dab_compact_count(dab_ctx* ctx, const void* mask, size_t run_len, size_t
 int32_t dab_compact(dab_ctx* ctx, int32_t elem_bytes, const void* mask, const void* src, size_t run_len, size_t runs, const int64_t* tile_incl,
                     const int64_t* run_info, int32_t nchunks, const size_t* cuts, void* const* chunk_ptrs);
 
+/* ==== indexed scatter K24 (row f14) =========================================================
+ * d[I[k]] = v[k]: one block of I::DArray{<:Integer} (1-based column-major LINEAR indices into the whole destination d, idx_dtype
+ * DAB_I32 or DAB_I64) per call, the inverse of K22.  The destination is described exactly as dab_index_gather's source (ndim, dims,
+ * grid, cuts, one pointer per chunk, local or a CUDA-IPC peer mapping, at most 1024 chunks); NaN payloads and -0.0 are stored as
+ * bytes.  Julia's setindex! is sequential, so the host runs, over every block of I, first dab_scatter_check, then (when a duplicate
+ * was flagged) dab_scatter_winners, then dab_scatter.  n == 0 launches nothing.  Asynchronous on the ctx stream. */
+/* Bounds and duplicates.  bitmap_ptrs: one zeroed bitmap of ceil(chunk length / 32) uint32 words per chunk of d (same table shape as
+ * chunk_ptrs, 4-byte aligned).  An index outside [1, prod(dims)] atomicMin's its block position into status[0] (initialise it to
+ * ULLONG_MAX); every valid index sets the bit of its element (atomicOr) and, when the bit was set already, sets status[1] to 1
+ * (initialise it to 0).  d itself is not read or written. */
+int32_t dab_scatter_check(dab_ctx* ctx, const void* idx, int32_t idx_dtype, size_t n, int32_t ndim, const size_t* dims, const int32_t* grid,
+                          const size_t* cuts, void* const* bitmap_ptrs, unsigned long long* status);
+/* The last occurrence of every destination: atomicMax of p + 1 into the winner table at the element of idx[k], with p the 0-based
+ * global column-major position of block element k in I: the block is a stack of runs of run_len elements, contiguous in I's global
+ * order, run r starting at run_lin[r] (Int64, device).  win_ptrs: one zeroed table of win_bytes (4, or 8 when length(I) >= 2^32) per
+ * element of each chunk of d.  Out-of-range indices are skipped. */
+int32_t dab_scatter_winners(dab_ctx* ctx, const void* idx, int32_t idx_dtype, size_t n, size_t run_len, const int64_t* run_lin, int32_t win_bytes,
+                            int32_t ndim, const size_t* dims, const int32_t* grid, const size_t* cuts, void* const* win_ptrs);
+/* The stores: the element of idx[k] takes src[k] (src: the block's values, aligned to elem_bytes 1, 4, 8 or 16) or, when src is NULL,
+ * the elem_bytes at the host pointer `scalar`.  win_bytes 0: every valid index stores (the indices are unique); 4 or 8: only the index
+ * whose p + 1 (as in dab_scatter_winners, with the same run table) equals its element's winner entry.  Out-of-range indices store
+ * nothing. */
+int32_t dab_scatter(dab_ctx* ctx, int32_t elem_bytes, const void* idx, int32_t idx_dtype, size_t n, const void* src, const void* scalar,
+                    size_t run_len, const int64_t* run_lin, int32_t win_bytes, int32_t ndim, const size_t* dims, const int32_t* grid,
+                    const size_t* cuts, void* const* chunk_ptrs, void* const* win_ptrs);
+
+/* ==== masked expansion K25 (row f14) =========================================================
+ * d[mask] = v, the inverse of dab_compact on the same tile table and plan (run_len, runs, tile_incl, run_info as there): the element
+ * of the chunk dst at run position i of run r that is the p-th true of its run takes v[run_info[2r] + p], read through the 1-D value
+ * table (nchunks 1..1024, nchunks + 1 cuts, one pointer per chunk, local or a CUDA-IPC peer mapping).  Positions at or past the
+ * values' length are not read.  scalar != NULL: every selected element takes the elem_bytes at the host pointer scalar, and tile_incl,
+ * run_info and the table are not used (NULL allowed).  elem_bytes 1, 4, 8 or 16, moved as bytes.  run_len == 0 or runs == 0 launches
+ * nothing.  Asynchronous on the ctx stream. */
+int32_t dab_expand(dab_ctx* ctx, int32_t elem_bytes, const void* mask, void* dst, size_t run_len, size_t runs, const int64_t* tile_incl,
+                   const int64_t* run_info, int32_t nchunks, const size_t* cuts, const void* const* chunk_ptrs, const void* scalar);
+
 /* ==== Level-2 linear algebra K9 (widening row f4; HBM-bound) ==============================
  * r = op(A) * x on ONE column-major chunk A (m x n, leading dimension m): trans = 0 -> r[m] = A x[n];
  * trans = 1 -> r[n] = A' x[m].  Replaces  localpart(A)*convert(localtype(x), xj)  (src/linalg.jl:95-97)

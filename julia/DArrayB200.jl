@@ -623,6 +623,84 @@ end
 Base.getindex(d::DArray{T,N,B200Array{T,N}}, m::DArray{Bool,N}) where {T,N} = compact(d, m, false)
 Base.findall(m::DArray{Bool,N,B200Array{Bool,N}}) where {N} = compact(m, m, true)   # linear indices, on the devices (DESIGN.md §3.10)
 
+# d[I::DArray{<:Integer}] = v (row f14; Base's setindex! writes one element per remote call): K24, DESIGN.md §3.11.  Unverified, as
+# the K22 / K23 bindings.  Every owner of a chunk of I checks its block against per-chunk bitmaps of d (peer atomics), the host combines
+# the flags (BoundsError before any store), duplicates take a winner table, then every owner stores its block through peer mappings.
+function Base.setindex!(d::DArray{T,N,B200Array{T,N}}, v, I::DArray{<:Integer}) where {T,N}
+    eltype(I) <: Union{Int32,Int64} || throw(ArgumentError("index element type $(eltype(I)) is not served (Int32, Int64)"))
+    v isa Number || filter(!=(1), size(v)) == filter(!=(1), size(I)) || throw(DimensionMismatch("tried to assign $(size(v)) to $(size(I))"))
+    isempty(I) && return d
+    owners = vec(d.pids)
+    lens = [prod(map(length, J)) for J in vec(d.indices)]
+    cuts = reduce(vcat, [cumsum([0; [length(d.indices[ntuple(j -> j == k ? c : 1, N)...][k]) for c in 1:size(d.pids, k)]]) for k in 1:N])
+    tab(n) = Dict(p => remotecall_fetch(() -> (t = B200Array(zeros(Int32, n(lens[c]))); (t, ipc_handle(t))), p) for (c, p) in enumerate(owners))
+    ptrs(h, get) = Ptr{Cvoid}[lens[c] == 0 ? C_NULL : q == myid() ? get(q) : ipc_open(h[q][2]) for (c, q) in enumerate(owners)]
+    dh = Dict(p => remotecall_fetch(() -> ipc_handle(localpart(d)), p) for p in owners)
+    bits = tab(n -> cld(n, 32))
+    vals = v isa Number ? nothing : reshape(collect(v), size(I))
+    sig = (Ptr{Cvoid}, Ptr{Cvoid}, Int32, Csize_t, Int32, Ptr{Csize_t}, Ptr{Int32}, Ptr{Csize_t}, Ptr{Ptr{Cvoid}}, Ptr{Cvoid})
+    flags = asyncmap(procs(I)) do p
+        remotecall_fetch(p) do
+            J = localindices(I)
+            any(isempty, J) && return (nothing, 0)
+            st = B200Array(UInt64[typemax(UInt64), 0])
+            check(ccall((:dab_scatter_check, libdab), Int32, sig, ctx(), localpart(I).ptr, dab_dtype(eltype(I)), length(localpart(I)), N,
+                        Csize_t[size(d)...], Int32[size(d.pids)...], Csize_t[cuts...], ptrs(bits, q -> bits[q][1].ptr), st.ptr), ctx())
+            b, dup = Array(st)
+            (b == typemax(UInt64) ? nothing : LinearIndices(size(I))[CartesianIndex(Tuple(CartesianIndices(map(length, J))[b + 1]) .+ first.(J) .- 1)], dup)
+        end
+    end
+    found = filter(!isnothing, first.(flags))
+    isempty(found) || throw(BoundsError(d, I[minimum(found)]))
+    dup = any(f -> f[2] != 0, flags)
+    length(I) < 2^32 || !dup || throw(ArgumentError("8-byte winner tables are served by the Python host runtime only"))
+    win = dup ? tab(identity) : nothing
+    for phase in (dup ? (:winners, :store) : (:store,))
+        asyncmap(procs(I)) do p
+            remotecall_fetch(p) do
+                J = localindices(I)
+                any(isempty, J) && return nothing
+                lin = B200Array([LinearIndices(size(I))[CartesianIndex(first(J[1]), Tuple(o)...)] - 1
+                                 for o in CartesianIndices(map(length, J[2:end])) .+ CartesianIndex(first.(J[2:end]) .- 1)])
+                wp = dup ? ptrs(win, q -> win[q][1].ptr) : Ptr{Cvoid}[]
+                if phase === :winners
+                    check(ccall((:dab_scatter_winners, libdab), Int32, (Ptr{Cvoid}, Ptr{Cvoid}, Int32, Csize_t, Csize_t, Ptr{Cvoid}, Int32, Int32,
+                                Ptr{Csize_t}, Ptr{Int32}, Ptr{Csize_t}, Ptr{Ptr{Cvoid}}), ctx(), localpart(I).ptr, dab_dtype(eltype(I)),
+                                length(localpart(I)), length(J[1]), lin.ptr, 4, N, Csize_t[size(d)...], Int32[size(d.pids)...], Csize_t[cuts...], wp), ctx())
+                else
+                    blk = vals === nothing ? nothing : B200Array(convert(Array{T}, vals[J...]))
+                    x = Ref{T}(v isa Number ? convert(T, v) : zero(T))
+                    check(ccall((:dab_scatter, libdab), Int32, (Ptr{Cvoid}, Int32, Ptr{Cvoid}, Int32, Csize_t, Ptr{Cvoid}, Ptr{Cvoid}, Csize_t,
+                                Ptr{Cvoid}, Int32, Int32, Ptr{Csize_t}, Ptr{Int32}, Ptr{Csize_t}, Ptr{Ptr{Cvoid}}, Ptr{Ptr{Cvoid}}), ctx(), sizeof(T),
+                                localpart(I).ptr, dab_dtype(eltype(I)), length(localpart(I)), blk === nothing ? C_NULL : blk.ptr, x, length(J[1]),
+                                lin.ptr, dup ? 4 : 0, N, Csize_t[size(d)...], Int32[size(d.pids)...], Csize_t[cuts...],
+                                ptrs(dh, q -> localpart(d).ptr), dup ? wp : C_NULL), ctx())
+                end
+                check(ccall((:dab_sync, libdab), Int32, (Ptr{Cvoid},), ctx()), ctx())   # the peer atomics / stores have landed
+                nothing
+            end
+        end
+    end
+    d
+end
+
+# d[m::DArray{Bool}] .= x (row f14): K25's scalar mode on every localpart of d, no plan.  Unverified.
+function Base.setindex!(d::DArray{T,N,B200Array{T,N}}, x::Number, m::DArray{Bool,N}) where {T,N}
+    size(m) == size(d) || throw(ArgumentError("logical indexing with a DArray{Bool} of other dims is not served"))
+    asyncmap(vec(d.pids)) do p
+        remotecall_fetch(p) do
+            L = localpart(d)
+            isempty(L) && return nothing
+            blk = B200Array(Array(m[localindices(d)...]))                       # the halo read of the mask block, uploaded
+            s = Ref{T}(convert(T, x))
+            check(ccall((:dab_expand, libdab), Int32, (Ptr{Cvoid}, Int32, Ptr{Cvoid}, Ptr{Cvoid}, Csize_t, Csize_t, Ptr{Cvoid}, Ptr{Cvoid}, Int32,
+                        Ptr{Csize_t}, Ptr{Ptr{Cvoid}}, Ptr{Cvoid}), ctx(), sizeof(T), blk.ptr, L.ptr, length(L), 1, C_NULL, C_NULL, 0, C_NULL, C_NULL, s), ctx())
+            nothing
+        end
+    end
+    d
+end
+
 # user code is then unchanged:
 #   d = DArray(I -> B200Array(rand(Float32, map(length, I))), (8 * 2^30,))
 #   d .= 1.5f0 .* d .+ 0.25f0 ;  map!(Affine(2f0, 1f0), d, d) ;  sum(d) ;  maximum(d) ;  sum(d2, dims = 1) ;  A * B ;  A' * x ;  sort(v)
