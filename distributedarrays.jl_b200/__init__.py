@@ -17,6 +17,11 @@ every key ``d[key]`` takes, and ``copyto(view, src)`` (a scatter on the GPU for 
 winning as in Julia's sequential ``setindex!``; ``d[mask] = v`` as the inverse of compaction; a scalar, host array or DArray value); sparse DArrays (``distribute`` of a scipy.sparse matrix: CSC
 localparts, ``nnz``, ``A*x`` / ``A'*x`` / ``mul!``).
 
+Element types: Float32, Float64, Int32, Int64, Bool, ComplexF32, ComplexF64 and Float16 (``np.float16``: storage, data movement,
+elementwise arithmetic with Julia's "widen to Float32, operate, round to Float16" semantics, ``Float16(x)`` inside kernels, and
+reductions with and without ``dims``; GEMM / GEMV, sort, scans, findmax, ``d[I::DArray]`` / ``d[mask]`` / ``filter`` and the
+``d[key] = v`` forms built on them, ``mapslices``, ``ppeval`` and sparse matrices refuse it with ``UnsupportedError``).
+
 Everything computes on the GPU through ``csrc/libdab200.so`` (C ABI: ``include/dab200.h``).  There is no CPU fallback:
 importing works anywhere, but the first op without the built extension or without an H100 raises.
 """
@@ -25,6 +30,7 @@ from ._lib import ArgumentError, DabError, DimensionMismatch, InexactError, Unsu
 from ._broadcast import (Expr, Int128, abs2, broadcast, broadcast_into, ceil, copy, cos, deepcopy, drandn, exp, floor, ifelse, inv, isnan, jl_max, jl_min,
                         log, map_, map_bang, map_inplace, map_localparts, mod, rem, sign, sin, sqrt, tan, tanh, widen)
 from ._broadcast import angle, cis, conj, imag, iszero, real  # noqa: F401 -- complex values (complex(x[, y]) below)
+from ._broadcast import Float16  # noqa: F401 -- Float16(x) inside a kernel
 from ._broadcast import complex_ as complex  # noqa: A004
 from ._broadcast import (acos, acosh, acot, acoth, acsc, acsch, asec, asech, asin, asinh, atan, atanh, cbrt, cosh, cospi, cot, coth, csc,  # noqa: F401
                         csch, deg2rad, erf, erfc, erfcinv, erfcx, erfinv, exp10, exp2, expm1, gamma, isfinite, isinf, log10, log1p, log2,

@@ -32,7 +32,7 @@ from .layout import shape_of
 from .runtime import close_remote_reads, open_remote_reads, runtime
 
 # Julia-type tags and the promotion lattice
-_RANK = {"bool": 0, "i32": 1, "i64": 2, "i128": 3, "f32": 4, "f64": 5}
+_RANK = {"bool": 0, "i32": 1, "i64": 2, "i128": 3, "f16": 4, "f32": 5, "f64": 6}
 
 
 class _TagTypes(dict):
@@ -45,13 +45,20 @@ class _TagTypes(dict):
 
 
 _NPT = _TagTypes({"bool": np.dtype(np.bool_), "i32": np.dtype(np.int32), "i64": np.dtype(np.int64), "f32": np.dtype(np.float32),
-                  "f64": np.dtype(np.float64), "c64": np.dtype(np.complex64), "c128": np.dtype(np.complex128)})
+                  "f64": np.dtype(np.float64), "c64": np.dtype(np.complex64), "c128": np.dtype(np.complex128),
+                  "f16": np.dtype(np.float16)})
 _TAG = {v: k for k, v in _NPT.items()}
 SLICE_TRACING = [0]   # > 0 while mapslices (_slices.py) calls f on the slice tracer
-_CT = {"bool": "bool", "i32": "int", "i64": "long long", "i128": "i128", "f32": "float", "f64": "double", "c64": "jl_c64", "c128": "jl_c128"}
+_CT = {"bool": "bool", "i32": "int", "i64": "long long", "i128": "i128", "f32": "float", "f64": "double", "c64": "jl_c64", "c128": "jl_c128",
+       "f16": "jl_f16"}
 # ComplexF32 / ComplexF64 <-> their component type (``real(T)`` / ``Complex{T}``)
 _COMP = {"c64": "f32", "c128": "f64"}
 _CPLX_OF = {"f32": "c64", "f64": "c128"}
+
+
+def _jl_name(t: str) -> str:
+    """Julia's name of a type tag, for messages."""
+    return {"bool": "Bool", "i32": "Int32", "i64": "Int64", "i128": "Int128", "f16": "Float16", "f32": "Float32", "f64": "Float64"}.get(t, t)
 
 
 def is_ctag(t: str) -> bool:
@@ -74,9 +81,9 @@ def promote(a: str, b: str) -> str:
         if "i128" in (a, b):
             raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "Int128 values mixed with complex values are not served")
         return _CPLX_OF[promote(_COMP.get(a, a), _COMP.get(b, b))]
-    if "f" in a[0] + b[0]:  # any float wins over ints/Bool (Int64 + Float32 -> Float32); Float64 only if one IS Float64
+    if "f" in a[0] + b[0]:  # any float wins over ints/Bool (Int64 + Float32 -> Float32, Int64 + Float16 -> Float16); else the wider float
         fl = [t for t in (a, b) if t[0] == "f"]
-        return "f64" if "f64" in fl else "f32"
+        return "f64" if "f64" in fl else ("f32" if "f32" in fl else "f16")
     return a if _RANK[a] >= _RANK[b] else b
 
 
@@ -108,6 +115,8 @@ class Expr:
             return Expr("const", (), "i64", int(v))  # Julia literal 1 is Int64
         if isinstance(v, np.float32):
             return Expr("const", (), "f32", float(v))
+        if isinstance(v, np.float16):
+            return Expr("const", (), "f16", float(v))   # a Float16 value (Python floats stay Float64 literals)
         if isinstance(v, (float, np.floating)):
             return Expr("const", (), "f64", float(v))  # Julia literal 1.5 is Float64
         from ._sparse import SparseDArray, refuse
@@ -183,6 +192,9 @@ class Expr:
                 r = binop("mul", r, b)
             return r
         pe = Expr.wrap(p)
+        if self.jt == "f16" and pe.jt in ("bool", "i32", "i64"):
+            # ^(x::Float16, n::Integer) = Float16(Float32(x)^n): the Float32 method below, rounded once to Float16
+            return convert(Expr("m_powi", (convert(self, "f32"), convert(pe, "i64")), "f32"), "f16")
         if self.jt == "f32" and pe.jt in ("bool", "i32", "i64"):
             # ^(x::Float32, n::Integer) (base/math.jl): n == -2 and n == 3 in Float32, otherwise power_by_squaring in Float64
             return Expr("m_powi", (self, convert(pe, "i64")), "f32")
@@ -268,7 +280,7 @@ def binop(op: str, a: Expr, b: Expr) -> Expr:
     if op in ("and", "or", "xor") and jt[0] == "f":
         raise TypeError(f"MethodError: no method matching {op}(::Float, ::Float)")
     if op == "idiv" and jt[0] == "f":
-        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "div on floats is not served")
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"div on floats is not served ({_jl_name(jt)} operands)")
     a, b = convert(a, jt), convert(b, jt)
     if op in _CMP:
         return Expr(op, (a, b), "bool")
@@ -321,6 +333,11 @@ def convert(a: Expr, jt: str) -> Expr:
         if a.op == "const" and complex(a.val).imag == 0:
             return convert(Expr("const", (), _COMP[a.jt], complex(a.val).real), jt)
         raise _lib.InexactError(_lib.ERR_UNSUPPORTED, f"InexactError: a {a.jt} value cannot be converted to {jt}")
+    if a.jt == "f16" and a.op != "const":
+        if is_ctag(jt):
+            return convert(convert(a, "f32"), jt)           # Complex{T}(x::Float16) = Complex{T}(Float32(x)): the widening is exact
+        if jt not in ("f32", "f64"):
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"converting Float16 values to {jt} (InexactError semantics) is not served")
     if a.op == "const":
         v = a.val
         if is_ctag(jt):
@@ -330,6 +347,8 @@ def convert(a: Expr, jt: str) -> Expr:
             return Expr("const", (), jt, z)
         if jt == "f32":
             v = float(np.float32(v))
+        elif jt == "f16":
+            v = float(np.float16(v))                            # one rounding from the exact value (Float64 -> Float16 directly)
         elif jt == "f64":
             v = float(v)
         elif jt in ("i32", "i64", "i128"):
@@ -347,12 +366,23 @@ def Int128(x) -> Expr:
 
 
 def widen(x) -> Expr:
-    """Julia's ``widen``: Int32 -> Int64, Int64 -> Int128, Float32 -> Float64."""
+    """Julia's ``widen``: Int32 -> Int64, Int64 -> Int128, Float16 -> Float32, Float32 -> Float64."""
     e = Expr.wrap(x)
-    to = {"bool": "i64", "i32": "i64", "i64": "i128", "f32": "f64"}.get(e.jt)
+    to = {"bool": "i64", "i32": "i64", "i64": "i128", "f16": "f32", "f32": "f64"}.get(e.jt)
     if to is None:
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"widen({e.jt}) is not served")
     return convert(e, to)
+
+
+def Float16(x) -> Expr:
+    """``Float16(x)`` inside a kernel: one rounding to the nearest Float16 (from Float64 directly, never through Float32); integers and Bool
+    convert exactly or overflow to +-Inf; ``Float16(x::Float16)`` is ``x``."""
+    e = Expr.wrap(x)
+    if is_ctag(e.jt):
+        raise _lib.InexactError(_lib.ERR_UNSUPPORTED, f"InexactError: a {e.jt} value cannot be converted to Float16")
+    if e.jt == "i128":
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "Float16 of an Int128 value is not served")
+    return convert(e, "f16")
 
 
 def uses_tag(e: Expr, tag: str) -> bool:
@@ -388,6 +418,8 @@ def cis(x) -> Expr:
     e = _traced(x, "cis")
     if is_ctag(e.jt):
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "cis of a complex value is not served (complex transcendental functions)")
+    if e.jt == "f16":
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "cis of a Float16 value would be a ComplexF16, which is not served")
     e = _float_of(e)
     return Expr("cis", (e,), _CPLX_OF[e.jt])
 
@@ -400,14 +432,16 @@ def complex_(x, y=None) -> Expr:
         if is_ctag(e.jt):
             return e
         if e.jt not in _CPLX_OF:
-            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"complex({e.jt}) would be Complex{{{e.jt}}}: only ComplexF32 / ComplexF64 are served")
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"complex({_jl_name(e.jt)}) would be Complex{{{_jl_name(e.jt)}}}: only ComplexF32 / "
+                                        "ComplexF64 are served")
         return convert(e, _CPLX_OF[e.jt])
     f = Expr.wrap(y)
     if is_ctag(e.jt) or is_ctag(f.jt):
         raise TypeError("MethodError: complex(x, y) takes two real parts")
     jt = promote(e.jt, f.jt)
     if jt not in _CPLX_OF:
-        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"complex of {jt} parts would be Complex{{{jt}}}: only ComplexF32 / ComplexF64 are served")
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"complex of {_jl_name(jt)} parts would be Complex{{{_jl_name(jt)}}}: only ComplexF32 / "
+                                    "ComplexF64 are served")
     return Expr("complex", (convert(e, jt), convert(f, jt)), _CPLX_OF[jt])
 
 
@@ -551,6 +585,8 @@ def _lit(jt: str, v) -> str:
         return "__int_as_float((int)0x%08x)" % struct.unpack("<I", struct.pack("<f", float(v)))[0]
     if jt == "f64":
         return "__longlong_as_double((long long)0x%016xULL)" % struct.unpack("<Q", struct.pack("<d", float(v)))[0]
+    if jt == "f16":
+        return "jl_f16_bits((unsigned short)0x%04x)" % int(np.asarray(v, dtype=np.float16).view(np.uint16))
     if is_ctag(jt):
         z = complex(v)
         return "%s(%s, %s)" % (_CT[jt], _lit(_COMP[jt], z.real), _lit(_COMP[jt], z.imag))
@@ -676,8 +712,9 @@ def run_local(rt, expr: Expr, out: B200Array, largs: List[LocalArg]):
     ctx = rt.ctx
     code = dab_dtype(out.dtype)
     rt.last_kernel = "fixed"
-    # complex trees never take a hand-written real kernel: they all go to the NVRTC kernel
+    # complex and Float16 trees never take a hand-written real kernel: they all go to the NVRTC kernel
     cplx = uses_complex(expr) or builtins_any(is_ctag(a.tag) for a in largs)
+    cplx = cplx or uses_tag(expr, "f16") or builtins_any(a.tag == "f16" for a in largs)
     # ---- hand-written kernels when the tree is one of the fixed shapes
     if same and not cplx and expr.jt == out_tag and out_tag != "bool":
         x0 = largs[0] if largs and largs[0].arr is not None and largs[0].tag == out_tag else None
@@ -971,6 +1008,14 @@ def drandn(dims, procs=None, dist=None, dtype=np.float64, seed: int = 1234, rt=N
         _broadcast_into(out, lambda a, b: complex_(0.7071067811865476 * a, 0.7071067811865476 * b), re, im)
         re.close()
         im.close()
+        return out
+    if dt == np.dtype(np.float16):
+        # randn(Float16) converts the Float64 normal once: Float16(randn(Float64)), from the Float64 stream of the same seed
+        from ._darray import darray_like
+        d64 = drandn(dims, procs, dist, dtype=np.float64, seed=seed, rt=rt)
+        out = darray_like(lambda I: B200Array.empty(d64.rt, shape_of(I), dt), d64, dtype=dt)
+        _broadcast_into(out, Float16, d64)
+        d64.close()
         return out
     if dt.kind != "f":
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"drandn of eltype {dt}")

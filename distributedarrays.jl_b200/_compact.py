@@ -30,7 +30,7 @@ from .runtime import close_remote_reads, open_remote_reads
 MAX_DIMS = 8
 MAX_CHUNKS = 1024          # dab_compact's destination table: the result's chunks travel in the kernel's parameter block
 _SERVED = {np.dtype(t) for t in (np.bool_, np.int32, np.float32, np.int64, np.float64, np.complex64, np.complex128)}
-_JL = {np.dtype(np.bool_): "Bool", np.dtype(np.int32): "Int32", np.dtype(np.int64): "Int64", np.dtype(np.float32): "Float32",
+_JL = {np.dtype(np.float16): "Float16", np.dtype(np.bool_): "Bool", np.dtype(np.int32): "Int32", np.dtype(np.int64): "Int64", np.dtype(np.float32): "Float32",
        np.dtype(np.float64): "Float64", np.dtype(np.complex64): "ComplexF32", np.dtype(np.complex128): "ComplexF64"}
 
 

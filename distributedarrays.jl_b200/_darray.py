@@ -26,9 +26,11 @@ from .runtime import Runtime, close_remote_reads, open_remote_reads, runtime
 
 _DT = {np.dtype(np.float32): _lib.F32, np.dtype(np.float64): _lib.F64, np.dtype(np.int32): _lib.I32,
        np.dtype(np.int64): _lib.I64, np.dtype(np.bool_): _lib.U8,   # UInt8 is NOT Bool: unserved eltypes raise (no silent reinterpretation)
-       np.dtype(np.complex64): _lib.C64, np.dtype(np.complex128): _lib.C128}   # ComplexF32 / ComplexF64, interleaved (re, im)
+       np.dtype(np.complex64): _lib.C64, np.dtype(np.complex128): _lib.C128,   # ComplexF32 / ComplexF64, interleaved (re, im)
+       np.dtype(np.float16): _lib.F16}
 _NP = {_lib.F32: np.dtype(np.float32), _lib.F64: np.dtype(np.float64), _lib.I32: np.dtype(np.int32),
-       _lib.I64: np.dtype(np.int64), _lib.U8: np.dtype(np.bool_), _lib.C64: np.dtype(np.complex64), _lib.C128: np.dtype(np.complex128)}
+       _lib.I64: np.dtype(np.int64), _lib.U8: np.dtype(np.bool_), _lib.C64: np.dtype(np.complex64), _lib.C128: np.dtype(np.complex128),
+       _lib.F16: np.dtype(np.float16)}
 
 
 def dab_dtype(dt) -> int:
@@ -50,6 +52,17 @@ def component_dtype(dt) -> np.dtype:
     """``real(T)``: the element type of each component of a complex type (the type itself for a real one)."""
     dt = np.dtype(dt)
     return {np.dtype(np.complex64): np.dtype(np.float32), np.dtype(np.complex128): np.dtype(np.float64)}.get(dt, dt)
+
+
+def refuse_float16(what: str, *xs):
+    """Float16 DArrays have storage, data movement, elementwise arithmetic and reductions; ``what`` has no Float16 kernel.  Raises
+    ``UnsupportedError`` naming the type when an operand (a DArray, view, transpose, array or scalar) holds Float16 values -- called
+    before anything is allocated or launched."""
+    for x in xs:
+        x = getattr(x, "parent", x) if not hasattr(x, "dtype") else x
+        dt = getattr(x, "dtype", None)
+        if dt is not None and np.dtype(dt) == np.dtype(np.float16):
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what} of Float16 data is not served (no Float16 kernel; no host fallback)")
 
 
 _allowscalar = [True]

@@ -20,7 +20,7 @@ import numpy as np
 
 from . import _lib
 from ._broadcast import broadcast, is_ctag
-from ._darray import B200Array, DArray, dab_dtype, is_complex
+from ._darray import B200Array, DArray, dab_dtype, is_complex, refuse_float16
 from ._mapreduce import _gather_slots, _normalise_region, classify_map, gather_fibres, plan_reducedim
 from .layout import reduction_passes, shape_of
 
@@ -52,6 +52,7 @@ def _findminmax(which: int, f: Optional[Callable], d, dims):
     if isinstance(d, SparseDArray):
         refuse("findmax / findmin / argmax / argmin")
     view = isinstance(d, SubDArray)
+    refuse_float16("findmax / findmin / argmax / argmin", d)
     if is_complex(d.dtype):                          # every check on the view itself: nothing is copied or launched before an error
         _not_ordered(d.dtype)
     mapc, _, expr = classify_map(f, d.dtype)

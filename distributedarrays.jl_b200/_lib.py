@@ -15,6 +15,7 @@ SO_PATH = os.path.join(_HERE, "csrc", "libdab200.so")
 # ---- enums (include/dab200.h) ----------------------------------------------------------------------------
 OK, ERR_CUDA, ERR_ARG, ERR_EMPTY, ERR_DIM_MISMATCH, ERR_NCCL, ERR_UNSUPPORTED, ERR_NVRTC, ERR_NOMEM = range(9)
 F32, F64, I32, I64, U8, I128, C64, C128 = range(8)     # I128: value type of dab_mapreduce_expr only; C64/C128: ComplexF32/F64
+F16 = 8                                                # Float16 (IEEE binary16)
 SUM, PROD, MAX, MIN, ALL, ANY, COUNT, EXTREMA = range(8)
 MAP_ID, MAP_ABS, MAP_ABS2, MAP_NEG, MAP_SQRT, MAP_INV, MAP_FLOOR, MAP_CEIL, MAP_SIGN = range(9)
 MAP_EQ, MAP_NE, MAP_LT, MAP_LE, MAP_GT, MAP_GE, MAP_ISNAN, MAP_NONZERO = range(16, 24)
@@ -96,6 +97,7 @@ _SIGS = {
     "dab_jit_compile_check": (_i32, [C.c_char_p, _i32, _i32, C.POINTER(_i32), C.POINTER(_i32), C.POINTER(_sz)]),
     "dab_mapreduce_expr": (_i32, [_vp, C.c_char_p, _i32, _i32, _sz, _i32, C.POINTER(_i32), _pvp, C.POINTER(_u64), _vp]),
     "dab_jit_compile_check_reduce": (_i32, [C.c_char_p, _i32, _i32, _i32, C.POINTER(_i32), C.POINTER(_i32), C.POINTER(_sz)]),
+    "dab_jit_source": (_i32, [_i32, C.c_char_p, _i32, _i32, _i32, C.POINTER(_i32), C.POINTER(_i32), C.c_char_p, _sz, C.POINTER(_sz)]),
     "dab_reduce": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp, _sz, _vp]),
     "dab_reduce_host": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp, _sz, _vp]),
     "dab_reduce_result_dtype": (_i32, [_i32, _i32, _i32, C.POINTER(_i32)]),

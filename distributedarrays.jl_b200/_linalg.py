@@ -22,7 +22,7 @@ from typing import Dict, List, Optional, Sequence, Tuple, Union
 import numpy as np
 
 from . import _lib
-from ._darray import B200Array, DArray, SubDArray, dab_dtype, darray
+from ._darray import refuse_float16, B200Array, DArray, SubDArray, dab_dtype, darray
 from ._sparse import SparseDArray, refuse
 from .layout import make_layout, rlen, shape_of
 from .runtime import Runtime, close_remote_reads, deliver, exchange_stacks, grouped_exchange, open_remote_reads
@@ -180,6 +180,7 @@ def mul_(y: DArray, A: Union[DArray, Transpose], x, alpha=1, beta=0) -> DArray:
     ``Transpose``/``Adjoint`` wrapper, :120-167.  Error contract as the reference: DimensionMismatch when the contracted sizes
     differ, ArgumentError when y's cuts do not match the matrix cuts along the kept dim."""
     _refuse_complex("mul!", y, A, x)
+    refuse_float16("mul!", y, A, x)
     M, trans = _unwrap(A)
     if isinstance(y, SparseDArray):
         refuse("mul! into it")
@@ -266,6 +267,7 @@ def matmul(A: Union[DArray, Transpose], x) -> DArray:
         from ._slices import matmul_of_slices
         return matmul_of_slices(A, x)
     _refuse_complex("A*x", A, x)
+    refuse_float16("A*x", A, x)
     M, trans = _unwrap(A)
     xnd = len(x.dims) if isinstance(x, DArray) else np.ndim(x)
     if xnd == 2:
@@ -340,6 +342,7 @@ def mul_mat_(Cd: DArray, A: Union[DArray, Transpose], B, alpha=1, beta=0) -> DAr
     src/linalg.jl:189-261).  Same errors as the reference: DimensionMismatch for the contracted / result sizes, ArgumentError when the
     cuts of C's first dimension differ from A's."""
     _refuse_complex("mul!", Cd, A, B)
+    refuse_float16("mul!", Cd, A, B)
     M, trans = _unwrap(A)
     _refuse_sparse_matmat(M)
     if isinstance(Cd, SparseDArray) or isinstance(B, SparseDArray):
@@ -432,6 +435,7 @@ def matmat(A: Union[DArray, Transpose], B) -> DArray:
     ``(size(procs(A),2), that min)``.  The reference asks ``procs(B)`` for its grid, so B is a DMatrix there; a host matrix is accepted
     here as a one-column grid (what ``distribute`` of a matrix no wider than tall gives on these workers)."""
     _refuse_complex("A*B", A, B)
+    refuse_float16("A*B", A, B)
     M, trans = _unwrap(A)
     _refuse_sparse_matmat(M)
     if M.ndim != 2:
@@ -462,6 +466,7 @@ def lmul_diag(d, DA: DArray) -> DArray:
     """``lmul!(D::Diagonal, DA::DMatrix)`` with ``d = D.diag`` (reference src/linalg.jl:169-177): DA[i,j] = d[i]*DA[i,j]."""
     from ._broadcast import broadcast_into
     _refuse_complex("lmul!(Diagonal, A)", d, DA)
+    refuse_float16("lmul!(Diagonal, A)", d, DA)
     dv = np.asarray(d)
     if DA.ndim != 2 or dv.shape != (DA.dims[0],):
         raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, f"lmul!: diagonal of length {dv.shape} vs matrix {DA.dims}")
@@ -472,6 +477,7 @@ def rmul_diag(DA: DArray, d) -> DArray:
     """``rmul!(DA::DMatrix, D::Diagonal)`` (reference src/linalg.jl:179-187): DA[i,j] = DA[i,j]*d[j]."""
     from ._broadcast import broadcast_into
     _refuse_complex("rmul!(A, Diagonal)", DA, d)
+    refuse_float16("rmul!(A, Diagonal)", DA, d)
     dv = np.asarray(d)
     if DA.ndim != 2 or dv.shape != (DA.dims[1],):
         raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, f"rmul!: diagonal of length {dv.shape} vs matrix {DA.dims}")

@@ -73,7 +73,7 @@ def classify_map(f: Optional[Callable], dtype) -> Tuple[Optional[int], Optional[
             x's type the comparison is equivalent in that type, and the predicate kernel can run on the raw chunk."""
             if side.op == "convert" and side.args[0].op == "arg" and side.args[0].jt == tag and const.op == "const":
                 c = const.val
-                if tag == "f32" and const.jt == "f64" and float(np.float32(c)) == c:
+                if tag in ("f32", "f16") and const.jt == "f64" and float(_NPT[tag].type(c)) == c:
                     return side.args[0], Expr("const", (), tag, c)
                 if tag in ("i32", "i64") and const.jt in ("i64",) and side.jt == "i64":
                     return side.args[0], Expr("const", (), tag, c) if -2**31 <= c < 2**31 or tag == "i64" else (side, const)
@@ -423,7 +423,7 @@ def extrema(d: DArray):
             tmp.close()
     if is_complex(d.dtype):
         raise TypeError(f"MethodError: no method matching isless(::{d.dtype}, ::{d.dtype}) -- complex numbers are not ordered")
-    if d.dtype == np.dtype(np.bool_):
+    if d.dtype in (np.dtype(np.bool_), np.dtype(np.float16)):
         return (_mapreduce_all(None, _lib.MIN, d), _mapreduce_all(None, _lib.MAX, d))
     _check_nonempty(d, _lib.MAX)
     rt, code, es = d.rt, dab_dtype(d.dtype), d.dtype.itemsize
@@ -734,6 +734,8 @@ def mean(d: DArray, dims=None, f: Optional[Callable] = None):
     out_t = np.float64 if S.dtype.kind in "iub" or S.dtype == np.float64 else np.float32
     if is_complex(S.dtype):
         out_t = component_dtype(S.dtype).type                                # Complex{T} ./ n: each component divided in T
+    if S.dtype == np.dtype(np.float16):
+        out_t = np.float16                                                    # Float16 ./ Int is Float16 (Int promotes to Float16)
     c = out_t(cnt)
     R = broadcast(lambda s: s / c, S)
     S.close()

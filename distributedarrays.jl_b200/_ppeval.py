@@ -163,6 +163,8 @@ def ppeval(f, *D, dim=None) -> DArray:
     for i, x in enumerate(D):
         if isinstance(x, SubDArray):
             raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "ppeval of a view: make it a DArray first (DArray(view))")
+        if (x.dtype if isinstance(x, DArray) else np.asarray(x).dtype) == np.dtype(np.float16):
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"ppeval with a Float16 argument ({i + 1}) is not served (no Float16 slice kernels)")
         if (x.dtype if isinstance(x, DArray) else np.asarray(x).dtype).kind == "c":
             raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"ppeval with a complex argument ({i + 1}) is not served (no complex slice kernels)")
         if isinstance(x, DArray):

@@ -401,7 +401,10 @@ def copyto_view(dest: SubDArray, src):
 
 def setindex(d: DArray, key, v):
     """``DArray.__setitem__``: dispatch on the key as ``__getitem__`` does."""
+    from ._darray import refuse_float16
     from ._sparse import SparseDArray
+    if isinstance(key, (DArray, SparseDArray)):
+        refuse_float16("d[key] = v with a DArray key (the scatter and expansion have no 2-byte instances)", d)
     if isinstance(key, DArray) and key.dtype == np.bool_ and key.dims == d.dims:
         return setindex_mask(d, key, v)
     if isinstance(key, (DArray, SparseDArray)):

@@ -421,6 +421,8 @@ def mapslices(f, D: DArray, dims) -> DArray:
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "mapslices of a view: make it a DArray first (DArray(view))")
     if D.dtype.kind == "c":
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"mapslices of a {D.dtype} DArray is not served (no complex slice kernels)")
+    from ._darray import refuse_float16
+    refuse_float16("mapslices", D)
     N = D.ndim
     dims = normalise_dims(dims, N)
     if N > 8:

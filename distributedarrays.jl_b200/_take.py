@@ -46,6 +46,8 @@ def _check(d, I):
     from ._sparse import SparseDArray, refuse
     if isinstance(d, SparseDArray) or isinstance(I, SparseDArray):
         refuse("indexing by a DArray")
+    from ._darray import refuse_float16
+    refuse_float16("d[I] with a DArray index (the index gather has no 2-byte instance)", d)
     T = np.dtype(I.dtype)
     if T == np.bool_:
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "logical indexing with a DArray{Bool} is not served (its values are not positions)")

@@ -248,7 +248,8 @@ int32_t dab_mapreduce_all(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, 
         if (op == DAB_EXTREMA) return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_mapreduce_all: extrema combines through dab_reduce + dab_allgather");
         return dab_fail(ctx, DAB_ERR_ARG, "bad dtype/op");
     }
-    const bool cplx = rdt == DAB_C64 || rdt == DAB_C128;  // 8- / 16-byte complex results: ordered fold below, not the mailbox combine
+    // 8- / 16-byte complex and 2-byte Float16 results: ordered fold below, not the mailbox combine (which folds the arithmetic types)
+    const bool cplx = rdt == DAB_C64 || rdt == DAB_C128 || rdt == DAB_F16;
     if ((ctx->mbox_ranks > 1 || !ctx->comm || ctx->nranks == 1) && n > 0 && !cplx) {
         // fused path: ONE kernel = chunk reduce + peer-memory all-gather + ordered fold + scalar into pinned host memory
         ctx->fuse_op = op;
@@ -265,8 +266,8 @@ int32_t dab_mapreduce_all(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, 
     }
     if (cplx && ctx->mbox_ranks > 1 && !ctx->comm) {
         DAB_FLUSH(ctx);
-        return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_mapreduce_all: a complex result across %d ranks needs the NCCL communicator "
-                        "(the mailbox combine carries 8-byte results)", ctx->mbox_ranks);
+        return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_mapreduce_all: a %s result across %d ranks needs the NCCL communicator "
+                        "(the mailbox combine folds Float32 / Float64 / integer results)", rdt == DAB_F16 ? "Float16" : "complex", ctx->mbox_ranks);
     }
     int32_t st = dab_reduce(ctx, dtype, op, map, map_param, x, n, ctx->result_slot);
     if (st != DAB_OK) return st;

@@ -133,6 +133,7 @@ static inline size_t dab_dtype_size(int32_t dt) {
         case DAB_U8: return 1;
         case DAB_C64: return 8;
         case DAB_C128: return 16;
+        case DAB_F16: return 2;
         default: return 0;
     }
 }
@@ -170,6 +171,71 @@ template <typename T>
 struct alignas(2 * sizeof(T)) Cplx {
     T re, im;
 };
+
+// Float16 element: the IEEE binary16 bits.  Conversions are single PTX cvt instructions: widening is exact, narrowing rounds once to
+// nearest even (from Float64 directly, never through Float32) and overflows to +-Inf.
+struct alignas(2) Half {
+    unsigned short bits;
+    Half() = default;
+    __device__ __forceinline__ explicit Half(float v) { asm("cvt.rn.f16.f32 %0, %1;" : "=h"(bits) : "f"(v)); }
+    __device__ __forceinline__ explicit Half(double v) { asm("cvt.rn.f16.f64 %0, %1;" : "=h"(bits) : "d"(v)); }
+    __device__ __forceinline__ explicit Half(int v) : Half((float)v) {}  // 0 / 1 of the ALL / ANY finalisation
+    __device__ __forceinline__ explicit operator float() const {
+        float f;
+        asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"(bits));
+        return f;
+    }
+    __device__ __forceinline__ explicit operator double() const {
+        double d;
+        asm("cvt.f64.f16 %0, %1;" : "=d"(d) : "h"(bits));
+        return d;
+    }
+};
+// Host-side Float16 <-> Float32 on the same bit representation (dab_combine_ordered's fold): widening is exact (a NaN keeps its payload);
+// narrowing rounds to nearest even, overflows to +-Inf at 65520 and keeps the top payload bits of a NaN (quieted).
+static inline float dab_half_to_float(unsigned short h) {
+    const uint32_t sign = (uint32_t)(h & 0x8000) << 16, e = (h >> 10) & 0x1f, m = h & 0x3ff;
+    uint32_t x;
+    if (e == 0x1f) x = sign | 0x7f800000u | (m << 13);
+    else if (e) x = sign | ((e + 112) << 23) | (m << 13);
+    else {
+        const float v = (float)m * 5.9604644775390625e-08f;  // m * 2^-24, exact
+        memcpy(&x, &v, 4);
+        x |= sign;
+    }
+    float f;
+    memcpy(&f, &x, 4);
+    return f;
+}
+static inline unsigned short dab_float_to_half(float f) {
+    uint32_t x;
+    memcpy(&x, &f, 4);
+    const uint32_t sign = (x >> 16) & 0x8000, ax = x & 0x7fffffffu;
+    if (ax > 0x7f800000u) return (unsigned short)(sign | 0x7e00 | ((ax >> 13) & 0x3ff));
+    if (ax >= 0x477ff000u) return (unsigned short)(sign | 0x7c00);  // |f| >= 65520 (and Inf)
+    uint32_t q, rem, half;
+    if (ax < 0x38800000u) {                                          // below 2^-14: a subnormal Float16 (or zero)
+        const uint32_t e = ax >> 23;
+        if (e < 102) return (unsigned short)sign;                    // below 2^-25
+        const uint32_t m = (ax & 0x7fffffu) | 0x800000u, shift = 126 - e;
+        q = m >> shift;
+        rem = m & ((1u << shift) - 1);
+        half = 1u << (shift - 1);
+    } else {
+        const uint32_t r = ax - 0x38000000u;                         // rebias the exponent from 127 to 15
+        q = r >> 13;
+        rem = r & 0x1fff;
+        half = 0x1000;
+    }
+    if (rem > half || (rem == half && (q & 1))) ++q;
+    return (unsigned short)(sign | q);
+}
+// evict-first scalar load of a Float16 element (the strided dims kernels read single elements)
+__device__ __forceinline__ Half __ldcs(const Half* p) {
+    Half h;
+    h.bits = __ldcs(reinterpret_cast<const unsigned short*>(p));
+    return h;
+}
 
 template <typename T>
 __device__ __forceinline__ Pack<T> as_pack(int4 r) {

@@ -493,6 +493,14 @@ struct RandGen {
     }
 };
 
+// Julia's rand(Float16): 10 random bits k, the value k * 2^-10 (exact in Float16)
+struct RandGenF16 {
+    uint64_t seed, off;
+    __device__ __forceinline__ Half operator()(size_t i) const {
+        return Half((float)(dab_hash_u32(seed, off + i) >> 22) * 0.0009765625f);  // 2^-10
+    }
+};
+
 template <typename T, typename Gen>
 static int32_t launch_generate(dab_ctx* ctx, T* x, size_t n, Gen gen) {
     if (n == 0) return DAB_OK;
@@ -516,6 +524,12 @@ int32_t dab_fill(dab_ctx* ctx, int32_t dtype, void* x, size_t n, const void* val
         case DAB_I32: return launch_generate(ctx, (int32_t*)x, n, FillGen<int32_t>{*(const int32_t*)value});
         case DAB_I64: return launch_generate(ctx, (long long*)x, n, FillGen<long long>{*(const long long*)value});
         case DAB_U8: return launch_generate(ctx, (uint8_t*)x, n, FillGen<uint8_t>{*(const uint8_t*)value});
+        case DAB_F16: {
+            DAB_REQUIRE(ctx, (uintptr_t)x % 2 == 0, DAB_ERR_ARG, "dab_fill: Float16 data needs 2-byte alignment");
+            FillGen<Half> g;
+            memcpy(&g.v, value, 2);
+            return launch_generate(ctx, (Half*)x, n, g);
+        }
         case DAB_C64:
         case DAB_C128: {  // interleaved (re, im): one element is 8 / 16 bytes, stored with the same 16-byte vectors
             const size_t es = dab_dtype_size(dtype);
@@ -539,7 +553,10 @@ int32_t dab_rand_u01(dab_ctx* ctx, int32_t dtype, void* x, size_t n, uint64_t se
     switch (dtype) {
         case DAB_F32: return launch_generate(ctx, (float*)x, n, RandGen<float>{seed, global_offset});
         case DAB_F64: return launch_generate(ctx, (double*)x, n, RandGen<double>{seed, global_offset});
-        default: return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_rand_u01: dtype %d (F32/F64 only)", dtype);
+        case DAB_F16:
+            DAB_REQUIRE(ctx, (uintptr_t)x % 2 == 0, DAB_ERR_ARG, "dab_rand_u01: Float16 data needs 2-byte alignment");
+            return launch_generate(ctx, (Half*)x, n, RandGenF16{seed, global_offset});
+        default: return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_rand_u01: dtype %d (F32/F64/F16 only)", dtype);
     }
 }
 

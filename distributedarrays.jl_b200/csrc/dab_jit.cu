@@ -364,6 +364,98 @@ DEV jl_c64 jl_cis(float x) { return jl_c64(cosf(x), sinf(x)); }
 DEV jl_c128 jl_cis(double x) { return jl_c128(cos(x), sin(x)); }
 )PRELUDE";
 
+// Float16 values (jl_f16: the IEEE binary16 bits).  Julia defines Float16 arithmetic as "widen to Float32, operate, round to Float16"
+// (base/float.jl); for + - * / and sqrt that IS the correctly rounded binary16 result (24 >= 2*11 + 2).  Math functions are
+// Float16(f(Float32(x))), as Julia's Float16 methods.  Conversions are single PTX cvt instructions: Float64 -> Float16 rounds once
+// (never through Float32); Int32 / Int64 values go through an exact or already-overflowing Float32.  Appended only to sources that use
+// the type (an argument, output or value dtype, or the name in the expression), so every other generated kernel is byte-for-byte what it
+// was; no toolkit header is needed.
+const char* kPreludeF16 = R"PRELUDE(
+struct __align__(2) jl_f16 {
+    unsigned short b;
+    jl_f16() = default;
+    DEV jl_f16(float x) { asm("cvt.rn.f16.f32 %0, %1;" : "=h"(b) : "f"(x)); }
+    DEV jl_f16(double x) { asm("cvt.rn.f16.f64 %0, %1;" : "=h"(b) : "d"(x)); }
+    DEV jl_f16(int x) : jl_f16((float)x) {}   // exact below 2^24; larger values overflow to +-Inf either way
+    DEV jl_f16(i64 x) : jl_f16((float)x) {}
+    DEV jl_f16(bool x) : b(x ? 0x3c00 : 0) {}
+    // Float32(x) / Float64(x): exact; a NaN keeps its sign and payload bits (the cvt instruction would return the canonical NaN)
+    DEV explicit operator float() const {
+        float f;
+        asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"(b));
+        return (b & 0x7fff) > 0x7c00 ? __int_as_float(((unsigned)(b & 0x8000) << 16) | 0x7f800000u | ((unsigned)(b & 0x3ff) << 13)) : f;
+    }
+    DEV explicit operator double() const {
+        double d;
+        asm("cvt.f64.f16 %0, %1;" : "=d"(d) : "h"(b));
+        return (b & 0x7fff) > 0x7c00 ? __longlong_as_double(((i64)(b & 0x8000) << 48) | 0x7ff0000000000000ll | ((i64)(b & 0x3ff) << 42)) : d;
+    }
+};
+DEV jl_f16 jl_f16_bits(unsigned short b) { jl_f16 r; r.b = b; return r; }
+// the operand of an arithmetic operation (its NaN results are canonical anyway)
+DEV float jl_w(jl_f16 a) { float f; asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"(a.b)); return f; }
+DEV jl_f16 jl_add(jl_f16 a, jl_f16 b) { return jl_f16(__fadd_rn(jl_w(a), jl_w(b))); }
+DEV jl_f16 jl_sub(jl_f16 a, jl_f16 b) { return jl_f16(__fsub_rn(jl_w(a), jl_w(b))); }
+DEV jl_f16 jl_mul(jl_f16 a, jl_f16 b) { return jl_f16(__fmul_rn(jl_w(a), jl_w(b))); }
+DEV jl_f16 jl_div(jl_f16 a, jl_f16 b) { return jl_f16(__fdiv_rn(jl_w(a), jl_w(b))); }
+DEV jl_f16 jl_max(jl_f16 a, jl_f16 b) { return jl_f16(jl_max(jl_w(a), jl_w(b))); }
+DEV jl_f16 jl_min(jl_f16 a, jl_f16 b) { return jl_f16(jl_min(jl_w(a), jl_w(b))); }
+DEV jl_f16 jl_rem(jl_f16 a, jl_f16 b) { return jl_f16(jl_rem(jl_w(a), jl_w(b))); }
+DEV jl_f16 jl_mod(jl_f16 a, jl_f16 b) { return jl_f16(jl_mod(jl_w(a), jl_w(b))); }
+DEV jl_f16 jl_pow(jl_f16 a, jl_f16 b) { return jl_f16(powf(jl_w(a), jl_w(b))); }
+DEV bool jl_lt(jl_f16 a, jl_f16 b) { return jl_w(a) < jl_w(b); }
+DEV bool jl_le(jl_f16 a, jl_f16 b) { return jl_w(a) <= jl_w(b); }
+DEV bool jl_gt(jl_f16 a, jl_f16 b) { return jl_w(a) > jl_w(b); }
+DEV bool jl_ge(jl_f16 a, jl_f16 b) { return jl_w(a) >= jl_w(b); }
+DEV bool jl_eq(jl_f16 a, jl_f16 b) { return jl_w(a) == jl_w(b); }
+DEV bool jl_ne(jl_f16 a, jl_f16 b) { return jl_w(a) != jl_w(b); }
+DEV jl_f16 jl_neg(jl_f16 a) { return jl_f16_bits(a.b ^ 0x8000); }
+DEV jl_f16 jl_abs(jl_f16 a) { return jl_f16_bits(a.b & 0x7fff); }
+DEV jl_f16 jl_sqrt(jl_f16 a) { return jl_f16(__fsqrt_rn(jl_w(a))); }
+DEV jl_f16 jl_inv(jl_f16 a) { return jl_f16(__fdiv_rn(1.0f, jl_w(a))); }
+DEV jl_f16 jl_floor(jl_f16 a) { return jl_f16(floorf(jl_w(a))); }
+DEV jl_f16 jl_ceil(jl_f16 a) { return jl_f16(ceilf(jl_w(a))); }
+DEV jl_f16 jl_sign(jl_f16 a) { return jl_f16(jl_sign(jl_w(a))); }
+DEV bool jl_isnan(jl_f16 a) { return (a.b & 0x7fff) > 0x7c00; }
+DEV bool jl_isinf(jl_f16 a) { return (a.b & 0x7fff) == 0x7c00; }
+DEV bool jl_isfinite(jl_f16 a) { return (a.b & 0x7c00) != 0x7c00; }
+#define JL_H1(name) DEV jl_f16 jl_##name(jl_f16 a) { return jl_f16(jl_##name(jl_w(a))); }
+JL_H1(sin) JL_H1(cos) JL_H1(tan) JL_H1(exp) JL_H1(exp2) JL_H1(log) JL_H1(log2) JL_H1(log10) JL_H1(tanh) JL_H1(sinh) JL_H1(cosh)
+JL_H1(atan) JL_H1(asin) JL_H1(acos) JL_H1(expm1) JL_H1(log1p) JL_H1(cbrt)
+DEV jl_f16 jl_angle(jl_f16 a) { return jl_f16(atan2f(0.f, jl_w(a))); }   // angle(x::Real) = atan(zero(x), x)
+)PRELUDE";
+
+// The Float16 methods of kPreludeExt's and kPreludeMethods' names, appended after those blocks when a source uses both.
+const char* kPreludeF16Ext = R"PRELUDE(
+JL_H1(x_asinh) JL_H1(x_acosh) JL_H1(x_atanh) JL_H1(x_exp10) JL_H1(x_sinpi) JL_H1(x_cospi) JL_H1(x_trunc) JL_H1(x_round)
+JL_H1(x_erf) JL_H1(x_erfc) JL_H1(x_erfinv) JL_H1(x_erfcinv) JL_H1(x_erfcx) JL_H1(x_gamma) JL_H1(x_loggamma)
+)PRELUDE";
+const char* kPreludeF16Methods = R"PRELUDE(
+DEV jl_f16 jl_m_copysign(jl_f16 a, jl_f16 b) { return jl_f16_bits((a.b & 0x7fff) | (b.b & 0x8000)); }
+)PRELUDE";
+
+bool uses_f16(const char* expr, int32_t dt0, int nargs, const int32_t* dts) {
+    if (dt0 == DAB_F16) return true;
+    for (int k = 0; k < nargs; ++k)
+        if (dts[k] == DAB_F16) return true;
+    return expr && strstr(expr, "jl_f16") != nullptr;
+}
+
+// the Float16 block and its companions for the blocks already in s
+void append_f16(std::string& s, const char* expr) {
+    s += kPreludeF16;
+    if (mentions_ext(expr)) s += kPreludeF16Ext;
+    if (mentions_methods(expr)) s += kPreludeF16Methods;
+}
+
+// elements per thread step of the linear kernel: 8 when an array argument or the output is Float16 (16-byte accesses), else 4
+int lin_width(int32_t out_dt, int nargs, const int32_t* dts) {
+    if (out_dt == DAB_F16) return 8;
+    for (int k = 0; k < nargs; ++k)
+        if (dts[k] == DAB_F16) return 8;
+    return 4;
+}
+
 bool is_cplx_dt(int32_t dt) { return dt == DAB_C64 || dt == DAB_C128; }
 
 bool uses_cplx(const char* expr, int32_t dt0, int nargs, const int32_t* dts) {
@@ -385,6 +477,7 @@ const char* ctype_of(int32_t dt) {
         case DAB_U8: return "bool";
         case DAB_C64: return "jl_c64";
         case DAB_C128: return "jl_c128";
+        case DAB_F16: return "jl_f16";
         default: return nullptr;
     }
 }
@@ -494,6 +587,8 @@ std::string build_source(const char* expr, int32_t out_dt, int nargs, const int3
     if (mentions_ext(expr)) s += kPreludeExt;
     if (mentions_methods(expr)) s += kPreludeMethods;
     if (uses_cplx(expr, out_dt, nargs, dts)) s += kPreludeCplx;
+    if (uses_f16(expr, out_dt, nargs, dts)) append_f16(s, expr);
+    const std::string W = std::to_string(lin_width(out_dt, nargs, dts));   // "4" except in Float16 kernels
     s += "typedef ";
     s += ctype_of(out_dt);
     s += " OUT_T;\n";
@@ -501,11 +596,11 @@ std::string build_source(const char* expr, int32_t out_dt, int nargs, const int3
     s += "#define DAB_EXPR (";
     s += expr;
     s += ")\n";
-    // ---- linear kernel: flat grid, one CTA per 2 x 256 vectors of 4 elements (same shape as ew1_kernel, which beat
+    // ---- linear kernel: flat grid, one CTA per 2 x 256 vectors of W elements (4; 8 in Float16 kernels) (same shape as ew1_kernel, which beat
     // the persistent grid-stride form); the extra last CTA takes the remainder vectors and the scalar tail
     s += "extern \"C\" __global__ void __launch_bounds__(256) dab_bc_linear(BcParams p) {\n"
          "  const u64 n = p.shape[0] * p.shape[1] * p.shape[2] * p.shape[3];\n"
-         "  const u64 nv = n / 4;\n"
+         "  const u64 nv = n / " + W + ";\n"
          "  const u64 ntiles = nv / 512;\n"
          "  OUT_T* o = (OUT_T*)p.out;\n";
     for (int k = 0; k < nargs; ++k) {
@@ -518,14 +613,14 @@ std::string build_source(const char* expr, int32_t out_dt, int nargs, const int3
     for (int k = 0; k < nargs; ++k)
         if (is_arr[k]) {
             std::string K = std::to_string(k);
-            s += "    const VecN<T" + K + ", 4> v" + K + "_0 = *(const VecN<T" + K + ", 4>*)(q" + K + " + 4 * i0);\n";
-            s += "    const VecN<T" + K + ", 4> v" + K + "_1 = *(const VecN<T" + K + ", 4>*)(q" + K + " + 4 * (i0 + 256));\n";
+            s += "    const VecN<T" + K + ", " + W + "> v" + K + "_0 = *(const VecN<T" + K + ", " + W + ">*)(q" + K + " + " + W + " * i0);\n";
+            s += "    const VecN<T" + K + ", " + W + "> v" + K + "_1 = *(const VecN<T" + K + ", " + W + ">*)(q" + K + " + " + W + " * (i0 + 256));\n";
         }
     for (int u = 0; u < 2; ++u) {
         std::string U = std::to_string(u);
-        s += "    { VecN<OUT_T, 4> r;\n"
+        s += "    { VecN<OUT_T, " + W + "> r;\n"
              "#pragma unroll\n"
-             "      for (int j = 0; j < 4; ++j) {\n";
+             "      for (int j = 0; j < " + W + "; ++j) {\n";
         for (int k = 0; k < nargs; ++k)
             if (is_arr[k]) {
                 std::string K = std::to_string(k);
@@ -533,7 +628,7 @@ std::string build_source(const char* expr, int32_t out_dt, int nargs, const int3
             }
         s += "        r.v[j] = (OUT_T)DAB_EXPR;\n"
              "      }\n"
-             "      *(VecN<OUT_T, 4>*)(o + 4 * (i0 + " + std::to_string(256 * u) + ")) = r; }\n";
+             "      *(VecN<OUT_T, " + W + ">*)(o + " + W + " * (i0 + " + std::to_string(256 * u) + ")) = r; }\n";
     }
     s += "    return;\n"
          "  }\n"
@@ -541,11 +636,11 @@ std::string build_source(const char* expr, int32_t out_dt, int nargs, const int3
     for (int k = 0; k < nargs; ++k)
         if (is_arr[k]) {
             std::string K = std::to_string(k);
-            s += "    const VecN<T" + K + ", 4> v" + K + " = *(const VecN<T" + K + ", 4>*)(q" + K + " + 4 * i);\n";
+            s += "    const VecN<T" + K + ", " + W + "> v" + K + " = *(const VecN<T" + K + ", " + W + ">*)(q" + K + " + " + W + " * i);\n";
         }
-    s += "    VecN<OUT_T, 4> r;\n"
+    s += "    VecN<OUT_T, " + W + "> r;\n"
          "#pragma unroll\n"
-         "    for (int j = 0; j < 4; ++j) {\n";
+         "    for (int j = 0; j < " + W + "; ++j) {\n";
     for (int k = 0; k < nargs; ++k)
         if (is_arr[k]) {
             std::string K = std::to_string(k);
@@ -553,9 +648,9 @@ std::string build_source(const char* expr, int32_t out_dt, int nargs, const int3
         }
     s += "      r.v[j] = (OUT_T)DAB_EXPR;\n"
          "    }\n"
-         "    *(VecN<OUT_T, 4>*)(o + 4 * i) = r;\n"
+         "    *(VecN<OUT_T, " + W + ">*)(o + " + W + " * i) = r;\n"
          "  }\n"
-         "  for (u64 i = nv * 4 + threadIdx.x; i < n; i += blockDim.x) {\n";
+         "  for (u64 i = nv * " + W + " + threadIdx.x; i < n; i += blockDim.x) {\n";
     for (int k = 0; k < nargs; ++k)
         if (is_arr[k]) {
             std::string K = std::to_string(k);
@@ -699,6 +794,15 @@ bool mr_spec(int32_t val_dt, int32_t op, MrSpec* sp) {
             default: return false;
         }
     }
+    if (val_dt == DAB_F16) {  // Float16 values: Float32 tile (exact widening), fp64 carrier, one rounding to Float16 (the slot's first 2 bytes)
+        switch (op) {
+            case DAB_SUM: *sp = {"float", "double", vt, "jl_add(a, b)", "jl_add(a, b)", "0.0"}; return true;
+            case DAB_PROD: *sp = {"float", "double", vt, "jl_mul(a, b)", "jl_mul(a, b)", "1.0"}; return true;
+            case DAB_MAX: *sp = {"float", "float", vt, "jl_max(a, b)", "jl_max(a, b)", "(-__int_as_float(0x7f800000))"}; return true;
+            case DAB_MIN: *sp = {"float", "float", vt, "jl_min(a, b)", "jl_min(a, b)", "__int_as_float(0x7f800000)"}; return true;
+            default: return false;
+        }
+    }
     if (is_cplx_dt(val_dt)) {  // complex fp64 carrier; sums add componentwise in the value type inside a tile, products widen first
         const char* out = val_dt == DAB_C64 ? "jl_c64_slot" : "jl_c128";
         switch (op) {
@@ -761,6 +865,7 @@ std::string build_mr_source(const char* expr, int32_t val_dt, int32_t op, int na
     if (mentions_ext(expr)) s += kPreludeExt;
     if (mentions_methods(expr)) s += kPreludeMethods;
     if (uses_cplx(expr, val_dt, nargs, dts)) s += kPreludeCplx;
+    if (uses_f16(expr, val_dt, nargs, dts)) append_f16(s, expr);
     if (val_dt == DAB_I128 || is_cplx_dt(val_dt)) s += "#define DAB_ACC16 1\n";   // 16-byte carrier: shuffles and the result slot move four words
     s += std::string("typedef ") + vtype_of(val_dt) + " VAL_T;\n";
     for (int k = 0; k < nargs; ++k) s += std::string("typedef ") + ctype_of(dts[k]) + " T" + std::to_string(k) + ";\n";
@@ -835,10 +940,12 @@ extern "C" __global__ void __launch_bounds__(256) dab_mr_final(MrFinal p) {
     }
 }
 )MR";
-    // ---- partial kernel
+    // ---- partial kernel: tiles of 2 x 256 vectors of W elements (4; 8 in Float16 kernels, 16-byte accesses)
+    const int wi = lin_width(DAB_F32, nargs, dts);
+    const std::string W = std::to_string(wi), W2 = std::to_string(2 * wi), WT = std::to_string(512 * wi);
     s += "extern \"C\" __global__ void __launch_bounds__(256) dab_mr_partial(MrParams p) {\n"
          "  __shared__ ACC_T smem[8];\n"
-         "  const u64 n = p.n, nv = n / 4, ntiles = nv / 512;\n";
+         "  const u64 n = p.n, nv = n / " + W + ", ntiles = nv / 512;\n";
     for (int k = 0; k < nargs; ++k) {
         std::string K = std::to_string(k);
         if (is_arr[k]) s += "  const T" + K + "* q" + K + " = (const T" + K + "*)p.ptr[" + K + "];\n";
@@ -853,28 +960,28 @@ extern "C" __global__ void __launch_bounds__(256) dab_mr_final(MrFinal p) {
     for (int k = 0; k < nargs; ++k)
         if (is_arr[k]) {
             std::string K = std::to_string(k);
-            s += "    const VecN<T" + K + ", 4> v" + K + "_0 = *(const VecN<T" + K + ", 4>*)(q" + K + " + 4 * i0);\n";
-            s += "    const VecN<T" + K + ", 4> v" + K + "_1 = *(const VecN<T" + K + ", 4>*)(q" + K + " + 4 * (i0 + 256));\n";
+            s += "    const VecN<T" + K + ", " + W + "> v" + K + "_0 = *(const VecN<T" + K + ", " + W + ">*)(q" + K + " + " + W + " * i0);\n";
+            s += "    const VecN<T" + K + ", " + W + "> v" + K + "_1 = *(const VecN<T" + K + ", " + W + ">*)(q" + K + " + " + W + " * (i0 + 256));\n";
         }
-    s += "    TILE_T m[8];\n";
+    s += "    TILE_T m[" + W2 + "];\n";
     for (int u = 0; u < 2; ++u) {
         std::string U = std::to_string(u);
-        s += "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n";
+        s += "#pragma unroll\n    for (int j = 0; j < " + W + "; ++j) {\n";
         for (int k = 0; k < nargs; ++k)
             if (is_arr[k]) {
                 std::string K = std::to_string(k);
                 s += "      const T" + K + " a" + K + " = v" + K + "_" + U + ".v[j];\n";
             }
-        s += "      m[" + std::to_string(4 * u) + " + j] = (TILE_T)((VAL_T)DAB_EXPR);\n    }\n";
+        s += "      m[" + std::to_string(wi * u) + " + j] = (TILE_T)((VAL_T)DAB_EXPR);\n    }\n";
     }
     s += "#pragma unroll\n"
-         "    for (int w = 8; w > 1; w >>= 1)\n"
+         "    for (int w = " + W2 + "; w > 1; w >>= 1)\n"
          "#pragma unroll\n"
          "      for (int k = 0; k < w / 2; ++k) m[k] = tile_comb(m[k], m[k + w / 2]);\n"
          "    acc = acc_comb(acc, (ACC_T)m[0]);\n"
          "  }\n"
          "  if (blockIdx.x == gridDim.x - 1) {\n"
-         "    for (u64 i = ntiles * 2048 + threadIdx.x; i < n; i += blockDim.x) {\n";
+         "    for (u64 i = ntiles * " + WT + " + threadIdx.x; i < n; i += blockDim.x) {\n";
     for (int k = 0; k < nargs; ++k)
         if (is_arr[k]) {
             std::string K = std::to_string(k);
@@ -963,7 +1070,8 @@ int32_t dab_broadcast_expr(dab_ctx* ctx, const char* expr, int32_t out_dtype, vo
     bool linear = true;
     for (int d = 0; d < 4; ++d)
         if (shape[d] > 1 && out_strides[d] != dense[d]) linear = false;
-    if ((uintptr_t)out % (4 * dab_dtype_size(out_dtype))) linear = false;
+    const size_t lw = (size_t)lin_width(out_dtype, nargs, arg_dtypes);   // elements per vector of the linear kernel
+    if ((uintptr_t)out % (lw * dab_dtype_size(out_dtype))) linear = false;
     for (int k = 0; k < nargs; ++k) {
         p.ptr[k] = arg_ptrs[k];
         p.scalar[k] = arg_scalars[k];
@@ -971,7 +1079,7 @@ int32_t dab_broadcast_expr(dab_ctx* ctx, const char* expr, int32_t out_dtype, vo
             p.str[k][d] = (long long)arg_strides[4 * k + d];
             if (is_arr[k] && shape[d] > 1 && arg_strides[4 * k + d] != dense[d]) linear = false;
         }
-        if (is_arr[k] && ((uintptr_t)arg_ptrs[k] % (4 * dab_dtype_size(arg_dtypes[k])))) linear = false;
+        if (is_arr[k] && ((uintptr_t)arg_ptrs[k] % (lw * dab_dtype_size(arg_dtypes[k])))) linear = false;
     }
     // rows kernel: dense destination, 4 | shape[0], every array argument dense-along-dim-0 with 4-element-aligned rows, or extruded
     bool rows = !linear && shape[0] % 4 == 0 && out_strides[0] == 1 && ((uintptr_t)out % (4 * dab_dtype_size(out_dtype))) == 0;
@@ -988,7 +1096,7 @@ int32_t dab_broadcast_expr(dab_ctx* ctx, const char* expr, int32_t out_dtype, vo
     void* args[] = {&p};
     CUfunction fn = linear ? comp.linear : (rows ? comp.rows : comp.general);
     size_t work = rows ? (n / 4 + 255) / 256 : (n + 255) / 256;
-    size_t grid = linear ? (n / 4) / 512 + 1 : (size_t)dab_grid_for(ctx, work, rows ? comp.occ_rows : comp.occ_general);
+    size_t grid = linear ? (n / lw) / 512 + 1 : (size_t)dab_grid_for(ctx, work, rows ? comp.occ_rows : comp.occ_general);
     if (grid > 0x7fffffffull) return dab_fail(ctx, DAB_ERR_ARG, "array too large for one launch");
     CUresult cr = drv.LaunchKernel(fn, (unsigned)grid, 1, 1, 256, 1, 1, 0, (CUstream)ctx->stream, args, nullptr);
     if (cr != CUDA_SUCCESS) {
@@ -1019,9 +1127,11 @@ int32_t dab_mapreduce_expr(dab_ctx* ctx, const char* expr, int32_t val_dtype, in
         is_arr[k] = arg_ptrs[k] != nullptr;
         DAB_REQUIRE(ctx, is_arr[k] || arg_dtypes[k] != DAB_C128, DAB_ERR_ARG, "dab_mapreduce_expr: a ComplexF64 scalar does not fit the 8-byte scalar slot of arg %d (pass complex(re, im) of two Float64 scalars)", k);
         key += std::to_string(arg_dtypes[k]) + (is_arr[k] ? "a" : "s");
-        if (is_arr[k] && ((uintptr_t)arg_ptrs[k] % (4 * dab_dtype_size(arg_dtypes[k])))) vec_ok = false;
     }
-    if (!vec_ok) return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_mapreduce_expr: arguments must be aligned to 4 elements");
+    const size_t lw = (size_t)lin_width(DAB_F32, nargs, arg_dtypes);   // elements per vector of the partial kernel (8 with Float16 arguments)
+    for (int k = 0; k < nargs; ++k)
+        if (is_arr[k] && ((uintptr_t)arg_ptrs[k] % (lw * dab_dtype_size(arg_dtypes[k])))) vec_ok = false;
+    if (!vec_ok) return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_mapreduce_expr: arguments must be aligned to %d elements", (int)lw);
     key += "|";
     key += expr;
     CompiledMr comp;
@@ -1046,7 +1156,7 @@ int32_t dab_mapreduce_expr(dab_ctx* ctx, const char* expr, int32_t val_dtype, in
             comp = it->second;
         }
     }
-    const size_t ntiles = (n / 4) / 512;
+    const size_t ntiles = (n / lw) / 512;
     size_t k = 2;
     const size_t max_parts = 16384;
     if ((ntiles + k - 1) / k > max_parts) k = (ntiles + max_parts - 1) / max_parts;
@@ -1074,6 +1184,32 @@ int32_t dab_mapreduce_expr(dab_ctx* ctx, const char* expr, int32_t val_dtype, in
         drv.LaunchKernel(comp.final_, 1, 1, 1, 256, 1, 1, 0, (CUstream)ctx->stream, a2, nullptr) != CUDA_SUCCESS)
         return dab_fail(ctx, DAB_ERR_CUDA, "cuLaunchKernel failed (dab_mapreduce_expr)");
     ctx->launches += 2;
+    return DAB_OK;
+}
+
+// Diagnostic (no GPU, no NVRTC): the generated source itself -- kind 0 the broadcast kernels of dab_broadcast_expr (dtype = output type),
+// kind 1 the fused map + reduce kernels of dab_mapreduce_expr (dtype = value type, op).  Copies at most cap bytes to buf and the full
+// length to *len; lets the tests pin the sources of existing expressions byte for byte.
+int32_t dab_jit_source(int32_t kind, const char* expr, int32_t dtype, int32_t op, int32_t nargs, const int32_t* arg_dtypes,
+                       const int32_t* arg_is_array, char* buf, size_t cap, size_t* len) {
+    if (!expr || !len || nargs < 0 || nargs > 8 || (nargs && (!arg_dtypes || !arg_is_array)) || (kind != 0 && kind != 1))
+        return dab_fail(nullptr, DAB_ERR_ARG, "dab_jit_source: bad argument");
+    bool is_arr[8] = {false};
+    for (int k = 0; k < nargs; ++k) {
+        if (!ctype_of(arg_dtypes[k])) return dab_fail(nullptr, DAB_ERR_ARG, "dab_jit_source: bad dtype of arg %d", k);
+        is_arr[k] = arg_is_array[k] != 0;
+    }
+    std::string src;
+    if (kind == 0) {
+        if (!ctype_of(dtype)) return dab_fail(nullptr, DAB_ERR_ARG, "dab_jit_source: bad out dtype %d", dtype);
+        src = build_source(expr, dtype, nargs, arg_dtypes, is_arr);
+    } else {
+        MrSpec sp;
+        if (!vtype_of(dtype) || !mr_spec(dtype, op, &sp)) return dab_fail(nullptr, DAB_ERR_UNSUPPORTED, "op %d on value dtype %d not served", op, dtype);
+        src = build_mr_source(expr, dtype, op, nargs, arg_dtypes, is_arr, sp);
+    }
+    *len = src.size();
+    if (buf && cap) memcpy(buf, src.data(), src.size() < cap ? src.size() : cap);
     return DAB_OK;
 }
 

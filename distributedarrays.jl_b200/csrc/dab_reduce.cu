@@ -349,6 +349,55 @@ int32_t reduce_c(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, const Cpl
                     dtype);
 }
 
+// Float16 chunks: the same kernel with Half elements (a 16-byte load carries 8), each value widened to Float32 by the map (HMapF); Float16
+// results for SUM / PROD / MAX / MIN (extrema of Float16 data is a MIN and a MAX reduction on the host side).
+template <int FN>
+int32_t reduce_h_arith(dab_ctx* ctx, int32_t op, const Half* x, size_t n, void* out) {
+    using M = HMapF<FN>;
+    const M map{};
+    switch (op) {
+        case DAB_SUM: return launch_reduce<Half, M, SumTraits<float>, Half>(ctx, x, n, map, out, 0);
+        case DAB_PROD: return launch_reduce<Half, M, ProdTraits<float>, Half>(ctx, x, n, map, out, 0);
+        case DAB_MAX: return launch_reduce<Half, M, MaxTraits<float>, Half>(ctx, x, n, map, out, 0);
+        case DAB_MIN: return launch_reduce<Half, M, MinTraits<float>, Half>(ctx, x, n, map, out, 0);
+        case DAB_EXTREMA: return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_reduce: EXTREMA is not served for Float16 (a MIN and a MAX reduction are)");
+        default: return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "reduce op %d needs a predicate map (no host fallback)", op);
+    }
+}
+
+template <int FN>
+int32_t reduce_h_pred(dab_ctx* ctx, int32_t op, const Half* x, size_t n, const void* param, void* out) {
+    HPredF<FN> map;
+    map.p.bits = 0;
+    if (param) memcpy(&map.p, param, 2);
+    const int mode = op == DAB_ALL ? 1 : (op == DAB_ANY ? 2 : 0);
+    if (op != DAB_ALL && op != DAB_ANY && op != DAB_COUNT && op != DAB_SUM)
+        return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "reduce op %d on a predicate map (no host fallback)", op);
+    return launch_reduce<Half, HPredF<FN>, CountTraits, long long>(ctx, x, n, map, out, mode);
+}
+
+int32_t reduce_h(dab_ctx* ctx, int32_t op, int32_t map, const void* param, const Half* x, size_t n, void* out) {
+    if ((uintptr_t)x % 2) return dab_fail(ctx, DAB_ERR_ARG, "dab_reduce: Float16 data needs 2-byte alignment");
+    switch (map) {
+        case DAB_MAP_ID: return reduce_h_arith<DAB_MAP_ID>(ctx, op, x, n, out);
+        case DAB_MAP_ABS: return reduce_h_arith<DAB_MAP_ABS>(ctx, op, x, n, out);
+        case DAB_MAP_ABS2: return reduce_h_arith<DAB_MAP_ABS2>(ctx, op, x, n, out);
+        case DAB_MAP_NEG: return reduce_h_arith<DAB_MAP_NEG>(ctx, op, x, n, out);
+#define P(FN) \
+    case FN: return reduce_h_pred<FN>(ctx, op, x, n, param, out)
+            P(DAB_MAP_EQ);
+            P(DAB_MAP_NE);
+            P(DAB_MAP_LT);
+            P(DAB_MAP_LE);
+            P(DAB_MAP_GT);
+            P(DAB_MAP_GE);
+            P(DAB_MAP_ISNAN);
+            P(DAB_MAP_NONZERO);
+#undef P
+        default: return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "map %d not served by a reduce kernel for Float16 (no host fallback)", map);
+    }
+}
+
 // The deferred dab_affine y .= a.*x .+ b and the reduction of y as ONE kernel: reads x, writes y, reduces y (8 B/element of
 // Float32 instead of 8 + 4).  Same CTA geometry, element-to-thread mapping and fold as reduce_arith<T, DAB_MAP_ID> on y.
 template <typename T>
@@ -404,6 +453,9 @@ int32_t empty_result(dab_ctx* ctx, int32_t dtype, int32_t op, void* out_dev) {
             } else if (dtype == DAB_F64) {
                 double one = 1.0;
                 memcpy(buf, &one, 8);
+            } else if (dtype == DAB_F16) {
+                const unsigned short one = 0x3c00;
+                memcpy(buf, &one, 2);
             } else if (dtype == DAB_C64) {
                 const float one[2] = {1.f, 0.f};
                 memcpy(buf, one, 8);
@@ -414,7 +466,7 @@ int32_t empty_result(dab_ctx* ctx, int32_t dtype, int32_t op, void* out_dev) {
                 long long one = 1;
                 memcpy(buf, &one, 8);
             }
-            if (flt) {
+            if (flt || dtype == DAB_F16) {
                 double one = 1.0;
                 memcpy(buf + 8, &one, 8);
             }
@@ -448,7 +500,7 @@ int32_t dab_reduce_result_dtype(int32_t dtype, int32_t op, int32_t map, int32_t*
     switch (op) {
         case DAB_SUM:
         case DAB_PROD:
-            *out_dtype = (!pred && (dtype == DAB_F32 || dtype == DAB_F64)) ? dtype : DAB_I64;
+            *out_dtype = (!pred && (dtype == DAB_F32 || dtype == DAB_F64 || dtype == DAB_F16)) ? dtype : DAB_I64;
             return DAB_OK;
         case DAB_MAX:
         case DAB_MIN:
@@ -494,6 +546,7 @@ int32_t dab_reduce(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, const v
         case DAB_I32: return reduce_t<int32_t>(ctx, op, map, map_param, (const int32_t*)x, n, out_dev);
         case DAB_I64: return reduce_t<long long>(ctx, op, map, map_param, (const long long*)x, n, out_dev);
         case DAB_U8: return reduce_u8(ctx, op, map, (const uint8_t*)x, n, out_dev);
+        case DAB_F16: return reduce_h(ctx, op, map, map_param, (const Half*)x, n, out_dev);
         default: return dab_fail(ctx, DAB_ERR_ARG, "dab_reduce: bad dtype %d", dtype);
     }
 }
@@ -598,6 +651,25 @@ int32_t dab_combine_ordered(int32_t rdt, int32_t op, const void* partials, size_
                 default: break;
             }
             break;
+        case DAB_F16: {  // Float16 arithmetic: each operation widened to Float32 and rounded back to Float16, as Julia's Float16 methods
+            const unsigned short* v = (const unsigned short*)partials;
+            float a = dab_half_to_float(v[0]);
+            for (size_t i = 1; i < p; ++i) {
+                const float b = dab_half_to_float(v[i]);
+                volatile float r;
+                switch (op) {
+                    case DAB_SUM: r = a + b; break;
+                    case DAB_PROD: r = a * b; break;
+                    case DAB_MAX: r = fmax_jl(a, b); break;
+                    case DAB_MIN: r = fmin_jl(a, b); break;
+                    default: return dab_fail(nullptr, DAB_ERR_UNSUPPORTED, "dab_combine_ordered: dtype %d (Float16) op %d", rdt, op);
+                }
+                a = dab_half_to_float(dab_float_to_half(r));
+            }
+            const unsigned short h = dab_float_to_half(a);
+            memcpy(out, &h, 2);
+            return DAB_OK;
+        }
         case DAB_C64:
             if (op == DAB_SUM || op == DAB_PROD) {  // Float32 arithmetic, each operation rounded (volatile: no wider intermediates)
                 const float* v = (const float*)partials;

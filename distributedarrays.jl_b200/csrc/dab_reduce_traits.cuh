@@ -350,5 +350,27 @@ struct CPredF {  // Complex{T} -> Bool: !iszero(z), isnan(z)
     }
 };
 
+// ---- Float16 element type: Half ------------------------------------------------------------------------------------------------------
+// Each value is widened to Float32 (exact) as it leaves the 16-byte vector; the map, the tile tree and the traits then work in Float32
+// (SumTraits<float> etc.: fp32 inside a tile step, fp64 carrier), and the result is rounded once to Float16.  abs2 rounds x*x to
+// Float16 first, as Julia's Float16 * does.
+template <int FN>
+struct HMapF {
+    using V = float;
+    Half p;
+    __device__ __forceinline__ V operator()(Half h) const {
+        const float x = (float)h;
+        if constexpr (FN == DAB_MAP_ABS) return fabsf(x);
+        else if constexpr (FN == DAB_MAP_ABS2) return (float)Half(jl::mul(x, x));   // x*x is exact in Float32: one rounding
+        else if constexpr (FN == DAB_MAP_NEG) return -x;
+        else return x;
+    }
+};
+template <int FN>
+struct HPredF {  // Float16 -> Bool, compared in Float32 (exact for Float16 operands)
+    using V = int;
+    Half p;
+    __device__ __forceinline__ V operator()(Half h) const { return PredF<float, FN>{(float)p}((float)h); }
+};
 
 }  // namespace

@@ -415,6 +415,21 @@ __global__ void scalar_into_kernel(const Out* __restrict__ slot, Out* __restrict
     *out = v;
 }
 
+// Float16 result of a full reduction in disguise (see dab_reducedim); accumulate folds in Float16 arithmetic (Float32, rounded back)
+__global__ void half_into_kernel(const Half* __restrict__ slot, Half* __restrict__ out, int accumulate, int op) {
+    Half v = *slot;
+    if (accumulate) {
+        const float o = (float)*out, w = (float)v;
+        switch (op) {
+            case DAB_SUM: v = Half(jl::add(o, w)); break;
+            case DAB_PROD: v = Half(jl::mul(o, w)); break;
+            case DAB_MAX: v = Half(jl::max(o, w)); break;
+            default: v = Half(jl::min(o, w)); break;
+        }
+    }
+    *out = v;
+}
+
 template <typename T>
 using ResultOfSum = typename std::conditional<std::is_floating_point<T>::value, T, long long>::type;
 
@@ -440,6 +455,31 @@ int32_t rdim_t(dab_ctx* ctx, int32_t op, int32_t map, const T* x, size_t inner, 
         case DAB_MAP_ABS2: return rdim_map<T, DAB_MAP_ABS2>(ctx, op, x, inner, red, outer, out, accumulate);
         case DAB_MAP_NEG: return rdim_map<T, DAB_MAP_NEG>(ctx, op, x, inner, red, outer, out, accumulate);
         default: return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_reducedim: map %d not served (no host fallback)", map);
+    }
+}
+
+// Float16 chunks: Half elements widened to Float32 by the map (HMapF), Float32 / fp64 traits as for Float32, Float16 output
+template <int FN>
+int32_t rdim_h_map(dab_ctx* ctx, int32_t op, const Half* x, size_t inner, size_t red, size_t outer, void* out, int accumulate) {
+    using M = HMapF<FN>;
+    const M map{};
+    Half* o = (Half*)out;
+    switch (op) {
+        case DAB_SUM: return launch_rdim<Half, M, SumTraits<float>, Half>(ctx, x, inner, red, outer, map, o, accumulate);
+        case DAB_PROD: return launch_rdim<Half, M, ProdTraits<float>, Half>(ctx, x, inner, red, outer, map, o, accumulate);
+        case DAB_MAX: return launch_rdim<Half, M, MaxTraits<float>, Half>(ctx, x, inner, red, outer, map, o, accumulate);
+        case DAB_MIN: return launch_rdim<Half, M, MinTraits<float>, Half>(ctx, x, inner, red, outer, map, o, accumulate);
+        default: return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_reducedim: op %d not served for Float16 (no host fallback)", op);
+    }
+}
+
+int32_t rdim_h(dab_ctx* ctx, int32_t op, int32_t map, const Half* x, size_t inner, size_t red, size_t outer, void* out, int accumulate) {
+    switch (map) {
+        case DAB_MAP_ID: return rdim_h_map<DAB_MAP_ID>(ctx, op, x, inner, red, outer, out, accumulate);
+        case DAB_MAP_ABS: return rdim_h_map<DAB_MAP_ABS>(ctx, op, x, inner, red, outer, out, accumulate);
+        case DAB_MAP_ABS2: return rdim_h_map<DAB_MAP_ABS2>(ctx, op, x, inner, red, outer, out, accumulate);
+        case DAB_MAP_NEG: return rdim_h_map<DAB_MAP_NEG>(ctx, op, x, inner, red, outer, out, accumulate);
+        default: return dab_fail(ctx, DAB_ERR_UNSUPPORTED, "dab_reducedim: map %d not served for Float16 (no host fallback)", map);
     }
 }
 
@@ -471,6 +511,7 @@ int32_t dab_reducedim(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, cons
         if (op == DAB_PROD) {
             if (rdt == DAB_F32) { float o = 1.f; memcpy(v, &o, 4); }
             else if (rdt == DAB_F64) { double o = 1.0; memcpy(v, &o, 8); }
+            else if (rdt == DAB_F16) { const unsigned short o = 0x3c00; memcpy(v, &o, 2); }
             else { long long o = 1; memcpy(v, &o, 8); }
         }
         return dab_fill(ctx, rdt, out, nout, v);
@@ -486,6 +527,7 @@ int32_t dab_reducedim(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, cons
             case DAB_F32: scalar_into_kernel<float><<<1, 1, 0, ctx->stream>>>((const float*)ctx->result_slot, (float*)out, accumulate, op); break;
             case DAB_F64: scalar_into_kernel<double><<<1, 1, 0, ctx->stream>>>((const double*)ctx->result_slot, (double*)out, accumulate, op); break;
             case DAB_I32: scalar_into_kernel<int32_t><<<1, 1, 0, ctx->stream>>>((const int32_t*)ctx->result_slot, (int32_t*)out, accumulate, op); break;
+            case DAB_F16: half_into_kernel<<<1, 1, 0, ctx->stream>>>((const Half*)ctx->result_slot, (Half*)out, accumulate, op); break;
             default: scalar_into_kernel<long long><<<1, 1, 0, ctx->stream>>>((const long long*)ctx->result_slot, (long long*)out, accumulate, op); break;
         }
         DAB_LAUNCHED(ctx);
@@ -496,6 +538,9 @@ int32_t dab_reducedim(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, cons
         case DAB_F64: return rdim_t<double>(ctx, op, map, (const double*)x, inner, reduce, outer, out, accumulate);
         case DAB_I32: return rdim_t<int32_t>(ctx, op, map, (const int32_t*)x, inner, reduce, outer, out, accumulate);
         case DAB_I64: return rdim_t<long long>(ctx, op, map, (const long long*)x, inner, reduce, outer, out, accumulate);
+        case DAB_F16:
+            DAB_REQUIRE(ctx, (uintptr_t)x % 2 == 0 && (uintptr_t)out % 2 == 0, DAB_ERR_ARG, "dab_reducedim: Float16 data needs 2-byte alignment");
+            return rdim_h(ctx, op, map, (const Half*)x, inner, reduce, outer, out, accumulate);
         default: return dab_fail(ctx, DAB_ERR_ARG, "dab_reducedim: bad dtype %d", dtype);
     }
 }

@@ -67,7 +67,7 @@ enum {
 enum { DAB_F32 = 0, DAB_F64 = 1, DAB_I32 = 2, DAB_I64 = 3, DAB_U8 = 4 /* Bool */,
        DAB_I128 = 5 /* Int128: ONLY as the value type of dab_mapreduce_expr (f widens, e.g. x -> Int128(x)^2; test/darray.jl:286-294);
                        there are no arrays of it.  Its result fills the whole 16-byte slot (two's complement, little endian). */,
-       DAB_C64 = 6 /* ComplexF32 */, DAB_C128 = 7 /* ComplexF64 */ };
+       DAB_C64 = 6 /* ComplexF32 */, DAB_C128 = 7 /* ComplexF64 */, DAB_F16 = 8 /* Float16 (IEEE binary16) */ };
 /* Complex element types are stored interleaved (re, im), as Julia's Complex{T}.  Entry points that accept them:
  *   dab_fill, dab_reduce / dab_reduce_host / dab_mapreduce_all / dab_reduce_result_dtype / dab_combine_ordered (see there),
  *   dab_broadcast_expr / dab_mapreduce_expr and their compile checks (argument, output and value types), dab_adjoint_box, and the
@@ -76,6 +76,18 @@ enum { DAB_F32 = 0, DAB_F64 = 1, DAB_I32 = 2, DAB_I64 = 3, DAB_U8 = 4 /* Bool */
  * complex + is componentwise); any other op or map returns DAB_ERR_UNSUPPORTED naming the dtype.  drand of a complex array calls
  * dab_rand_u01 on the real view of 2n components at global offset 2g.  Every other entry point returns DAB_ERR_UNSUPPORTED (or
  * DAB_ERR_ARG) for them, naming the dtype. */
+/* Float16 (DAB_F16, 2 bytes) is accepted by:
+ *   dab_fill (2-byte value), dab_rand_u01 (element g = (hash32(seed, g) >> 22) * 2^-10, Julia's rand(Float16)),
+ *   dab_reduce / dab_reduce_host / dab_mapreduce_all / dab_reduce_result_dtype / dab_combine_ordered: SUM / PROD / MAX / MIN with
+ *     MAP_ID, MAP_ABS, MAP_ABS2, MAP_NEG (Float16 result: fp32 over each tile step, fp64 carrier, one rounding to Float16 at the end;
+ *     MAX / MIN exact), and COUNT / ANY / ALL / SUM with the predicate maps (Int64); EXTREMA returns DAB_ERR_UNSUPPORTED (extrema of
+ *     Float16 data is a MIN and a MAX reduction).  dab_mapreduce_all folds Float16 results through dab_reduce + allgather + dab_combine_ordered.
+ *   dab_reducedim: SUM / PROD / MAX / MIN with MAP_ID, MAP_ABS, MAP_ABS2, MAP_NEG, Float16 output.
+ *   dab_broadcast_expr / dab_mapreduce_expr and their compile checks (argument, output and value types: "widen to Float32, operate,
+ *     round to Float16" per operation, as Julia's Float16 methods),
+ *   the byte movers with 2-byte elements (dab_copy_box, dab_gather_box, dab_transpose_box, dab_h2d, ...).
+ * Every other entry point returns DAB_ERR_UNSUPPORTED (or DAB_ERR_ARG) for it, naming the dtype; the index-gather, compaction, expansion
+ * and scatter kernels (dab_index_gather, dab_compact, dab_expand, dab_scatter) have no 2-byte instances. */
 
 /* ---- reduce operators  (op argument of Base.mapreduce; src/mapreduce.jl:31) ----------- */
 enum {
@@ -218,6 +230,10 @@ int32_t dab_mapreduce_expr(dab_ctx* ctx, const char* expr, int32_t val_dtype, in
                            const void* const* arg_ptrs, const uint64_t* arg_scalars, void* out_dev);
 int32_t dab_jit_compile_check_reduce(const char* expr, int32_t val_dtype, int32_t op, int32_t nargs, const int32_t* arg_dtypes,
                                      const int32_t* arg_is_array, size_t* cubin_bytes);
+/* Diagnostic (no GPU, no NVRTC): the generated CUDA source -- kind 0 dab_broadcast_expr's kernels (dtype = output type), kind 1
+ * dab_mapreduce_expr's (dtype = value type, op).  At most cap bytes go to buf, the full length to *len. */
+int32_t dab_jit_source(int32_t kind, const char* expr, int32_t dtype, int32_t op, int32_t nargs, const int32_t* arg_dtypes,
+                       const int32_t* arg_is_array, char* buf, size_t cap, size_t* len);
 
 /* ==== whole-chunk reductions K4 / K7 (HBM-bound, 4 B/element) ==========================
  * Replace mapreduce(f, op, localpart(d)) / reduce(f, localpart(d)) run per worker at

@@ -64,6 +64,7 @@ end
 dab_dtype(::Type{Float32}) = Int32(0); dab_dtype(::Type{Float64}) = Int32(1)
 dab_dtype(::Type{Int32}) = Int32(2);   dab_dtype(::Type{Int64}) = Int32(3); dab_dtype(::Type{Bool}) = Int32(4)
 dab_dtype(::Type{ComplexF32}) = Int32(6); dab_dtype(::Type{ComplexF64}) = Int32(7)   # interleaved (re, im), Julia's own layout
+dab_dtype(::Type{Float16}) = Int32(8)   # IEEE binary16
 
 # ---- the chunk type ------------------------------------------------------------------------------------------------------------
 mutable struct B200Array{T,N} <: AbstractArray{T,N}
@@ -139,8 +140,10 @@ const FN1 = Dict{Any,String}((-) => "jl_neg", abs => "jl_abs", abs2 => "jl_abs2"
                              ceil => "jl_ceil", sign => "jl_sign", sin => "jl_sin", cos => "jl_cos", tan => "jl_tan", exp => "jl_exp",
                              log => "jl_log", tanh => "jl_tanh", isnan => "jl_isnan", identity => "")
 ctype(::Type{Float32}) = "float"; ctype(::Type{Float64}) = "double"; ctype(::Type{Int32}) = "int"; ctype(::Type{Int64}) = "long long"; ctype(::Type{Bool}) = "bool"
+ctype(::Type{Float16}) = "jl_f16"   # the NVRTC prelude's Float16 (widen to Float32, operate, round to Float16)
 literal(x::Float32) = "__int_as_float((int)0x$(string(reinterpret(UInt32, x), base = 16)))"
 literal(x::Float64) = "__longlong_as_double((long long)0x$(string(reinterpret(UInt64, x), base = 16))ULL)"
+literal(x::Float16) = "jl_f16_bits((unsigned short)0x$(string(reinterpret(UInt16, x), base = 16)))"
 literal(x::Integer) = "(($(ctype(typeof(x))))$(x))"
 literal(x::Bool) = x ? "true" : "false"
 
