@@ -398,13 +398,23 @@ int32_t launch_rdim(dab_ctx* ctx, const T* x, size_t inner, size_t red, size_t o
     return DAB_OK;
 }
 
-// out[0] (op)= slot[0]: lands the result of the flat whole-chunk reduce kernel when the "dimensional" reduction is really a
-// full reduction (inner == outer == 1)
+// out[0] (op)= S: lands the result of the flat whole-chunk reduce kernel when the "dimensional" reduction is really a full reduction
+// (inner == outer == 1).  Accumulating a float SUM / PROD combines out[0] with the un-rounded fp64 carrier S at slot bytes [8, 16) and
+// rounds once, as the launch_rdim kernels do; combining with the rounded slot[0] would round twice.
+__device__ __forceinline__ double slot_carrier(const void* slot) { return *reinterpret_cast<const double*>((const char*)slot + 8); }
+
 template <typename Out>
 __global__ void scalar_into_kernel(const Out* __restrict__ slot, Out* __restrict__ out, int accumulate, int op) {
     Out v = *slot;
     if (accumulate) {
         Out o = *out;
+        if constexpr (std::is_same<Out, float>::value) {
+            if (op == DAB_SUM || op == DAB_PROD) {
+                const double s = slot_carrier(slot);
+                *out = (float)(op == DAB_SUM ? jl::add((double)o, s) : jl::mul((double)o, s));
+                return;
+            }
+        }
         switch (op) {
             case DAB_SUM: v = jl::add(o, v); break;
             case DAB_PROD: v = jl::mul(o, v); break;
@@ -415,14 +425,15 @@ __global__ void scalar_into_kernel(const Out* __restrict__ slot, Out* __restrict
     *out = v;
 }
 
-// Float16 result of a full reduction in disguise (see dab_reducedim); accumulate folds in Float16 arithmetic (Float32, rounded back)
+// Float16 result of a full reduction in disguise (see dab_reducedim); accumulate rounds op(out, S) once to Float16: SUM / PROD in the fp64
+// carrier, MAX / MIN exactly in Float32
 __global__ void half_into_kernel(const Half* __restrict__ slot, Half* __restrict__ out, int accumulate, int op) {
     Half v = *slot;
     if (accumulate) {
         const float o = (float)*out, w = (float)v;
         switch (op) {
-            case DAB_SUM: v = Half(jl::add(o, w)); break;
-            case DAB_PROD: v = Half(jl::mul(o, w)); break;
+            case DAB_SUM: v = Half(jl::add((double)o, slot_carrier(slot))); break;
+            case DAB_PROD: v = Half(jl::mul((double)o, slot_carrier(slot))); break;
             case DAB_MAX: v = Half(jl::max(o, w)); break;
             default: v = Half(jl::min(o, w)); break;
         }

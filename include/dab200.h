@@ -269,8 +269,9 @@ int32_t dab_combine_ordered(int32_t result_dtype, int32_t op, const void* partia
  * the column-major shape (inner, reduce, outer): out[i + inner*o] (op)= x[i + inner*(r + reduce*o)].
  * accumulate == 0: out is overwritten with the reduction (SUM/PROD seeded with 0/1, MAX/MIN with
  * the first element); accumulate != 0: the reduction is combined ONTO the existing out
- * (how init= and the between-phase enter, SURVEY Appendix A.3).  Output dtype follows
- * dab_reduce_result_dtype. */
+ * (how init= and the between-phase enter, SURVEY Appendix A.3).  For float SUM / PROD the combine
+ * rounds op(out, S) ONCE to the output type: S, the reduction, stays in its fp64 carrier until then,
+ * on every launch path.  Output dtype follows dab_reduce_result_dtype. */
 int32_t dab_reducedim(dab_ctx* ctx, int32_t dtype, int32_t op, int32_t map, const void* x, size_t inner, size_t reduce,
                       size_t outer, void* out, int32_t accumulate);
 

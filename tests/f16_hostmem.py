@@ -90,6 +90,10 @@ def install():
                 return 3
             r = _fold(m, op) if int(n) else np.asarray(1.0 if op == 1 else 0.0, _H)
             slot[:2] = np.asarray([r], dtype=_H).view(np.uint8)
+            if op in (0, 1):                                         # the fp64 carrier, as the kernel leaves it in bytes [8, 16)
+                with np.errstate(all="ignore"):
+                    w = m.astype(np.float64)
+                    slot[8:] = np.asarray([w.sum() if op == 0 else w.prod()]).view(np.uint8)
         C.memmove(hm._addr(out), slot.ctypes.data, 16)
         self.launches += 1
         return 0
@@ -142,6 +146,8 @@ def install():
         if not _float16_call(dts, nargs, val_dtype):
             return orig["dab_mapreduce_expr"](self, ctx, src, val_dtype, op, n, nargs, dts, ptrs, scal, out)
         op, n = int(op), int(n)
+        if any(ptrs[k] and hm._addr(ptrs[k]) % (8 * _dt(dts[k]).itemsize) for k in range(int(nargs))):
+            return 6                                                 # DAB_ERR_UNSUPPORTED: arrays must be aligned to 8 elements
         args = []
         for k in range(int(nargs)):
             dt = _dt(dts[k])
@@ -152,12 +158,13 @@ def install():
         if v.dtype == np.bool_:
             c = int(np.count_nonzero(v))
             slot.view(np.int64)[:] = [{0: c, 6: c, 4: int(c == n), 5: int(c != 0)}[op], c]
-        elif v.dtype == _H:
-            slot[:2] = np.asarray([_fold(v.astype(np.float32), op)], dtype=_H).view(np.uint8)
-        else:                                                        # Float32 / Float64 values of Float16 arguments
-            with np.errstate(all="ignore"):
+        else:                                                        # word 1: the fp64 carrier of + and *; max / min: the extreme again,
+            with np.errstate(all="ignore"):                          # in Float32 for Float16 values
                 acc = (v.astype(np.float64).sum() if op == 0 else v.astype(np.float64).prod()) if op in (0, 1) else hm.jl_extreme(v, 0, op == 2)
             slot[:v.itemsize] = np.asarray([acc], dtype=v.dtype).view(np.uint8)
+            wide = np.float64 if op in (0, 1) else (np.float32 if v.dtype == _H else v.dtype)
+            b = np.asarray([acc], dtype=wide).view(np.uint8)
+            slot[8:8 + b.size] = b
         C.memmove(hm._addr(out), slot.ctypes.data, 16)
         self.launches += 2
         return 0

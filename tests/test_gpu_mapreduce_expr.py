@@ -16,9 +16,11 @@ result is exact, and comparisons are bit for bit on the whole 16-byte result slo
   * max / min: Julia's rules -- any NaN gives NaN, a zero result is +0.0 for max when a +0.0 is present and -0.0 for min when a
     -0.0 is present.  The reference functions are this module's own.
 
-The deciding values sit where the kernel splits its work: element 0 and n-1, both sides of every tile boundary and of the +1024 half
-inside a tile, the four lanes of one vector, both sides of CTA boundaries (the ones ``dab_mr_final`` reads in its 4-load loop
-included) and the first element of the scalar tail.
+The deciding values sit where the kernel splits its work: element 0 and n-1, both sides of every tile boundary and of the half-tile
+inside a tile, the lanes of one vector, both sides of CTA boundaries (the ones ``dab_mr_final`` reads in its 4-load loop included)
+and the first element of the scalar tail.  A Float16 argument makes every thread step 8 elements wide (16-byte loads), so tiles are
+4096 elements instead of 2048; the model and the edges take the width, and every launch case is run at both widths, with Float16,
+Float32 and Float64 values of Float16 arguments (Float16 values: a Float32 tile, the fp64 carrier, one rounding to Float16).
 """
 import ctypes as C
 import os
@@ -30,15 +32,22 @@ pytestmark = pytest.mark.gpu
 
 HOSTMEM = os.environ.get("DAB_HOSTMEM") == "1"
 OK, ERR_ARG, ERR_EMPTY, ERR_UNSUPPORTED = 0, 2, 3, 6
-F32, F64, I32, I64, U8, I128, C64, C128 = range(8)
+F32, F64, I32, I64, U8, I128, C64, C128, F16 = range(9)
 SUM, PROD, MAX, MIN, ALL, ANY, COUNT, EXTREMA = range(8)
 NP = {F32: np.dtype(np.float32), F64: np.dtype(np.float64), I32: np.dtype(np.int32), I64: np.dtype(np.int64), U8: np.dtype(np.bool_),
-      C64: np.dtype(np.complex64), C128: np.dtype(np.complex128)}
+      C64: np.dtype(np.complex64), C128: np.dtype(np.complex128), F16: np.dtype(np.float16)}
 TILE, MAX_PARTS = 2048, 16384           # 2 x 256 threads x 4 elements; dab_mr_final folds at most this many partials
+TILE16 = 4096                           # with a Float16 argument a thread step takes 8 elements (16-byte loads): 2 x 256 x 8
 G = 2.0 ** -10
 M64, M128 = (1 << 64) - 1, (1 << 128) - 1
 SERVED = ([(v, op) for v in (F32, F64, I32, I64, I128) for op in (SUM, PROD, MAX, MIN)] + [(U8, op) for op in (SUM, COUNT, ALL, ANY)] +
           [(v, op) for v in (C64, C128) for op in (SUM, PROD)])
+# Float16 arguments: Float16, Float32 and Float64 values, each with + * max min (the kernel takes 8 elements per thread step)
+SERVED16 = [(v, op) for v in (F16, F32, F64) for op in (SUM, PROD, MAX, MIN)]
+
+if HOSTMEM:                                                     # the Float16 code of the host-memory emulation
+    import f16_hostmem
+    f16_hostmem.install()
 
 
 def _lib():
@@ -52,20 +61,21 @@ def _bc():
 
 
 # ---------------------------------------------------------------------------------------------------------- the launch model
-def model_mr(n):
-    """``dab_mapreduce_expr``'s launch plan for n elements: tiles, tiles per CTA, grid, the last CTA's tiles, tail, final-fold case."""
-    ntiles = n // TILE
+def model_mr(n, tile=TILE):
+    """``dab_mapreduce_expr``'s launch plan for n elements: tiles, tiles per CTA, grid, the last CTA's tiles, tail, final-fold case.
+    ``tile`` is 512 thread steps of the lane width: TILE, or TILE16 with a Float16 argument."""
+    ntiles = n // tile
     k = 2
     if -(-ntiles // k) > MAX_PARTS:
         k = -(-ntiles // MAX_PARTS)
     grid = max(1, -(-ntiles // k))
     last = ntiles - (grid - 1) * k if ntiles else 0
     final = "parts<=768" if grid <= 768 else "768<parts<=1024" if grid <= 1024 else "parts=16384" if grid == MAX_PARTS else "parts>1024"
-    return dict(ntiles=ntiles, k=k, grid=grid, last_tiles=last, tail=(ntiles * TILE, n), final=final)
+    return dict(ntiles=ntiles, k=k, grid=grid, last_tiles=last, tail=(ntiles * tile, n), final=final)
 
 
-def branches(n):
-    m = model_mr(n)
+def branches(n, tile=TILE):
+    m = model_mr(n, tile)
     out = {m["final"], "k=2" if m["k"] == 2 else "k>2"}
     if m["ntiles"] == 0:
         out.add("tail only")
@@ -75,7 +85,7 @@ def branches(n):
         out.add("tiles and tail")
     if m["ntiles"] and m["last_tiles"] < m["k"]:
         out.add("short last CTA")
-    if n % 4:
+    if n % (tile // 512):
         out.add("partial vector")
     return out
 
@@ -92,6 +102,12 @@ I128_SIZES = [s for s in SIZES if s < 3 * TILE + 6] if HOSTMEM else SIZES   # th
 PARTS_16384_N = 32767 * TILE + 5                # 16384 partials, the last CTA with one tile, a tail
 K_GT_2_N = 32771 * TILE + 7                     # 3 tiles per CTA (the first size past 16384 partials of 2), short last CTA, a tail
 BOOL_2_31_N = (1 << 31) + 2 * TILE + 3
+# the same cases with 8-element thread steps
+SIZES16 = [1, 3, 7, 8, 9, TILE16 - 1, TILE16, TILE16 + 1, 2 * TILE16, 3 * TILE16 + 5, 5 * TILE16 + 4095,
+           767 * 2 * TILE16 + 4093, 768 * 2 * TILE16, 768 * 2 * TILE16 + TILE16 + 1, 1024 * 2 * TILE16, 1024 * 2 * TILE16 + 2 * TILE16 + 3]
+PARTS_16384_N16 = 32767 * TILE16 + 5
+K_GT_2_N16 = 32771 * TILE16 + 7
+FULL_SIZE_RUNS16 = [(F16, SUM), (F32, MAX)]     # both sizes, in test_full_size_float16_argument
 
 
 def carrier(val, op):
@@ -119,24 +135,30 @@ def test_shape_table_reaches_every_branch():
         assert REQUIRED <= got, (width, sorted(REQUIRED - got))
     assert model_mr(K_GT_2_N)["k"] == 3 and model_mr(K_GT_2_N - 7 - 3 * TILE)["k"] == 2     # the first ntiles past 2 * 16384
     assert model_mr(PARTS_16384_N)["grid"] == MAX_PARTS and model_mr(1)["grid"] == 1
+    got = set()                                                  # 8-element steps: SIZES16 and the full-size Float16-argument runs
+    for n in SIZES16 + [PARTS_16384_N16, K_GT_2_N16]:
+        got |= branches(n, TILE16)
+    assert REQUIRED <= got, ("width 8", sorted(REQUIRED - got))
+    assert model_mr(K_GT_2_N16, TILE16)["k"] == 3 and model_mr(PARTS_16384_N16, TILE16)["grid"] == MAX_PARTS
 
 
-def edge_positions(n):
-    """Where the kernel changes what it does, for n elements."""
-    m = model_mr(n)
+def edge_positions(n, tile=TILE):
+    """Where the kernel changes what it does, for n elements and a tile of ``tile`` elements (lane width tile // 512)."""
+    m = model_mr(n, tile)
     k, grid, nt = m["k"], m["grid"], m["ntiles"]
-    pos = {0, 1, 2, 3, n - 2, n - 1}
+    w, half = tile // 512, tile // 2
+    pos = {0, 1, 2, 3, w - 1, w, n - 2, n - 1}
     for t in {0, 1, nt // 2, nt - 2, nt - 1}:
         if 0 <= t < nt:
-            b = t * TILE
-            pos |= {b, b + 1, b + 1023, b + 1024, b + 1025, b + TILE - 1}
-    lane = 4 * 37                                    # the four lanes of thread 37's vectors, in both halves of the first and last tile
+            b = t * tile
+            pos |= {b, b + 1, b + half - 1, b + half, b + half + 1, b + tile - 1}
+    lane = w * 37                                    # the lanes of thread 37's vectors, in both halves of the first and last tile
     for t in {0, max(nt - 1, 0)}:
-        pos |= {t * TILE + h + lane + j for h in (0, 1024) for j in range(4)}
+        pos |= {t * tile + h + lane + j for h in (0, half) for j in range(w)}
     for c in {1, 2, grid // 2, grid - 1, 256, 511, 512, 767, 768, 769, 1023, 1024}:
         if 0 < c < grid:
-            pos |= {c * k * TILE - 1, c * k * TILE}
-    tail = nt * TILE
+            pos |= {c * k * tile - 1, c * k * tile}
+    tail = nt * tile
     pos |= {tail - 1, tail, tail + 1}
     return np.asarray(sorted(p for p in pos if 0 <= p < n), dtype=np.int64)
 
@@ -160,9 +182,24 @@ def jl_extreme(m, is_max):
     return r
 
 
-def spec(val, op):
+def spec16(val, op):
+    """(Float16, traced closure, its NumPy twin) with a Float16 argument: Float16 values (every operation rounds to Float16, as NumPy's
+    float16 does), Float32 values (a Float32 constant promotes) and Float64 values (a Python float is a Float64 literal)."""
+    if val in (F16, F32):
+        T = NP[val].type
+        f = {SUM: lambda x: x * T(2) - T(2.0 ** -7), PROD: lambda x: (x + x) * T(0.5)}.get(op, lambda x: -(x * T(2)))
+        return NP[F16], f, f
+    f, twin = {SUM: (lambda x: x * 2.0 - 2.0 ** -7, lambda x: x.astype(np.float64) * 2.0 - 2.0 ** -7),
+               PROD: (lambda x: (x + x) * 0.5, lambda x: (x + x).astype(np.float64) * 0.5)}.get(
+        op, (lambda x: -(x * 2.0), lambda x: -(x.astype(np.float64) * 2.0)))
+    return NP[F16], f, twin
+
+
+def spec(val, op, arg16=False):
     """(input element type, traced closure, its NumPy twin).  None of the closures is one of the fixed map codes."""
     bc = _bc()
+    if arg16:
+        return spec16(val, op)
     if val in (F32, F64):
         T = NP[val].type
         if op == SUM:
@@ -276,6 +313,10 @@ def want_slot(val, op, acc, n):
         R = np.float32 if val == C64 else np.float64
         w[:2 * np.dtype(R).itemsize] = np.asarray([acc.real, acc.imag], dtype=np.float64).astype(R).tobytes()
         fl = [(0, R), (np.dtype(R).itemsize, R)]
+    elif val == F16:                                       # Float32 carrier for max / min
+        w[:2] = np.float16(acc).tobytes()
+        w[8:16 if op in (SUM, PROD) else 12] = (np.float64 if op in (SUM, PROD) else np.float32)(acc).tobytes()
+        fl = [(0, np.float16), (8, np.float64 if op in (SUM, PROD) else np.float32)]
     elif val in (F32, F64):
         T = NP[val].type
         if op in (SUM, PROD):
@@ -374,27 +415,27 @@ def code_of(dt):
 
 
 def val_code(jt):
-    return {"f32": F32, "f64": F64, "i32": I32, "i64": I64, "bool": U8, "i128": I128, "c64": C64, "c128": C128}[jt]
+    return {"f32": F32, "f64": F64, "i32": I32, "i64": I64, "bool": U8, "i128": I128, "c64": C64, "c128": C128, "f16": F16}[jt]
 
 
 # ---------------------------------------------------------------------------------------------------------- input builders
 def nan_values(T, count):
     """NaNs of both signs, quiet and signalling, with payloads."""
-    U = {4: np.uint32, 8: np.uint64}[np.dtype(T).itemsize]
-    bits = 8 * np.dtype(T).itemsize
-    expo = 0x7F800000 if bits == 32 else 0x7FF0000000000000
-    quiet = 1 << (22 if bits == 32 else 51)
+    U = {2: np.uint16, 4: np.uint32, 8: np.uint64}[np.dtype(T).itemsize]
+    bits, nmant = 8 * np.dtype(T).itemsize, np.finfo(T).nmant
+    quiet = 1 << (nmant - 1)
+    expo = ((1 << (bits - 1)) - 1) ^ ((1 << nmant) - 1)
     out = []
     for j in range(count):
-        payload = (0x2A5 + 7 * j) | (quiet if j % 4 < 2 else 0)
+        payload = ((0x2A5 + 7 * j) & (quiet - 1)) | (quiet if j % 4 < 2 else 0)
         out.append(np.asarray([expo | payload | ((1 << (bits - 1)) if j % 2 else 0)], dtype=U).view(T)[0])
     return out
 
 
-def base_input(val, op, n, rng):
+def base_input(val, op, n, rng, arg16=False):
     """Input values whose mapped values never decide a max / min / all / any on their own and keep every sum and product exact."""
-    T = spec(val, op)[0]
-    if val in (F32, F64):
+    T = spec(val, op, arg16)[0]
+    if val in (F32, F64, F16):
         if op == SUM:
             return (rng.integers(-8, 9, n) * G).astype(T)
         if op == PROD:
@@ -429,7 +470,7 @@ def edge_cases(val, op, x_e, rng):
     T = x_e.dtype.type
     k = len(x_e)
     cases = []
-    if val in (F32, F64):
+    if val in (F32, F64, F16):
         if op in (SUM, PROD):
             fin = np.asarray([16, -15, 14, -13, 12, -11] if op == SUM else [2, -0.5, -2, 0.5], dtype=np.float64)
             fin = (fin * (G if op == SUM else 1.0))[np.arange(k) % len(fin)].astype(T)
@@ -517,13 +558,15 @@ def run_positions(k):
     return range(k) if not HOSTMEM else range(0, k, max(1, k // 3))
 
 
-def run_abi_cases(rt, slot, val, op, n, rng):
-    """Upload one input of n elements, then run every edge case of (val, op) on it; returns a list of failures."""
-    T, f, twin = spec(val, op)
+def run_abi_cases(rt, slot, val, op, n, rng, arg16=False):
+    """Upload one input of n elements, then run every edge case of (val, op) on it; returns a list of failures.  arg16: the input is
+    Float16 (spec16), and the edges are those of 8-element thread steps."""
+    T, f, twin = spec(val, op, arg16)
     src, jt = source(f, [_bc().tag_of(T)])
     assert val_code(jt) == val, (jt, val)
-    x = base_input(val, op, n, rng)
-    E = edge_positions(n)
+    x = base_input(val, op, n, rng, arg16)
+    tile = TILE16 if arg16 else TILE
+    E = edge_positions(n, tile)
     rest = np.ones(n, dtype=bool)
     rest[E] = False
     acc_rest = acc_of(val, op, mapped(val, twin, x[rest]))
@@ -549,7 +592,7 @@ def run_abi_cases(rt, slot, val, op, n, rng):
                 bad.append(f"n={n}: {rt.launches() - n0} launches")
             elif not slot_matches(got, want, fl, zero_sign_free=val in (C64, C128) and op == PROD):
                 changed = E[np.flatnonzero(case.view(np.uint8).reshape(len(E), -1).any(axis=1))][:4]
-                bad.append(f"n={n} model={model_mr(n)} edges~{changed.tolist()}: got [{show(got)}] want [{show(want)}]")
+                bad.append(f"n={n} model={model_mr(n, tile)} edges~{changed.tolist()}: got [{show(got)}] want [{show(want)}]")
     finally:
         xd.free()
     return bad
@@ -557,7 +600,7 @@ def run_abi_cases(rt, slot, val, op, n, rng):
 
 # ---------------------------------------------------------------------------------------------------------- (1) every served pair, every size
 def _sid(p):
-    return {F32: "f32", F64: "f64", I32: "i32", I64: "i64", U8: "bool", I128: "i128", C64: "c64", C128: "c128"}[p[0]] + "-" + \
+    return {F32: "f32", F64: "f64", I32: "i32", I64: "i64", U8: "bool", I128: "i128", C64: "c64", C128: "c128", F16: "f16"}[p[0]] + "-" + \
         {SUM: "sum", PROD: "prod", MAX: "max", MIN: "min", ALL: "all", ANY: "any", COUNT: "count"}[p[1]]
 
 
@@ -572,6 +615,101 @@ def test_abi_exact_on_every_launch_path(dab, rt1, pair):
     finally:
         slot.free()
     assert not bad, f"{len(bad)} failures: " + "; ".join(bad[:6])
+
+
+SIZES16_RUN = SIZES16 if not HOSTMEM else [s for s in SIZES16 if s < 6 * TILE16]   # the emulation evaluates Float16 trees slowly
+
+
+@pytest.mark.parametrize("pair", SERVED16, ids=lambda p: "f16arg-" + _sid(p))
+def test_abi_exact_float16_argument_every_launch_path(dab, rt1, pair):
+    """A Float16 argument makes every thread step 8 elements wide (tiles of 4096): every launch case at that width, for Float16,
+    Float32 and Float64 values."""
+    val, op = pair
+    slot = Slot(rt1)
+    bad = []
+    try:
+        for si, n in enumerate(SIZES16_RUN):
+            bad += run_abi_cases(rt1, slot, val, op, n, np.random.default_rng(1000 * si + 10 * val + op), arg16=True)
+    finally:
+        slot.free()
+    assert not bad, f"{len(bad)} failures: " + "; ".join(bad[:6])
+
+
+@pytest.mark.parametrize("n", [9, TILE16 + 1, 3 * TILE16 + 5, 40 * TILE16 + 1001])
+def test_argument_tables_float16_mixed_widths(dab, rt1, n):
+    """Float16 arrays with Float32, Float64 and Int32 arrays and a Float16 scalar (the 8-element step reads 16, 32 and 64 bytes per
+    argument), and pointers 8 or 16 elements past their allocation."""
+    rng = np.random.default_rng(n)
+    h = _grid(rng, n).astype(np.float16)
+    f32 = _grid(rng, n).astype(np.float32)
+    f64 = _grid(rng, n).astype(np.float64)
+    i32 = rng.integers(-1000, 1000, n).astype(np.int32)
+    f16 = np.float16
+    cases = [
+        (lambda a, x: a * x, [h, f32], SUM, lambda: h.astype(np.float32) * f32),                       # Float32 values
+        (lambda a, x: a * x, [h, f32], MAX, lambda: h.astype(np.float32) * f32),
+        (lambda a, y: a * y + a, [h, f64], SUM, lambda: h.astype(np.float64) * f64 + h),                 # Float64 values
+        (lambda a, i: a * i, [h, i32], SUM, lambda: h * i32.astype(f16)),                                # Float16 * Int32: Float16, rounded
+        (lambda a, i: a * i, [h, i32], MIN, lambda: h * i32.astype(f16)),
+        (lambda a, s: a * s, [h, (f16(1.5), f16)], SUM, lambda: h * f16(1.5)),                            # a Float16 scalar
+        (lambda a, x, y, i: (a * x + y) * i, [h, f32, f64, i32], SUM, lambda: (h.astype(np.float32) * f32 + f64) * i32),
+    ]
+    slot = Slot(rt1)
+    bad = []
+    try:
+        for ci, (f, args, op, ref) in enumerate(cases):
+            with np.errstate(all="ignore"):
+                m = np.asarray(ref())
+            for offs in ([0] * len(args), [8 * (k % 3) for k in range(len(args))]):
+                st, got, want = _arg_table_case(rt1, slot, f, args, op, m, offs)
+                if st != OK:
+                    bad.append(f"case {ci} offs {offs}: status {st}")
+                elif not slot_matches(got, *want):
+                    bad.append(f"case {ci} offs {offs}: got [{show(got)}] want [{show(want[0])}]")
+    finally:
+        slot.free()
+    assert not bad, "; ".join(bad)
+
+
+def test_float16_alignment_refusals(dab, rt1):
+    """With a Float16 argument every array argument must be aligned to 8 of its elements: a Float16 array 1..7 elements in, a Float32 array
+    4 elements (16 bytes) in and a Float64 array 4 elements (32 bytes) in are refused without a launch; 8 elements in is served exactly."""
+    rng = np.random.default_rng(17)
+    n = 2 * TILE16 + 5
+    h = _grid(rng, n).astype(np.float16)
+    x32 = _grid(rng, n).astype(np.float32)
+    x64 = _grid(rng, n).astype(np.float64)
+    slot = Slot(rt1)
+    bufs = {dt: Dev(rt1, np.zeros(n + 16, NP[dt])) for dt in (F16, F32, F64)}
+
+    def place(dt, a, e):                                                   # a, e elements past a 256-byte aligned allocation
+        bufs[dt].put(e, a)
+        return bufs[dt].ptr + e * NP[dt].itemsize
+
+    try:
+        src1, _ = source(lambda a: a * np.float16(2), ["f16"])
+        src2, _ = source(lambda a, x: a * x, ["f16", "f32"])
+        src3, _ = source(lambda a, y: a * y, ["f16", "f64"])
+        refusals = [(src1, F16, [F16], [place(F16, h, e)]) for e in range(1, 8)]
+        refusals += [(src2, F32, [F16, F32], [place(F16, h, 0), place(F32, x32, 4)]), (src3, F64, [F16, F64], [place(F16, h, 0), place(F64, x64, 4)])]
+        for src, val, dts, ptrs in refusals:
+            slot.clear()
+            n0 = rt1.launches()
+            assert mr_status(rt1, src, val, SUM, n, dts, ptrs, [0] * len(dts), slot.ptr) == ERR_UNSUPPORTED, (val, ptrs)
+            assert rt1.launches() == n0 and slot.get() == Slot.FILL, (val, ptrs)
+        served = [(src1, F16, [F16], [h], h * np.float16(2)), (src2, F32, [F16, F32], [h, x32], h.astype(np.float32) * x32),
+                  (src3, F64, [F16, F64], [h, x64], h.astype(np.float64) * x64)]
+        for src, val, dts, arrs, m in served:
+            ptrs = [place(dt, a, 8) for dt, a in zip(dts, arrs)]           # 8 elements in: aligned, served
+            slot.clear()
+            assert mr_status(rt1, src, val, SUM, n, dts, ptrs, [0] * len(dts), slot.ptr) == OK, val
+            want, fl = want_slot(val, SUM, acc_of(val, SUM, m), n)
+            got = slot.get()
+            assert slot_matches(got, want, fl), (val, show(got), show(want))
+    finally:
+        slot.free()
+        for d in bufs.values():
+            d.free()
 
 
 # ---------------------------------------------------------------------------------------------------------- (2) argument tables
@@ -980,6 +1118,23 @@ def test_full_size_16384_partials(dab, rt1):
     try:
         for val, op in FULL_SIZE_RUNS[PARTS_16384_N]:
             bad += run_abi_cases(rt1, slot, val, op, PARTS_16384_N, np.random.default_rng(val * 10 + op + 1))
+    finally:
+        slot.free()
+    assert not bad, "; ".join(bad[:6])
+
+
+@pytest.mark.parametrize("n", [PARTS_16384_N16, K_GT_2_N16], ids=["parts16384", "k3"])
+def test_full_size_float16_argument(dab, rt1, n):
+    """The final-fold cases of 8-element steps: 16384 partials (the last CTA with one tile) and 3 tiles per CTA, each with a tail, for a
+    Float16 argument (about 134M elements) with Float16 and Float32 values (8- and 4-byte carriers)."""
+    _need(rt1, 2)
+    m = model_mr(n, TILE16)
+    assert (m["grid"] == MAX_PARTS) if n == PARTS_16384_N16 else (m["k"] == 3), m
+    slot = Slot(rt1)
+    bad = []
+    try:
+        for val, op in FULL_SIZE_RUNS16:
+            bad += run_abi_cases(rt1, slot, val, op, n, np.random.default_rng(val * 10 + op + 2), arg16=True)
     finally:
         slot.free()
     assert not bad, "; ".join(bad[:6])

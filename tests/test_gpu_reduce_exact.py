@@ -5,11 +5,15 @@ API with inputs whose results are exact, so every comparison is bit for bit (NaN
 
   * integers: any values -- the map runs in the element type (``abs``/``abs2``/``-`` wrap at 32 bits for Int32, as in Julia), then
     Int32 widens to Int64 and ``+``/``*`` run mod 2^64, which is associative, so every grouping gives the same bits;
-  * float sums: multiples of 2^-10 with |x| <= 8*2^-10 -- every tile of <= 16 values is exact in Float32 and the fp64 carrier is
-    exact, so the result is the exact sum rounded once;
+  * float sums: multiples of 2^-10 with |x| <= 8*2^-10 -- every tile of <= 32 values is exact in Float32 and the fp64 carrier is
+    exact, so the result is the exact sum rounded once; with ``accumulate`` the result is op(out, S) rounded once;
   * float products: +-1 with +-2 / +-0.5 at the edge positions (the exponent stays in {-1, 0, 1}), exact in any order;
   * max / min / extrema: Julia's rules -- any NaN gives NaN, otherwise the extreme value, and a zero result is +0.0 for max when
     a +0.0 is present and -0.0 for min when a -0.0 is present.
+
+Float16 elements are widened to Float32 by the map (abs2 rounds x*x to Float16 first), so the same inputs are exact for them, and the
+references round the exact fp64 result once to Float16; their edge values add +-65504 and subnormals.  Fibres whose sum lies just past
+a rounding midpoint (``ROUND_ONCE``) tell one rounding from a rounding through Float32 on every path.
 
 Edge values (NaN with payloads and both signs, +-0, +-Inf, typemin / typemax, Int32 values near +-2^30 and +-2^31) sit where the
 kernels split their work: first and last element of a run, the head peel of an unaligned run, the last partial 16-byte vector, the
@@ -26,12 +30,18 @@ pytestmark = pytest.mark.gpu
 
 HOSTMEM = os.environ.get("DAB_HOSTMEM") == "1"
 F32, F64, I32, I64, U8 = range(5)
+F16 = 8
 SUM, PROD, MAX, MIN, ALL, ANY, COUNT, EXTREMA = range(8)
 MAP_ID, MAP_ABS, MAP_ABS2, MAP_NEG = range(4)
-NP = {F32: np.float32, F64: np.float64, I32: np.int32, I64: np.int64, U8: np.uint8}
+NP = {F32: np.float32, F64: np.float64, I32: np.int32, I64: np.int64, U8: np.uint8, F16: np.float16}
 OPS = (SUM, PROD, MAX, MIN)
 MAPS = (MAP_ID, MAP_ABS, MAP_ABS2, MAP_NEG)
 RD_THREADS, RD_UNROLL = 256, 4
+DTS, DT_IDS = [F32, F64, I32, I64, F16], ["f32", "f64", "i32", "i64", "f16"]
+
+if HOSTMEM:                                                     # the Float16 code of the host-memory emulation
+    import f16_hostmem
+    f16_hostmem.install()
 
 
 def _lib():
@@ -49,7 +59,7 @@ def same_bits(got, want):
     nan = np.isnan(want)
     if not np.array_equal(np.isnan(got), nan):
         return False
-    u = {4: np.uint32, 8: np.uint64}[got.dtype.itemsize]
+    u = {2: np.uint16, 4: np.uint32, 8: np.uint64}[got.dtype.itemsize]
     return np.array_equal(got.view(u)[~nan], want.view(u)[~nan])
 
 
@@ -79,21 +89,23 @@ def jl_extreme(m, axis, is_max):
     return np.where(nan.any(axis=axis), m.dtype.type(np.nan), r).astype(m.dtype)
 
 
-def ref_reduce(m, op, axis):
-    """m: mapped values in the element type."""
+def ref_reduce(m, op, axis, wide=False):
+    """m: mapped values in the element type.  wide: a float sum / product as its exact fp64 value S, not rounded to the element type."""
     m = np.asarray(m)
     with np.errstate(all="ignore"):
         if op in (SUM, PROD):
             if m.dtype.kind == "f":
                 w = m.astype(np.float64)               # exact: see the module docstring
-                return (w.sum(axis=axis) if op == SUM else w.prod(axis=axis)).astype(m.dtype)
+                w = w.sum(axis=axis) if op == SUM else w.prod(axis=axis)
+                return w if wide else w.astype(m.dtype)
             w = m.astype(np.int64)                     # NumPy's Int64 sum / prod wrap mod 2^64
             return w.sum(axis=axis, dtype=np.int64) if op == SUM else w.prod(axis=axis, dtype=np.int64)
         return jl_extreme(m, axis, op == MAX)
 
 
 def ref_combine(o, r, op):
-    """op(o, r) elementwise in the result type (the accumulate=1 prefill)."""
+    """op(o, r) elementwise in the result type (the accumulate=1 prefill).  A float sum / product r is given as its exact fp64 value S
+    (``ref_reduce(..., wide=True)``): o + S and o * S are exact in fp64 here and round once to the result type."""
     o, r = np.asarray(o), np.asarray(r)
     if op in (MAX, MIN):
         return jl_extreme(np.stack([o, r]), 0, op == MAX)
@@ -185,9 +197,9 @@ def shape_table(dt, sm_count):
 
 
 def test_shape_table_reaches_every_branch(dab, rt1):
-    """The table below reaches every branch of launch_rdim, for a 4-byte and an 8-byte element type, on this device."""
+    """The table below reaches every branch of launch_rdim, for a 2-, a 4- and an 8-byte element type, on this device."""
     sm = rt1.device_info()["sm_count"]
-    for dt in (F32, F64, I32, I64):
+    for dt in DTS:
         got = set()
         for name, (inner, red, outer, off) in shape_table(dt, sm).items():
             es = np.dtype(NP[dt]).itemsize
@@ -247,13 +259,13 @@ def build(dt, op, inner, red, outer, edges, seed, kind_shift=0, kinds=None):
             xf[ii[sel], :, oo[sel]] = -np.abs(xf[ii[sel], :, oo[sel]])
             sel = kind == 3
             xf[ii[sel], :, oo[sel]] = np.abs(xf[ii[sel], :, oo[sel]])
-            U = {np.float32: np.uint32, np.float64: np.uint64}[T]
-            bits = 8 * np.dtype(T).itemsize
-            sign, quiet, frac = 1 << (bits - 1), 1 << (bits - 10 if T == np.float32 else bits - 13), (1 << (23 if T == np.float32 else 52)) - 1
-            expo = 0x7F800000 if T == np.float32 else 0x7FF0000000000000
+            U = {np.float16: np.uint16, np.float32: np.uint32, np.float64: np.uint64}[T]
+            bits, nmant = 8 * np.dtype(T).itemsize, np.finfo(T).nmant
+            sign, quiet, frac = 1 << (bits - 1), 1 << (nmant - 1), (1 << nmant) - 1
+            expo = ((1 << (bits - 1)) - 1) ^ frac
             f = np.flatnonzero(kind == 0)                       # NaN: quiet and signalling payloads, both signs
             g = f // 6
-            payload = (rng.integers(1, 1 << 20, f.size).astype(np.uint64) | np.where(g % 4 < 2, quiet, 0).astype(np.uint64)) & np.uint64(frac)
+            payload = (rng.integers(1, min(1 << 20, quiet), f.size).astype(np.uint64) | np.where(g % 4 < 2, quiet, 0).astype(np.uint64)) & np.uint64(frac)
             nanv = (np.uint64(expo) | payload | np.where(g % 2 == 1, np.uint64(sign), np.uint64(0))).astype(U).view(T)
             xf[ii[f], e1[f], oo[f]] = nanv
             f = np.flatnonzero(kind == 1)
@@ -264,10 +276,22 @@ def build(dt, op, inner, red, outer, edges, seed, kind_shift=0, kinds=None):
             xf[ii[f], e2[f], oo[f]] = T(-0.0)
             f = np.flatnonzero(kind == 3)
             xf[ii[f], e1[f], oo[f]] = T(-0.0)
-            if op != PROD:
+            if op != PROD and T != np.float16:
                 f = np.flatnonzero(kind == 4)
                 xf[ii[f], e1[f], oo[f]] = T(16 * 2.0 ** -10)
                 xf[ii[f], e2[f], oo[f]] = T(-16 * 2.0 ** -10)
+            elif op != PROD:
+                # Float16 extremes.  max / min: +-65504 and the smallest and largest subnormals decide (abs2 takes 65504 to Inf).  Sums:
+                # 65504 twice with one sign overflows to +-Inf (once, the result stays 65504: the rest is far below its 16-unit rounding
+                # margin); subnormals 2^-24 and -3 * 2^-24 pull an exact sum 2^-23 below its grid point, which for half the sums is just
+                # below a Float16 rounding midpoint: one rounding goes down, a rounding through Float32 lands on the midpoint first
+                s = np.where(np.arange(len(kind)) % 2 == 0, 1.0, -1.0)              # one sign per fibre
+                f = np.flatnonzero(kind == 4)
+                xf[ii[f], e1[f], oo[f]] = (s[f] * 65504.0).astype(T)
+                xf[ii[f], e2[f], oo[f]] = (s[f] * (65504.0 if op == SUM else -2.0 ** -24)).astype(T)
+                f = np.flatnonzero(kind == 5)
+                xf[ii[f], e1[f], oo[f]] = T(2.0 ** -24)
+                xf[ii[f], e2[f], oo[f]] = T(-3 * 2.0 ** -24 if op == SUM else -1023 * 2.0 ** -24)
         return np.asfortranarray(xf)
     info = np.iinfo(T)
     if op == PROD:                                              # odd factors never reach 0 mod 2^64
@@ -356,15 +380,15 @@ def rdim_call(rt, dt, op, mapc, x, inner, red, outer, out, acc):
 
 
 def _maps_for(dt, op, k):
-    """Int32 (widened sums and products; -x under max / min) takes every map on every shape; the other types take two maps per
-    shape, in turn."""
-    if dt == I32:
+    """Int32 (widened sums and products; -x under max / min) and Float16 (maps in Float32, abs2 rounded to Float16) take every map on
+    every shape; the other types take two maps per shape, in turn."""
+    if dt in (I32, F16):
         return MAPS
     return (MAPS[k % 4], MAPS[(k + 1) % 4])
 
 
 # ---------------------------------------------------------------------------------------------------------- (a) dab_reducedim
-@pytest.mark.parametrize("dt", [F32, F64, I32, I64], ids=["f32", "f64", "i32", "i64"])
+@pytest.mark.parametrize("dt", DTS, ids=DT_IDS)
 @pytest.mark.parametrize("name", list(shape_table(F32, 132)))
 def test_reducedim_exact(dab, rt1, name, dt):
     sm = rt1.device_info()["sm_count"]
@@ -386,7 +410,9 @@ def test_reducedim_exact(dab, rt1, name, dt):
         rdt = result_dtype(T, op)
         try:
             for mapc in _maps_for(dt, op, k + op + shift):
-                want = ref_reduce(ref_map(x, mapc), op, axis=1).reshape(-1, order="F").astype(rdt)
+                mx = ref_map(x, mapc)
+                want = ref_reduce(mx, op, axis=1).reshape(-1, order="F").astype(rdt)
+                wide = ref_reduce(mx, op, axis=1, wide=True).reshape(-1, order="F")
                 if (np.isfinite(want) & (want != 0)).any():
                     finite_nonzero.add(op)
                 out = Dev(rt1, np.zeros(inner * outer, dtype=rdt), 0)
@@ -402,7 +428,7 @@ def test_reducedim_exact(dab, rt1, name, dt):
                     out.put(pre)
                     rdim_call(rt1, dt, op, mapc, xd, inner, red, outer, out, 1)
                     got = out.get()
-                    want1 = ref_combine(pre, want, op)
+                    want1 = ref_combine(pre, wide, op)
                     if not same_bits(got, want1):
                         idx = first_bad(got, want1)
                         bad.append(f"op={op} map={mapc} acc=1 first bad outputs {idx.tolist()}: got {got[idx].tolist()} want {want1[idx].tolist()}")
@@ -414,7 +440,7 @@ def test_reducedim_exact(dab, rt1, name, dt):
     assert finite_nonzero == set(OPS), f"{name}: no finite nonzero result checked for ops {set(OPS) - finite_nonzero}"
 
 
-@pytest.mark.parametrize("dt", [F32, F64, I32, I64], ids=["f32", "f64", "i32", "i64"])
+@pytest.mark.parametrize("dt", DTS, ids=DT_IDS)
 def test_reducedim_empty_extents(dab, rt1, dt):
     """reduce == 0: SUM / PROD write the identity, MAX / MIN throw, accumulate leaves R as it is; inner*outer == 0 touches nothing."""
     L = _lib()
@@ -458,13 +484,20 @@ def reduce_call(rt, dt, op, mapc, x, n, slot):
     return slot.get(16, np.uint8)
 
 
-@pytest.mark.parametrize("dt", [F32, F64, I32, I64], ids=["f32", "f64", "i32", "i64"])
+@pytest.mark.parametrize("dt", DTS, ids=DT_IDS)
 def test_reduce_exact(dab, rt1, dt):
     T = NP[dt]
     vpt = 16 // np.dtype(T).itemsize
     slot = Dev(rt1, np.zeros(16, dtype=np.uint8), 0)
     bad = []
     finite_nonzero = set()
+    ops = OPS if dt == F16 else OPS + (EXTREMA,)          # Float16 extrema is a MIN and a MAX reduction: EXTREMA is refused
+    if dt == F16:
+        xd = Dev(rt1, np.ones(8, dtype=T), 0)
+        with pytest.raises(_lib().DabError) as err:
+            reduce_call(rt1, dt, EXTREMA, MAP_ID, xd, 8, slot)
+        assert err.value.status == _lib().ERR_UNSUPPORTED
+        xd.free()
     try:
         for si, n in enumerate(reduce_sizes(dt)):
             offs = range(vpt) if n < 10000 else (0, 1 % vpt)
@@ -476,7 +509,7 @@ def test_reduce_exact(dab, rt1, dt):
                                                            for p in (head + t * tile - 1, head + t * tile) if 0 <= p < n]
                 # floats: one input with NaN, +-Inf or a signed-zero rule (kinds 0-3), one with finite values (kinds 4-7), in turn
                 rot = si + off
-                for op, shift in [(op, shift) for op in OPS + (EXTREMA,)
+                for op, shift in [(op, shift) for op in ops
                                   for shift in (((rot + op) % 4, 4 + (rot + op) % 4) if np.dtype(T).kind == "f" else (0,))]:
                     data_op = PROD if op == PROD else SUM if op == EXTREMA else op
                     x = build(dt, data_op, 1, n, 1, sorted(set(edges)), seed=si * 31 + off * 7 + op + 1000 * shift, kind_shift=shift).reshape(-1)
@@ -501,7 +534,7 @@ def test_reduce_exact(dab, rt1, dt):
     finally:
         slot.free()
     assert not bad, "; ".join(bad[:12]) + f" ({len(bad)} cases)"
-    missing = {(op, n) for op in OPS + (EXTREMA,) for n in reduce_sizes(dt)} - finite_nonzero
+    missing = {(op, n) for op in ops for n in reduce_sizes(dt)} - finite_nonzero
     assert not missing, f"no finite nonzero result checked for (op, n) in {sorted(missing)}"
 
 
@@ -528,6 +561,144 @@ def test_reduce_bool_exact(dab, rt1, n):
                         assert slot_value(s, np.dtype(np.uint8)) == (x.max() if op == MAX else x.min()), (n, off, p, op)
     finally:
         slot.free()
+
+
+# ---------------------------------------------------------------------------------------------------------- (b2) one rounding
+# Fibres whose exact sum S lies just past a rounding midpoint of the result type, built so that every Float32 tile of every kernel is
+# exact (r = 0 and r = red - 1 never share a tile on these shapes) and only the fp64 carrier holds S:
+#   Float16: 32768 at r = 0, 16 in the middle, 2^-10 at r = red - 1: S = 32784 + 2^-10 rounds once to 32800 and to 32768 through
+#            Float32 (where 32784 is a tie, which goes to even);
+#   Float32: 1 at r = 0, 2^-27 at r = red - 1: S = 1 + 2^-27 is 1 in Float32; onto a prefill of 2^24, one rounding gives 2^24 + 2 and
+#            a rounding through Float32 S gives 2^24 (a tie again).
+# Signs alternate by fibre.  The prefills are chosen so that rounding op(out, S) once and rounding op(out, round(S)) differ.
+ROUND_ONCE = {F16: ((32768.0, 16.0, 2.0 ** -10), (-2.0 ** -10, 0.0, 2.0 ** -10, -2.0 ** -9)),
+              F32: ((1.0, 0.0, 2.0 ** -27), (2.0 ** 24, 2.0 ** 24 + 4, 0.0))}
+
+
+def round_once_input(dt, inner, red, outer):
+    big, mid, tiny = ROUND_ONCE[dt][0]
+    sgn = np.where(np.arange(inner * outer) % 2 == 0, 1.0, -1.0).reshape((inner, outer), order="F")
+    x = np.zeros((inner, red, outer))
+    x[:, 0, :], x[:, red // 2, :], x[:, red - 1, :] = big * sgn, mid * sgn, tiny * sgn
+    return np.asfortranarray(x.astype(NP[dt]))
+
+
+def round_once_prefill(dt, S):
+    """Prefills relative to the sign of S (see ROUND_ONCE), in turn."""
+    o = np.asarray(ROUND_ONCE[dt][1])
+    return (o[np.arange(S.size) % len(o)] * np.where(S < 0, -1.0, 1.0)).astype(NP[dt])
+
+
+@pytest.mark.parametrize("dt", [F32, F16], ids=["f32", "f16"])
+@pytest.mark.parametrize("name", list(shape_table(F32, 132)))
+def test_reducedim_rounds_once(dab, rt1, name, dt):
+    """Float SUM with accumulate = 0 and 1 on every launch_rdim branch: the result is S rounded once, and op(out, S) rounded once."""
+    sm = rt1.device_info()["sm_count"]
+    inner, red0, outer, off = shape_table(dt, sm)[name]
+    T = NP[dt]
+    es = np.dtype(T).itemsize
+    red = max(red0, 3)                                            # room for the three values; the branch stays the same
+    m = model_rdim(dt, inner, red, outer, (off * es) % 16, sm)
+    assert m == model_rdim(dt, inner, red0, outer, (off * es) % 16, sm), (name, m)
+    x = round_once_input(dt, inner, red, outer)
+    xd = Dev(rt1, x, off)
+    bad = []
+    try:
+        for mapc in (MAP_ID, MAP_ABS, MAP_NEG):
+            S = ref_reduce(ref_map(x, mapc), SUM, axis=1, wide=True).reshape(-1, order="F")
+            want0 = S.astype(T)
+            pre = round_once_prefill(dt, S)
+            want1 = (pre.astype(np.float64) + S).astype(T)
+            twice = (pre.astype(np.float64) + S.astype(T).astype(np.float64)).astype(T)
+            if dt == F16:
+                assert not (S.astype(np.float32).astype(T) == want0).any(), "the data does not tell one rounding from two"
+            assert (twice != want1).sum() >= S.size // len(ROUND_ONCE[dt][1]), "the prefills do not tell one rounding from two"
+            out = Dev(rt1, np.zeros(inner * outer, dtype=T), 0)
+            try:
+                nl = rdim_call(rt1, dt, SUM, mapc, xd, inner, red, outer, out, 0)
+                got = out.get()
+                if not HOSTMEM:
+                    assert nl == m["launches"], (mapc, nl, m)
+                if not same_bits(got, want0):
+                    idx = first_bad(got, want0)
+                    bad.append(f"map={mapc} acc=0 first bad outputs {idx.tolist()}: got {got[idx].tolist()} want {want0[idx].tolist()}")
+                out.put(pre)
+                rdim_call(rt1, dt, SUM, mapc, xd, inner, red, outer, out, 1)
+                got = out.get()
+                if not same_bits(got, want1):
+                    idx = first_bad(got, want1)
+                    bad.append(f"map={mapc} acc=1 first bad outputs {idx.tolist()}: got {got[idx].tolist()} want {want1[idx].tolist()} "
+                               f"(prefill {pre[idx].tolist()}; op(out, round(S)) = {twice[idx].tolist()})")
+            finally:
+                out.free()
+    finally:
+        xd.free()
+    assert not bad, f"{name} {np.dtype(T).name} {m}: " + "; ".join(bad)
+
+
+def test_reduce_f16_rounds_once(dab, rt1):
+    """dab_reduce of Float16 round-once fibres at every size and head offset of test_reduce_exact: the slot holds S rounded once to
+    Float16 and the exact fp64 carrier S."""
+    slot = Dev(rt1, np.zeros(16, dtype=np.uint8), 0)
+    bad = []
+    try:
+        for n in reduce_sizes(F16):
+            if n < 3:
+                continue
+            for off in (0, 1, 7) if n < 10000 else (0, 1):
+                if n == 8 and off == 0:                       # one 16-byte vector: all eight values share one Float32 tile
+                    continue
+                x = round_once_input(F16, 1, n, 1).reshape(-1)
+                xd = Dev(rt1, x, off)
+                try:
+                    for mapc in (MAP_ID, MAP_ABS, MAP_NEG):
+                        S = float(ref_reduce(ref_map(x, mapc), SUM, axis=0, wide=True))
+                        s = reduce_call(rt1, F16, SUM, mapc, xd, n, slot)
+                        got, carrier = slot_value(s, np.dtype(np.float16)), s[8:16].view(np.float64)[0]
+                        if got != np.float16(S) or carrier != S:
+                            bad.append(f"n={n} off={off} map={mapc}: got {got!r} carrier {carrier!r}, want {np.float16(S)!r} carrier {S!r}")
+                finally:
+                    xd.free()
+    finally:
+        slot.free()
+    assert not bad, "; ".join(bad[:12]) + f" ({len(bad)} cases)"
+
+
+PRED_MAPS = range(16, 24)                # EQ NE LT LE GT GE ISNAN NONZERO
+
+
+@pytest.mark.parametrize("n", [1, 9, 8193, (1 << 20) + 5])
+def test_reduce_f16_predicates(dab, rt1, n):
+    """COUNT / ANY / ALL of Float16 data through every predicate map, with Float16 parameters (signed zeros, a subnormal, 65504, Inf,
+    NaN): compared in Float32, which is exact for Float16 operands, so NumPy's Float16 comparisons are the reference."""
+    rng = np.random.default_rng(n)
+    x = rng.integers(0, 1 << 16, n).astype(np.uint16).view(np.float16)             # every kind of bit pattern, NaN payloads included
+    specials = np.asarray([0.0, -0.0, 2.0 ** -24, 65504.0, -np.inf, np.nan, 1.5], dtype=np.float16)
+    params = [np.float16(v) for v in (0.0, -0.0, 2.0 ** -24, 65504.0, np.inf, np.nan, 1.5)]
+    slot = Dev(rt1, np.zeros(16, dtype=np.uint8), 0)
+    bad = []
+    try:
+        for off in (0, 3):
+            xs = x.copy()
+            for k, p in enumerate(edge_positions(n, min((8 - off) % 8, n), 8, 1)):
+                xs[p] = specials[k % len(specials)]
+            xd = Dev(rt1, xs, off)
+            try:
+                for mapc in PRED_MAPS:
+                    for p in (params if mapc < 22 else params[:1]):
+                        with np.errstate(invalid="ignore"):
+                            m = {16: xs == p, 17: xs != p, 18: xs < p, 19: xs <= p, 20: xs > p, 21: xs >= p, 22: np.isnan(xs), 23: xs != 0}[mapc]
+                        pa = np.asarray([p], dtype=np.float16)
+                        for op, want in ((COUNT, int(m.sum())), (ANY, int(m.any())), (ALL, int(m.all()))):
+                            _lib().call("dab_reduce", rt1.ctx, F16, op, mapc, C.c_void_p(pa.ctypes.data), C.c_void_p(xd.ptr), n, C.c_void_p(slot.ptr))
+                            got = int(slot.get(16, np.uint8)[:8].view(np.int64)[0])
+                            if got != want:
+                                bad.append(f"off={off} map={mapc} param={p!r} op={op}: got {got} want {want}")
+            finally:
+                xd.free()
+    finally:
+        slot.free()
+    assert not bad, "; ".join(bad[:12]) + f" ({len(bad)} cases)"
 
 
 # ---------------------------------------------------------------------------------------------------------- (c) the fused step

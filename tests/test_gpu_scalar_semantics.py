@@ -21,7 +21,8 @@ pytestmark = pytest.mark.gpu
 
 HOSTMEM = os.environ.get("DAB_HOSTMEM") == "1"
 F32, F64, I32, I64, U8 = range(5)
-CODE = {"f32": F32, "f64": F64, "i32": I32, "i64": I64, "bool": U8}
+F16 = 8
+CODE = {"f32": F32, "f64": F64, "i32": I32, "i64": I64, "bool": U8, "f16": F16}
 MAP_ID, MAP_ABS, MAP_ABS2, MAP_NEG, MAP_SQRT, MAP_INV, MAP_FLOOR, MAP_CEIL, MAP_SIGN = range(9)
 ADD, SUB, MUL, DIV, REM, BMAX, BMIN, MOD, IDIV, AND, OR, XOR = range(12)
 UNARY = {MAP_ID: None, MAP_ABS: "abs", MAP_ABS2: "abs2", MAP_NEG: "neg", MAP_SQRT: "sqrt", MAP_INV: "inv", MAP_FLOOR: "floor",
@@ -33,6 +34,10 @@ INT_OPS = (ADD, SUB, MUL, REM, BMAX, BMIN, MOD, IDIV, AND, OR, XOR)
 GUARD = 64                                                   # elements of sentinel before and after every output
 SENTINEL = 0xA5
 TAGS = ("f32", "f64", "i32", "i64")
+
+if HOSTMEM:                                                     # the Float16 code of the host-memory emulation
+    import f16_hostmem
+    f16_hostmem.install()
 
 
 def _lib():
@@ -54,7 +59,7 @@ def same_bits(got, want):
     nan = np.isnan(want)
     if not np.array_equal(np.isnan(got), nan):
         return False
-    u = {4: np.uint32, 8: np.uint64}[got.dtype.itemsize]
+    u = {2: np.uint16, 4: np.uint32, 8: np.uint64}[got.dtype.itemsize]
     return np.array_equal(got.view(u)[~nan], want.view(u)[~nan])
 
 
@@ -224,14 +229,16 @@ def test_dab_binary_scalar_both_sides(dab, rt1, t):
 # ------------------------------------------------------------------------------------------------- NVRTC kernels
 def bc_variant(shape, out_strides, out_ptr, out_size, args):
     """The host predicate of ``dab_broadcast_expr`` (dab_jit.cu): which of linear / rows / general runs.  args: (ptr, strides, elem size)
-    per array argument."""
+    per array argument.  The linear kernel steps ``lw`` elements per thread (``lin_width``): 8 when the output or an argument is Float16
+    (the only 2-byte element type), else 4, and needs every pointer aligned to lw elements; the rows kernel always steps 4."""
     dense, acc = [], 1
     for d in range(4):
         dense.append(acc)
         acc *= shape[d]
-    linear = all(not (shape[d] > 1 and out_strides[d] != dense[d]) for d in range(4)) and out_ptr % (4 * out_size) == 0
+    lw = 8 if 2 in [out_size] + [es for _, _, es in args] else 4
+    linear = all(not (shape[d] > 1 and out_strides[d] != dense[d]) for d in range(4)) and out_ptr % (lw * out_size) == 0
     for ptr, st, es in args:
-        if any(shape[d] > 1 and st[d] != dense[d] for d in range(4)) or ptr % (4 * es):
+        if any(shape[d] > 1 and st[d] != dense[d] for d in range(4)) or ptr % (lw * es):
             linear = False
     if linear:
         return "linear"
@@ -250,7 +257,7 @@ def run_bc(rt, src, out_tag, n0, n1, out_ld, out_off, args):
     """Run one NVRTC kernel on an (n0, n1) box.  args: list of (logical 2-D values of shape (n0, n1) or (1, n1), element offset, leading
     dimension).  Returns (values in the box, variant)."""
     L = _lib()
-    odt = np.dtype(jl.NPT[out_tag])
+    odt = np.dtype(np.float16 if out_tag == "f16" else jl.NPT[out_tag])
     out = Buf(rt, odt, out_ld * (n1 - 1) + n0, out_off)
     bufs, ptrs, strides, dts, scal, spec = [], [], [], [], [], []
     for v, off, ld in args:
@@ -266,7 +273,7 @@ def run_bc(rt, src, out_tag, n0, n1, out_ld, out_off, args):
             st[0] = 1
         ptrs.append(b.ptr)
         strides += st
-        dts.append(CODE[jl.tag(v.ravel()[0])])
+        dts.append(CODE["f16" if v.dtype == np.float16 else jl.tag(v.ravel()[0])])
         scal.append(0)
         spec.append((b.ptr, st, v.dtype.itemsize))
     shape = [n0, n1, 1, 1]
@@ -366,6 +373,54 @@ def test_nvrtc_unary_matches_handwritten(dab, rt1, t):
             assert same_bits(got[:, 0], jl.table1(UNARY[c], g)[idx].astype(T)), (t, UNARY[c])
         x.free()
         y.free()
+
+
+def bc16_layouts():
+    """(label, n0, n1, out_ld, out_off, [(off, ld, extruded)] per argument) for Float16 kernels, whose linear kernel steps 8 elements.  The
+    element offsets 2 / 4 / 8 of the second argument give the same variant for a 2- and an 8-byte element: 4 or 16 bytes (general), 8 or
+    32 bytes (rows: 4-aligned, but not 8-aligned as the linear kernel needs) and 16 or 64 bytes (linear)."""
+    out = []
+    for n in (1, 7, 8, 9, 4095, 4096, 4097, 2 * 4096 - 3, 3 * 4096 + 5, 8 * 4096 + 4):      # n % 8 != 0, both sides of 4096 k
+        out.append(("linear", n, 1, n, 0, [(0, n, False), (8, n, False)]))
+    out.append(("rows", 4100, 1, 4100, 0, [(0, 4100, False), (4, 4100, False)]))     # second argument 4 elements in: not 8-aligned
+    out.append(("rows", 4100, 1, 4100, 4, [(0, 4100, False), (8, 4100, False)]))     # the output 4 elements in
+    out.append(("rows", 64, 9, 72, 0, [(0, 72, False), (8, 80, False)]))             # padded leading dimensions
+    out.append(("general", 4100, 1, 4100, 0, [(0, 4100, False), (2, 4100, False)]))  # second argument 2 elements in
+    out.append(("general", 4097, 1, 4097, 1, [(1, 4097, False), (1, 4097, False)]))
+    out.append(("general", 63, 7, 63, 0, [(0, 63, False), (0, 1, True)]))            # shape[0] % 4 != 0, second argument extruded
+    return out
+
+
+F16_BC = [  # (argument tags, output tag, traced closure, NumPy model on (Float16 x, y))
+    (["f16", "f16"], "f16", lambda a, b: a * b + a, lambda a, b: a * b + a),                          # every operation rounded to Float16
+    (["f16", "f64"], "f16", lambda a, y: a * y, lambda a, y: (a.astype(np.float64) * y).astype(np.float16)),   # Float64, rounded once
+    (["f16", "f16"], "f32", lambda a, b: a - b, lambda a, b: (a - b).astype(np.float32)),              # Float16, widened exactly
+]
+
+
+@pytest.mark.parametrize("case", range(len(F16_BC)), ids=["f16-f16", "f16-f64-to-f16", "f16-to-f32"])
+def test_nvrtc_float16_every_variant(dab, rt1, case):
+    """The linear, rows and general broadcast kernels with Float16 operands against NumPy's Float16 arithmetic, bit for bit, on random bit
+    patterns (NaN, Inf, subnormals, signed zeros).  The guard bands of every output check that the 16-byte stores of the 8-element step
+    stop at n."""
+    bc = _bc()
+    tags, out_tag, f, model = F16_BC[case]
+    src = bc.codegen(bc.convert(bc.trace(f, tags), out_tag))
+    rng = np.random.default_rng(case)
+    reached = set()
+    for k, (label, n0, n1, out_ld, out_off, specs) in enumerate(bc16_layouts()):
+        x = rng.integers(0, 1 << 16, (n0, n1)).astype(np.uint16).view(np.float16)
+        if tags[1] == "f16":
+            y = rng.integers(0, 1 << 16, (1 if specs[1][2] else n0, n1)).astype(np.uint16).view(np.float16)
+        else:
+            y = rng.standard_normal((1 if specs[1][2] else n0, n1)) * np.exp2(rng.integers(-30, 20, (1 if specs[1][2] else n0, n1)))
+        got, variant = run_bc(rt1, src, out_tag, n0, n1, out_ld, out_off, [(x, specs[0][0], specs[0][1]), (y, specs[1][0], specs[1][1])])
+        assert variant == label, (k, label, variant)
+        reached.add(variant)
+        with np.errstate(all="ignore"):
+            want = np.asarray(model(x, np.broadcast_to(y, x.shape)))
+        assert same_bits(got, want), (tags, out_tag, label, (n0, n1), first_bad(got.ravel("F"), want.ravel("F")))
+    assert reached == {"linear", "rows", "general"}
 
 
 MIXED = [(a, b) for a in ("bool", "i32", "i64", "f32", "f64") for b in ("bool", "i32", "i64", "f32", "f64")]
