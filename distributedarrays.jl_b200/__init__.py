@@ -5,7 +5,8 @@ loader shim).  The public names mirror DistributedArrays.jl's for this path: ``D
 ``localindices``, ``locate``, ``makelocal``, ``procs``, ``dzeros/dones/dfill/drand``, ``map`` (``map_``), ``map!``
 (``map_inplace``), broadcast (``broadcast`` / ``broadcast_into``), ``reduce``, ``mapreduce``, ``sum``, ``prod``,
 ``maximum``, ``minimum``, ``all``, ``any``, ``count``, ``extrema``, ``findmax`` / ``findmin`` / ``argmax`` / ``argmin`` (with and without
-``dims``), ``sort`` and ``sortperm`` of a DVector (``sortperm(d; sample, by)``: stable, 1-based, the layout of ``sort``),
+``dims``), ``sort`` and ``sortperm`` of a DVector (``sortperm(d; sample, by)``: stable, 1-based, the layout of ``sort``) and along a
+dimension (``sortperm(A; dims, by)``: 1-based global linear indices per fibre, stable; ``sort(A; dims, by)``; segmented sorts on the GPU),
 ``mapslices`` (with ``sort``, ``svdvals``, ``eigvals``, reductions,
 elementwise and constant slice functions), ``ppeval`` (batched slice products ``ppeval(operator.matmul, A, B)``, ``eigvals`` of symmetric
 slices, and every ``mapslices`` slice function), ``cumsum`` / ``cumprod`` / ``accumulate`` and their ``!`` forms

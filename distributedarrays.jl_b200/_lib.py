@@ -22,6 +22,7 @@ MAP_EQ, MAP_NE, MAP_LT, MAP_LE, MAP_GT, MAP_GE, MAP_ISNAN, MAP_NONZERO = range(1
 FINDMAX, FINDMIN = range(2)                   # which of dab_findminmax / dab_findminmax_dim / dab_combine_findminmax
 ADD, SUB, MUL, DIV, REM, BMAX, BMIN, MOD, IDIV, AND, OR, XOR = range(12)
 SORT_SLICES_SMEM_LEN = 8192                   # longest fibre dab_sort_slices sorts in shared memory
+SORTPERM_SLICES_SMEM_LEN = 4096               # longest fibre dab_sortperm_slices sorts in shared memory
 SVDVALS_MAX_K, SVDVALS_MAX_ELEMS = 32, 4096   # dab_svdvals_batched serves min(m, n) <= 32 and m * n <= 4096
 EIGVALS_SYM_MAX_N = 64                        # dab_eigvals_sym_batched serves n <= 64
 COMPACT_TILE, COMPACT_INDEX = 4096, 0          # dab_compact_count / dab_compact: tile length, index mode
@@ -131,6 +132,7 @@ _SIGS = {
     "dab_sort_pairs": (_i32, [_vp, _i32, _vp, _vp, _vp, C.c_int64, _vp, _vp, _sz, _sz]),
     "dab_sort_pairs_scratch_bytes": (_i32, [_i32, _sz, C.POINTER(_sz)]),
     "dab_sort_slices": (_i32, [_vp, _i32, _vp, _vp, _sz, _sz, _sz]),
+    "dab_sortperm_slices": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp]),
     "dab_svdvals_batched": (_i32, [_vp, _i32, _vp, _sz, _sz, _sz, _vp, _vp]),
     "dab_matmul_batched": (_i32, [_vp, _i32, _sz, _sz, _sz, _vp, _sz, _vp, _sz, _vp, _sz]),
     "dab_eigvals_sym_batched": (_i32, [_vp, _i32, _vp, _sz, _sz, _vp, _vp]),

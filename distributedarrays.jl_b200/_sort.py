@@ -40,6 +40,16 @@ _SORT_DTYPES = (np.dtype(np.float32), np.dtype(np.float64), np.dtype(np.int32), 
 SAMPLE_SIZE_ON_WORKER = 512                                    # src/sort.jl:69
 
 
+class _SampleDefault:
+    """``sample`` not given: ``true`` for a DVector; told apart from an explicit ``sample``, which is refused together with ``dims``."""
+
+    def __repr__(self):
+        return "true"
+
+
+_SAMPLE_DEFAULT = _SampleDefault()
+
+
 def _typemin(dt):
     return -np.inf if dt.kind == "f" else np.iinfo(dt).min
 
@@ -187,12 +197,16 @@ def sort_exchange_plan(pids, sizes, rank_of, my_rank: int):
     return plan
 
 
-def sort(d: DArray, sample=True, by=None, alg=None, **kwargs) -> DArray:  # noqa: A001 - mirrors Base.sort
+def sort(d: DArray, sample=_SAMPLE_DEFAULT, by=None, alg=None, dims=None, **kwargs) -> DArray:  # noqa: A001 - mirrors Base.sort
     """``sort(d::DVector; sample=true, alg, by)`` (reference src/sort.jl:107-170).  ``sample``: True (<= 512 sampled keys per
     worker balance the parts), False (uniform between min(d) and max(d)), a ``(min, max)`` tuple, or an array used as the sample.
     ``by``: a traceable key function (same closures as broadcast / map); values are ordered stably by ``by(x)``.
     ``alg`` is accepted and ignored: a keys-only sort has one result whatever the algorithm, and the keyed sort is stable like
-    Julia's default.  Called on the slice of ``mapslices(sort, D; dims)`` it stands for the per-slice sort (``dab_sort_slices``)."""
+    Julia's default.  Called on the slice of ``mapslices(sort, D; dims)`` it stands for the per-slice sort (``dab_sort_slices``).
+
+    ``sort(A; dims=d)`` (1-based ``d``) sorts every fibre of ``A`` along ``d``: the values and the layout of ``mapslices(sort, A, dims=d)``,
+    bit for bit.  With ``by = f`` the values of every fibre are put in the stable ``isless`` order of their keys ``f.(A)`` (K26,
+    ``dab_sortperm_slices``), in the same layout.  A DVector with ``dims=1`` is ``sort(v)``.  Only ``by`` and ``alg`` go with ``dims``."""
     from ._sparse import SparseDArray, refuse
     if isinstance(d, SparseDArray):
         refuse("sort")
@@ -200,7 +214,10 @@ def sort(d: DArray, sample=True, by=None, alg=None, **kwargs) -> DArray:  # noqa
     if isinstance(d, Expr):
         from . import _slices
         if _slices.tracing():
-            return _slices.sort_of_slice(d, by, kwargs)
+            return _slices.sort_of_slice(d, by, kwargs if dims is None else dict(kwargs, dims=dims))
+    if dims is not None:
+        return _sort_dims(d, dims, by, sample, kwargs, perm=False)
+    sample = True if sample is _SAMPLE_DEFAULT else sample
     if isinstance(d, DArray) and d.dtype.kind == "c" and by is None:
         raise TypeError(f"MethodError: no method matching isless(::{d.dtype}, ::{d.dtype}) -- complex numbers are not ordered")
     return sort_with_boundaries(d, sample, by, alg, **kwargs)[0]
@@ -213,16 +230,27 @@ def sort_with_boundaries(d: DArray, sample=True, by=None, alg=None, **kwargs):
     return _samplesort(d, d.chunks, d.dtype, presample, kf, perm=False)
 
 
-def sortperm(d: DArray, sample=True, by=None, alg=None, **kwargs) -> DArray:
+def sortperm(d: DArray, sample=_SAMPLE_DEFAULT, by=None, alg=None, dims=None, **kwargs) -> DArray:
     """``sortperm(d::DVector; sample=true, by)``: the DVector of Int64 with ``d[p]`` sorted -- Julia's ``sortperm(Array(d))``, 1-based
     global indices in ``isless`` order, STABLE (equal keys, and all NaNs, keep ascending index order).  The samplesort of ``sort``
     with K21 (``dab_sort_pairs``) carrying every key's global index: chunk j of the result indexes the elements in chunk j of
     ``sort(d; sample)``, the layout is the same.  (Only when the reference's scan would leave NaNs ahead of larger keys, so that
     ``sort(d)`` itself is out of ``isless`` order, are the NaNs moved to the last receiving piece and the chunk sizes differ.)
-    ``by = f``: ``sortperm(f.(d))``, with ``sample`` in key space.  ``alg`` is accepted and ignored (one stable result)."""
+    ``by = f``: ``sortperm(f.(d))``, with ``sample`` in key space.  ``alg`` is accepted and ignored (one stable result).
+
+    ``sortperm(A; dims=d)`` (1-based ``d``): a ``DArray{Int64}`` of ``A``'s dims in which every fibre along ``d`` holds, at rank r, the
+    1-based global column-major LINEAR index into ``A`` of the fibre element of rank r -- Julia >= 1.9's ``sortperm(A; dims)``, the
+    ``LinearIndices(A)`` convention of ``findmax(A; dims)``.  Stable ``isless`` order: equal keys keep ascending index order, -0.0 sorts
+    before +0.0, NaNs go last in input order.  ``by = f`` is ``sortperm(f.(A); dims)`` (a Bool key orders as 0 / 1).  The layout is
+    ``sort(A; dims)``'s (that of ``mapslices(sort, A, dims=d)``), so ``A[sortperm(A; dims)]`` equals ``sort(A; dims)`` element for
+    element -- except inside a run of NaNs with different payloads, which ``sort`` orders by bits and ``sortperm`` keeps in input
+    order.  A DVector with ``dims=1`` is ``sortperm(v)``.  Only ``by`` and ``alg`` go with ``dims``."""
     from ._sparse import SparseDArray, refuse
     if isinstance(d, SparseDArray):
         refuse("sortperm")
+    if dims is not None:
+        return _sort_dims(d, dims, by, sample, kwargs, perm=True)
+    sample = True if sample is _SAMPLE_DEFAULT else sample
     if isinstance(d, DArray) and d.dtype.kind == "c" and by is None:
         raise TypeError(f"MethodError: no method matching isless(::{d.dtype}, ::{d.dtype}) -- complex numbers are not ordered")
     kf, pids = _check_args(d, sample, by, kwargs, "sortperm")
@@ -450,3 +478,103 @@ def _samplesort(d: DArray, src: Dict[int, B200Array], dt: np.dtype, presample, k
         chunks[pids[j]] = out
     layout = layout_from_chunk_shapes([(totals[j],) for j in keep], (len(keep),), [pids[j] for j in keep])
     return DArray(layout, np.int64 if perm else dt, chunks, rt), boundaries
+
+
+# ---- sort(A; dims) / sortperm(A; dims): segmented sorts of the fibres along one dimension ----------------------------------------------
+
+_CHUNK_LIMIT_LONG = 0xFFFFF000                                 # K21's bound, which K26's long-fibre passes inherit
+
+
+def check_dims(dims, ndim: int, what: str) -> int:
+    """``dims`` of ``sort`` / ``sortperm``: a Python or NumPy integer (not a Bool) in ``1:ndim``."""
+    if isinstance(dims, (bool, np.bool_)) or not isinstance(dims, (int, np.integer)) or not 1 <= int(dims) <= ndim:
+        raise _lib.ArgumentError(_lib.ERR_ARG, f"{what}: dims = {dims!r} is not a dimension of a {ndim}-dimensional DArray (an integer in 1:{ndim})")
+    return int(dims)
+
+
+def _check_dims_args(A, dims, by, sample, kwargs, what: str):
+    """Every refusal of ``sort`` / ``sortperm`` with ``dims``, before anything is allocated or launched: (dim, traced ``by`` or None)."""
+    from ._darray import SubDArray, refuse_float16
+    if isinstance(A, SubDArray):
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what}(view; dims) is not served: make it a DArray first (DArray(view))")
+    if sample is not _SAMPLE_DEFAULT or kwargs:
+        given = (["sample"] if sample is not _SAMPLE_DEFAULT else []) + sorted(kwargs)
+        raise _lib.ArgumentError(_lib.ERR_ARG, f"Only `alg`, `by` and `dims` are supported as keyword arguments with `dims` (got {', '.join(given)})")
+    dim = check_dims(dims, A.ndim, what)
+    dt = A.dtype
+    if dt.kind == "c":
+        if by is None:
+            raise TypeError(f"MethodError: no method matching isless(::{dt}, ::{dt}) -- complex numbers are not ordered")
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what}(A; dims, by) of a {dt} DArray is not served (no complex values are moved)")
+    refuse_float16(what, A)
+    if dt not in _SORT_DTYPES:
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what}: eltype {dt} (served: Float32 Float64 Int32 Int64)")
+    kf = _KeyFn(A.rt, by, dt) if by is not None else None       # traced before any launch: an untraceable `by` raises here
+    if kf is not None and kf.kdt not in _SORT_DTYPES:
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what}: keys of type {kf.kdt} (served: Float32 Float64 Int32 Int64)")
+    if A.ndim > 8:
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what} with dims over more than 8 dimensions is not served")
+    return dim, kf
+
+
+def _sort_dims(A, dims, by, sample, kwargs, perm: bool) -> DArray:
+    """``sort(A; dims, by)`` / ``sortperm(A; dims, by)``.  Checks, then the working layout of ``mapslices(..., dims)`` (A's own when the
+    dimension is whole on every worker, else the reference's redistribution ``p``), then one K26 launch per local chunk."""
+    what = "sortperm" if perm else "sort"
+    dim, kf = _check_dims_args(A, dims, by, sample, kwargs, what)
+    if A.ndim == 1:                                             # a DVector: the samplesort, in its own layout
+        return sortperm(A, by=by) if perm else sort(A, by=by)
+    if not perm and kf is None:                                 # mapslices(sort, A, dims): K13 and the reference's redistribution
+        from ._slices import mapslices
+        return mapslices(sort, A, dims=dim)
+    from . import _slices
+    from .layout import make_layout, rlen, shape_of
+    p = _slices.redistribution_grid(A.dims, A.layout.grid, (dim,), len(A.layout.pids))
+    L = A.layout if p is None else make_layout(A.dims, list(A.layout.pids), p)
+    if any(rlen(r) == 0 for I in L.indices for r in I):
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what} with dims over a DArray with an empty localpart is not served")
+    shapes = [shape_of(I) for I in L.indices]
+    if A.dims[dim - 1] > _lib.SORTPERM_SLICES_SMEM_LEN and any(int(np.prod(s)) >= _CHUNK_LIMIT_LONG for s in shapes):
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what} with dims: chunks of 2^32 - 4096 or more elements with fibres longer "
+                                    f"than {_lib.SORTPERM_SLICES_SMEM_LEN} are not served")
+    layout = layout_from_chunk_shapes(shapes, L.grid, L.pids)
+    rt = A.rt
+    W = A if p is None else _slices._redistribute(A, p)
+    odt = np.dtype(np.int64) if perm else A.dtype
+    chunks: Dict[int, B200Array] = {}
+    try:
+        for pid, ch in W.chunks.items():
+            I = L.indices[L.pids.index(pid)]
+            out = B200Array.empty(rt, ch.shape, odt)
+            chunks[pid] = out
+            keys = kf.keys_of(ch) if kf is not None else ch
+            try:
+                sortperm_slices_chunk(rt, keys, [r[0] - 1 for r in I], A.dims, dim, out if perm else None, None if perm else (ch, out))
+            finally:
+                if keys is not ch:
+                    keys.free()
+    except BaseException:
+        for out in chunks.values():
+            out.free()
+        raise
+    finally:
+        if W is not A:
+            W.close()
+    return DArray(layout, odt, chunks, rt)
+
+
+def sortperm_slices_chunk(rt, keys: B200Array, lo, gdims, dim: int, perm_out, vals):
+    """One K26 launch: ``perm_out`` (Int64, the chunk's shape) gets the global indices; with ``vals = (src, dst)`` the values of ``src`` go
+    to ``dst`` in the same order (then ``perm_out`` may be None: the indices go to a temporary)."""
+    N = keys.ndim
+    SZ = C.c_size_t * N
+    tmp = B200Array.empty(rt, keys.shape, np.int64, temp=True) if perm_out is None else None
+    P = perm_out if perm_out is not None else tmp
+    try:
+        src, dst = vals if vals is not None else (None, None)
+        _lib.call("dab_sortperm_slices", rt.ctx, dab_dtype(keys.dtype), C.c_void_p(keys.ptr), N, SZ(*keys.shape), SZ(*lo), SZ(*gdims), dim,
+                  C.c_void_p(P.ptr), src.dtype.itemsize if src is not None else 0, C.c_void_p(src.ptr if src is not None else None),
+                  C.c_void_p(dst.ptr if dst is not None else None))
+    finally:
+        if tmp is not None:
+            tmp.free()

@@ -521,6 +521,22 @@ int32_t dab_sorted_split(dab_ctx* ctx, int32_t dtype, const void* sorted, size_t
  * other overlaps are not allowed.  Scratch of the long-fibre path comes from the ctx block cache.  dtypes: F32 F64 I32 I64. */
 int32_t dab_sort_slices(dab_ctx* ctx, int32_t dtype, const void* in, void* out, size_t inner, size_t len, size_t outer);
 
+/* ==== sortperm along a dimension K26 (row f15) ============================================
+ * The  sortperm(A; dims=dim)  of one chunk in which dimension dim (1-based) is whole.  The chunk (ndim <= 8 column-major dims chunk_dims,
+ * first global index chunk_lo[k], 0-based, in an array of global_dims) is collapsed to (inner, len, outer) around dim.  For every fibre
+ * (i, o) and rank r < len:  perm[i + inner*(r + len*o)] = the 1-based global column-major linear index of the fibre element of rank r in
+ * the stable isless order of keys (-0.0 < 0.0; NaNs last, equal to each other, so they keep their input order) -- Julia's
+ * sortperm(A; dims) entries, LinearIndices(A).  With vals / vals_out (both or neither; val_bytes 4 or 8) that element's value is moved
+ * to the same place of vals_out, as bytes.  Fibres of len <= DAB_SORTPERM_SLICES_SMEM_LEN are sorted in shared memory by a bitonic
+ * network over (radix key, position) pairs; longer fibres take two chunk-wide stable K21 passes (by key, then by fibre id) whatever the
+ * number of fibres, with scratch from the ctx block cache, and need a chunk of fewer than 2^32 - 4096 elements (otherwise
+ * DAB_ERR_UNSUPPORTED).  DAB_ERR_ARG: chunk_dims[dim-1] != global_dims[dim-1], a chunk outside the array, or a NULL pointer;
+ * DAB_ERR_UNSUPPORTED: key dtypes other than F32 F64 I32 I64, ndim > 8.  keys and vals are only read; perm / vals_out must not overlap
+ * them.  An empty chunk launches nothing.  Asynchronous on the ctx stream. */
+#define DAB_SORTPERM_SLICES_SMEM_LEN 4096
+int32_t dab_sortperm_slices(dab_ctx* ctx, int32_t key_dtype, const void* keys, int32_t ndim, const size_t* chunk_dims, const size_t* chunk_lo,
+                            const size_t* global_dims, int32_t dim, int64_t* perm, int32_t val_bytes, const void* vals, void* vals_out);
+
 /* Limits of dab_svdvals_batched: min(m, n) and m * n. */
 #define DAB_SVDVALS_MAX_K 32
 #define DAB_SVDVALS_MAX_ELEMS 4096

@@ -23,6 +23,7 @@
 #   src/sort.jl:8,22,61  sort(localpart(d)), sort!(lp)    Base.sort / Base.sort!                     dab_sort
 #   src/sort.jl:8,22,61  sort(localpart(d); by = f)       sort_by (keys = f.(a) by broadcast)        dab_sort_by_key
 #   (Base.sortperm: scalar getindex)  sortperm(localpart(d)), sortperm(d)   Base.sortperm (chunk and DVector methods)   dab_sort_pairs
+#   (Base.sortperm: scalar getindex)  sortperm(A; dims)                    Base.sortperm(::DArray; dims), unverified   dab_sortperm_slices
 #   src/mapreduce.jl:205 mapslices(f, localpart(y), dims) mapslices_sort / svdvals_batched       dab_sort_slices / dab_svdvals_batched
 #   src/mapreduce.jl:315 _ppeval(f, localparts...; dim)   matmul_batched / eigvals_sym_batched  dab_matmul_batched / dab_eigvals_sym_batched
 #   (no reference method)  accumulate!(op, lp, lp; dims)   Base.accumulate! (cumsum! / cumprod!)   dab_scan
@@ -428,6 +429,29 @@ function Base.sortperm(d::DArray{T,1,B200Array{T,1}}; by = identity, kw...) wher
             end for p in procs(d)]
     keys = reduce(vcat, first.(runs)); idx = reduce(vcat, last.(runs))
     distribute(idx[sortperm(keys; alg = Base.Sort.DEFAULT_STABLE)]; procs = procs(d))
+end
+
+# sortperm(localpart(A); dims) with global indices (K26, unverified: no Julia run on a GPU yet): every fibre along `dims` of the chunk at
+# 0-based offset `lo` in an array of size `gdims` gets the 1-based global LinearIndices of its elements in the stable isless order of
+# `keys`; with `vals` the values are moved to the same places.  `dims` must be whole in the chunk.
+function sortperm_slices(keys::B200Array{K,N}, dims::Integer, lo::NTuple{N,Int}, gdims::NTuple{N,Int};
+                         vals::Union{Nothing,B200Array} = nothing) where {K,N}
+    perm = B200Array{Int64,N}(undef, size(keys))
+    vout = vals === nothing ? nothing : similar(vals)
+    check(ccall((:dab_sortperm_slices, libdab), Int32,
+                (Ptr{Cvoid}, Int32, Ptr{Cvoid}, Int32, Ptr{Csize_t}, Ptr{Csize_t}, Ptr{Csize_t}, Int32, Ptr{Cvoid}, Int32, Ptr{Cvoid}, Ptr{Cvoid}),
+                ctx(), dab_dtype(K), keys.ptr, N, Csize_t[size(keys)...], Csize_t[lo...], Csize_t[gdims...], dims, perm.ptr,
+                vals === nothing ? 0 : sizeof(eltype(vals)), vals === nothing ? C_NULL : vals.ptr, vout === nothing ? C_NULL : vout.ptr), ctx())
+    perm, vout
+end
+# sortperm(A::DArray; dims): each worker runs K26 on its localpart when `dims` is whole there (the Python runtime also redistributes as
+# mapslices does when it is split); the result has A's layout.
+function Base.sortperm(A::DArray{T,N,B200Array{T,N}}; dims::Integer, by = identity, kw...) where {T,N}
+    size(A.indices, dims) == 1 || throw(ArgumentError("sortperm(A; dims): dimension dims is split over workers; redistribute first"))
+    DArray(size(A), procs(A), size(A.indices)) do I
+        a = localpart(A)
+        sortperm_slices(by === identity ? a : by.(a), dims, Tuple(first(r) - 1 for r in I), size(A))[1]
+    end
 end
 
 # mapslices(f, localpart(y), dims=z)  (src/mapreduce.jl:205) for f = sort (one dim) and f = svdvals (two dims, slices already packed as
