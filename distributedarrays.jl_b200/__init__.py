@@ -9,7 +9,8 @@ loader shim).  The public names mirror DistributedArrays.jl's for this path: ``D
 dimension (``sortperm(A; dims, by)``: 1-based global linear indices per fibre, stable; ``sort(A; dims, by)``; segmented sorts on the GPU),
 ``mapslices`` (with ``sort``, ``svdvals``, ``eigvals``, reductions,
 elementwise and constant slice functions), ``ppeval`` (batched slice products ``ppeval(operator.matmul, A, B)``, ``eigvals`` of symmetric
-slices, and every ``mapslices`` slice function), ``cumsum`` / ``cumprod`` / ``accumulate`` and their ``!`` forms
+slices, solves ``ppeval(ldiv, A, B)`` (Julia's ``A \\ B``) and determinants ``ppeval(det, A)`` / ``mapslices(det, D, dims)``, and every
+``mapslices`` slice function), ``cumsum`` / ``cumprod`` / ``accumulate`` and their ``!`` forms
 (``cumsum_`` ...), ``Array(d)`` (``to_array``), range ``getindex``, ``d[I]`` with ``I`` a DArray of Int32 / Int64 (a gather on the GPU:
 ``v[sortperm(v)]``, ``A[findmax(A; dims)[2]]``; a DArray key holds Julia's 1-based linear indices, host Python indices stay 0-based),
 logical indexing ``d[mask]`` with a Bool DArray of ``d``'s dims, ``findall(mask)`` / ``findall(f, d)`` (1-based linear indices as a
@@ -27,7 +28,7 @@ Everything computes on the GPU through ``csrc/libdab200.so`` (C ABI: ``include/d
 importing works anywhere, but the first op without the built extension or without an H100 raises.
 """
 from . import _lib
-from ._lib import ArgumentError, DabError, DimensionMismatch, InexactError, UnsupportedError
+from ._lib import ArgumentError, DabError, DimensionMismatch, InexactError, SingularException, UnsupportedError
 from ._broadcast import (Expr, Int128, abs2, broadcast, broadcast_into, ceil, copy, cos, deepcopy, drandn, exp, floor, ifelse, inv, isnan, jl_max, jl_min,
                         log, map_, map_bang, map_inplace, map_localparts, mod, rem, sign, sin, sqrt, tan, tanh, widen)
 from ._broadcast import angle, cis, conj, imag, iszero, real  # noqa: F401 -- complex values (complex(x[, y]) below)
@@ -47,7 +48,7 @@ from ._findmax import argmax, argmin, findmax, findmin
 from ._compact import filter, findall  # noqa: A004
 from ._sort import sort, sort_with_boundaries, sortperm
 from ._scan import accumulate, accumulate_, cumprod, cumprod_, cumsum, cumsum_
-from ._slices import eigvals, mapslices, svdvals
+from ._slices import det, eigvals, ldiv, mapslices, svdvals
 from ._ppeval import ppeval
 from ._sparse import SparseChunk, SparseDArray
 from .runtime import Runtime, init, myid, nworkers, runtime, workers

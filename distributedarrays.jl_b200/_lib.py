@@ -25,6 +25,8 @@ SORT_SLICES_SMEM_LEN = 8192                   # longest fibre dab_sort_slices so
 SORTPERM_SLICES_SMEM_LEN = 4096               # longest fibre dab_sortperm_slices sorts in shared memory
 SVDVALS_MAX_K, SVDVALS_MAX_ELEMS = 32, 4096   # dab_svdvals_batched serves min(m, n) <= 32 and m * n <= 4096
 EIGVALS_SYM_MAX_N = 64                        # dab_eigvals_sym_batched serves n <= 64
+LU_MAX_N = 64                                 # dab_ldiv_batched / dab_det_batched serve n <= 64
+LU_STATUS_CLEAR, LU_STATUS_NONFINITE = (1 << 64) - 1, 0x80   # dab_ldiv_batched's status word: no failure / low byte of a NaN / Inf
 COMPACT_TILE, COMPACT_INDEX = 4096, 0          # dab_compact_count / dab_compact: tile length, index mode
 
 
@@ -51,6 +53,17 @@ class InexactError(DabError, ValueError):
 class UnsupportedError(DabError, NotImplementedError):
     """The op/dtype is not served by a kernel.  The analogue of ``allowscalar(false)`` (reference
     src/darray.jl:638-640): we raise instead of silently computing on the host."""
+
+
+class SingularException(DabError):
+    """Julia ``LinearAlgebra.SingularException``: ``A \\ b`` met an exactly-zero diagonal entry or pivot; ``info`` is its 1-based index."""
+
+    def __init__(self, info: int):
+        super().__init__(ERR_ARG, f"SingularException({int(info)})")
+        self.info = int(info)
+
+    def __str__(self) -> str:
+        return f"SingularException({self.info})"
 
 
 _EXC = {ERR_ARG: ArgumentError, ERR_EMPTY: ArgumentError, ERR_DIM_MISMATCH: DimensionMismatch, ERR_UNSUPPORTED: UnsupportedError}
@@ -136,6 +149,8 @@ _SIGS = {
     "dab_svdvals_batched": (_i32, [_vp, _i32, _vp, _sz, _sz, _sz, _vp, _vp]),
     "dab_matmul_batched": (_i32, [_vp, _i32, _sz, _sz, _sz, _vp, _sz, _vp, _sz, _vp, _sz]),
     "dab_eigvals_sym_batched": (_i32, [_vp, _i32, _vp, _sz, _sz, _vp, _vp]),
+    "dab_ldiv_batched": (_i32, [_vp, _i32, _sz, _sz, _vp, _sz, _vp, _sz, _vp, _sz, _vp]),
+    "dab_det_batched": (_i32, [_vp, _i32, _sz, _vp, _sz, _vp, _sz]),
     "dab_comm_unique_id": (_i32, [_vp]),
     "dab_comm_init_rank": (_i32, [_vp, _vp, _i32, _i32]),
     "dab_comm_destroy": (_i32, [_vp]),

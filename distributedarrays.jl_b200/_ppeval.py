@@ -13,6 +13,8 @@ are.  The served forms:
   ---------------------------------------------  ------------------------------------------------------------------------------------
   ``a @ b`` (Julia's ``*``: ``operator.matmul``,  ``dab_matmul_batched``; a matrix slice times a vector or matrix slice, either operand
   a lambda using ``@``, ``dab.matmul``)           possibly a host array that is broadcast (uploaded once, batch stride 0)
+  ``ldiv(a, b)`` (Julia's ``a \\ b``)             ``dab_ldiv_batched`` (K27); a square matrix slice and a vector or matrix slice, either
+                                                 possibly a broadcast host array; Int32 / Int64 operands are converted to Float64 first
   one sliced argument, any ``mapslices`` slice   the ``mapslices`` chunk code over all dimensions but ``dim`` (``eigvals`` of a square
   function (``eigvals``, ``sort``, ``svdvals``,  slice: ``dab_eigvals_sym_batched``); when ``dim`` is not last, one ``dab_gather_box``
   reductions, elementwise maps, constants)       first moves it last
@@ -32,7 +34,8 @@ import numpy as np
 from . import _lib
 from ._broadcast import SLICE_TRACING, Expr, tag_of
 from ._darray import B200Array, DArray, SubDArray, dab_dtype
-from ._slices import SliceMatmul, _dense_strides, _gather, _is_slice, check_limits, plan_of, raise_on_status, run_chunk
+from ._broadcast import LocalArg, convert, run_local
+from ._slices import SliceLdiv, SliceMatmul, _dense_strides, _gather, _is_slice, check_limits, plan_of, raise_on_status, run_chunk
 from .layout import Layout, layout_from_chunk_shapes, ravel, rlen, unravel
 
 _MATMUL_DTYPES = (np.dtype(np.float32), np.dtype(np.float64), np.dtype(np.int32), np.dtype(np.int64))
@@ -84,13 +87,14 @@ class _MatmulPlan:
         return (self.m,) if self.vec else (self.m, self.n)
 
 
-def _matmul_plan(r: SliceMatmul, slice_shapes: Dict[int, Tuple[int, ...]], dtypes: Dict[int, np.dtype]) -> _MatmulPlan:
+def _operands(r, slice_shapes: Dict[int, Tuple[int, ...]], dtypes: Dict[int, np.dtype], what: str):
+    """The two operands of ``a @ b`` / ``a \\ b``: ``("slice", argument index)`` or ``("host", array)``, with their shapes and eltypes."""
     ops, shapes, dts = [], [], []
     for x in (r.a, r.b):
         if isinstance(x, Expr):
             if not _is_slice(x) or x.val not in slice_shapes:
-                raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "ppeval: a matrix product of an expression of a slice is not served "
-                                            "(multiply the slices themselves)")
+                raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"ppeval: a {what} of an expression of a slice is not served "
+                                            "(pass the slices themselves)")
             ops.append(("slice", x.val))
             shapes.append(slice_shapes[x.val])
             dts.append(dtypes[x.val])
@@ -99,11 +103,15 @@ def _matmul_plan(r: SliceMatmul, slice_shapes: Dict[int, Tuple[int, ...]], dtype
         else:
             a = np.asarray(x)
             if a.dtype == object or a.ndim == 0:
-                raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"ppeval: a matrix product with a {type(x).__name__} is not served")
+                raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"ppeval: a {what} with a {type(x).__name__} is not served")
             ops.append(("host", np.asfortranarray(a)))
             shapes.append(a.shape)
             dts.append(a.dtype)
-    (sa, sb), (ta, tb) = shapes, dts
+    return ops, shapes, dts
+
+
+def _matmul_plan(r: SliceMatmul, slice_shapes: Dict[int, Tuple[int, ...]], dtypes: Dict[int, np.dtype]) -> _MatmulPlan:
+    ops, (sa, sb), (ta, tb) = _operands(r, slice_shapes, dtypes, "matrix product")
     if len(sa) != 2:
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"ppeval: a * b with a of {len(sa)} dimensions; served: a matrix times a vector "
                                     "or a matrix")
@@ -120,6 +128,51 @@ def _matmul_plan(r: SliceMatmul, slice_shapes: Dict[int, Tuple[int, ...]], dtype
     return _MatmulPlan(ops, m, k, 1 if len(sb) == 1 else int(sb[1]), len(sb) == 1, ta)
 
 
+class _LdivPlan:
+    """``a \\ b`` of slices: each operand as in ``_MatmulPlan``; ``dtype`` is the working and result eltype (Float64 for integers)."""
+
+    def __init__(self, ops, n: int, nrhs: int, vec: bool, dtype: np.dtype):
+        self.ops, self.n, self.nrhs, self.vec, self.dtype = ops, n, nrhs, vec, dtype
+
+    def rshape(self) -> Tuple[int, ...]:
+        return (self.n,) if self.vec else (self.n, self.nrhs)
+
+
+def _ldiv_plan(r: SliceLdiv, slice_shapes: Dict[int, Tuple[int, ...]], dtypes: Dict[int, np.dtype]) -> _LdivPlan:
+    ops, (sa, sb), (ta, tb) = _operands(r, slice_shapes, dtypes, "left division")
+    if len(sa) != 2:
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"ppeval: a \\ b with a of {len(sa)} dimensions; served: a square matrix")
+    if len(sb) not in (1, 2):
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"ppeval: a \\ b with b of {len(sb)} dimensions; served: a vector or a matrix")
+    if ta != tb or ta not in _MATMUL_DTYPES:
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"ppeval: a \\ b of eltypes {ta} and {tb} (served: equal Float32 Float64 Int32 "
+                                    "Int64)")
+    m, n = int(sa[0]), int(sa[1])
+    if m != n:
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"ppeval: a \\ b with a of {m}x{n}: the least-squares solution of a non-square "
+                                    "system (Julia's pivoted QR) is not served")
+    if n > _lib.LU_MAX_N:
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"ppeval: a \\ b with a of {n}x{n}; served: n <= {_lib.LU_MAX_N}")
+    if int(sb[0]) != n:
+        raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, f"B has leading dimension {sb[0]}, but needs {n}")
+    wdt = ta if ta.kind == "f" else np.dtype(np.float64)           # lutype(Int) = Float64
+    ops = [(kind, np.asfortranarray(v, dtype=wdt)) if kind == "host" else (kind, v) for kind, v in ops]
+    return _LdivPlan(ops, n, 1 if len(sb) == 1 else int(sb[1]), len(sb) == 1, wdt)
+
+
+def _first_failure(st: np.ndarray, slots, order) -> Tuple[int, ...]:
+    """This rank's first failing ``ldiv`` slice from the status words of ``slots``: ``(order(slot, b)..., info)``, or None."""
+    best = None
+    for slot in slots:
+        w = int(st[slot]) & _lib.LU_STATUS_CLEAR
+        if w == _lib.LU_STATUS_CLEAR:
+            continue
+        low = w & 0xFF
+        cand = order(slot, w >> 8) + (0 if low == _lib.LU_STATUS_NONFINITE else low,)
+        best = cand if best is None or cand < best else best
+    return best
+
+
 def _trace(f, D):
     args = []
     for i, x in enumerate(D):
@@ -131,7 +184,7 @@ def _trace(f, D):
         raise
     except Exception as e:  # noqa: BLE001 - anything f does with the tracers that is not a served form
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"ppeval: {getattr(f, '__name__', f)!r} is not a served slice function "
-                                    f"({type(e).__name__}: {e}); served: a * b (operator.matmul), eigvals, and for one sliced argument "
+                                    f"({type(e).__name__}: {e}); served: a * b (operator.matmul), ldiv, det, eigvals, and for one sliced argument "
                                     "every mapslices slice function") from None
     finally:
         SLICE_TRACING[0] -= 1
@@ -209,6 +262,9 @@ def ppeval(f, *D, dim=None) -> DArray:
     if isinstance(r, SliceMatmul):
         plan = _matmul_plan(r, slice_shapes, dtypes)
         rshape, rdtype = plan.rshape(), plan.dtype
+    elif isinstance(r, SliceLdiv):
+        plan = _ldiv_plan(r, slice_shapes, dtypes)
+        rshape, rdtype = plan.rshape(), plan.dtype
     elif len(sliced) == 1:
         i0 = sliced[0]
         sdims = tuple(range(1, len(slice_shapes[i0]) + 1))
@@ -218,7 +274,7 @@ def ppeval(f, *D, dim=None) -> DArray:
         rshape, rdtype = plan.rshape(pshape0), plan.dtype
     else:
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"ppeval: f of {len(sliced)} sliced DArrays is served for a * b (operator.matmul) "
-                                    "only")
+                                    "and ldiv only")
     # ---- the result layout: DArray(reshape(refs, (sd[1:nd-1]..., sd[end]))) (:320-322)
     out_shapes = [tuple(rshape) + (nlocal[pid],) for pid in pids]
     grid = result_grid(L1.grid, len(rshape) + 1, len(pids))
@@ -230,12 +286,16 @@ def ppeval(f, *D, dim=None) -> DArray:
     chunks: Dict[int, B200Array] = {}
     status = cdev = None
     try:
-        if isinstance(plan, _MatmulPlan):
+        if isinstance(plan, (_MatmulPlan, _LdivPlan)):
             host = {}
             for kind, v in plan.ops:
                 if kind == "host" and id(v) not in host:
                     host[id(v)] = B200Array.from_numpy(rt, v)
                     temps.append(host[id(v)])
+        if isinstance(plan, _LdivPlan):
+            status = B200Array.empty(rt, (max(1, len(D1.chunks)),), np.int64, temp=True)
+        elif isinstance(plan, _MatmulPlan):
+            pass
         elif plan.kind in ("svdvals", "eigvals"):
             status = B200Array.empty(rt, (max(1, len(D1.chunks)),), np.int32, temp=True)
         elif plan.kind == "const" and plan.const.size:
@@ -245,7 +305,7 @@ def ppeval(f, *D, dim=None) -> DArray:
         for slot, (pid, ch1) in enumerate(D1.chunks.items()):
             out = B200Array.empty(rt, out_shapes[pids.index(pid)], rdtype)
             chunks[pid] = out
-            if out.size == 0:
+            if out.size == 0 and not (isinstance(plan, _LdivPlan) and plan.n):     # an empty b still factors A (lu checks it)
                 continue
             nb = nlocal[pid]
             if isinstance(plan, _MatmulPlan):
@@ -259,6 +319,23 @@ def ppeval(f, *D, dim=None) -> DArray:
                 (pa, sa), (pb, sb) = ptrs
                 _lib.call("dab_matmul_batched", rt.ctx, dab_dtype(plan.dtype), plan.m, plan.n, plan.k, C.c_void_p(pa), sa, C.c_void_p(pb), sb,
                           C.c_void_p(out.ptr), nb)
+            elif isinstance(plan, _LdivPlan):
+                ptrs = []
+                for kind, v in plan.ops:
+                    if kind == "host":
+                        ptrs.append((host[id(v)].ptr, 0))
+                        continue
+                    P = _slices_last(rt, D[v].chunks[pid], dim[v], temps)
+                    if P.dtype != plan.dtype:                      # lu of an integer matrix works in Float64
+                        W = B200Array.empty(rt, P.shape, plan.dtype, temp=True)
+                        temps.append(W)
+                        run_local(rt, convert(Expr("arg", (), tag_of(P.dtype), 0), tag_of(plan.dtype)), W, [LocalArg(P, None, tag_of(P.dtype))])
+                        P = W
+                    ptrs.append((P.ptr, P.size // nb))
+                (pa, sa), (pb, sb) = ptrs
+                _lib.call("dab_ldiv_batched", rt.ctx, dab_dtype(plan.dtype), plan.n, plan.nrhs, C.c_void_p(pa), sa, C.c_void_p(pb), sb,
+                          C.c_void_p(out.ptr), nb, C.c_void_p(status.ptr + 8 * slot))
+                ran.append(slot)
             elif plan.kind == "const":
                 c = plan.const
                 _gather(rt, c.dtype.itemsize, out.ptr, _dense_strides(out.shape), cdev.ptr, _dense_strides(c.shape) + [0], out.shape)
@@ -268,7 +345,12 @@ def ppeval(f, *D, dim=None) -> DArray:
                 view = B200Array(rt, out.ptr, plan.out_shape(P.shape), rdtype, own=False)
                 run_chunk(rt, plan, P, view, status.ptr + 4 * slot if status is not None else 0, None, temps)
                 ran.append(slot)
-        if status is not None:
+        if isinstance(plan, _LdivPlan):
+            # slices in the order of the result's last dimension (its global index, then the chunk's place on the grid)
+            slot_pid = list(D1.chunks)
+            raise_on_status(rt, 0, _first_failure(status.to_numpy(), ran, lambda slot, b: (
+                layout.localindices(slot_pid[slot])[-1][0] + b, pids.index(slot_pid[slot]))))
+        elif status is not None:
             st = status.to_numpy()
             raise_on_status(rt, int(np.bitwise_or.reduce(st[ran], initial=0)) if ran else 0)
     except BaseException:

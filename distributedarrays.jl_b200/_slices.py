@@ -16,6 +16,7 @@ and the kernels behind them:
                                                  one ``dab_gather_box`` scatters (k, 1, batch) back; Int32 / Int64 are converted to
                                                  Float64 first, as Julia's ``svdvals`` does
   ``eigvals``, two dimensions, square slices     the same with ``dab_eigvals_sym_batched`` (real symmetric slices; see ``eigvals``)
+  ``det``, two dimensions, square slices         the same with ``dab_det_batched`` (K27), one value per slice
   ``sum/prod/maximum/minimum(g(slice))``, g an   the per-chunk dimensional reduction (``reduce_chunk_dims``); with ``dims=()`` there is
   elementwise traced expression (or identity)    nothing to reduce and it is one elementwise launch of g
   an elementwise expression ``g(slice)``         one elementwise launch (the result has the slice's shape)
@@ -41,8 +42,8 @@ _SORT_DTYPES = (np.dtype(np.float32), np.dtype(np.float64), np.dtype(np.int32), 
 
 
 def tracing() -> bool:
-    """True while ``mapslices`` / ``ppeval`` call ``f`` on slice tracers: ``sort``, ``svdvals``, ``eigvals``, ``@`` and the reductions then
-    return a marker."""
+    """True while ``mapslices`` / ``ppeval`` call ``f`` on slice tracers: ``sort``, ``svdvals``, ``eigvals``, ``det``, ``@``, ``ldiv`` and
+    the reductions then return a marker."""
     return SLICE_TRACING[0] > 0
 
 
@@ -58,8 +59,19 @@ class SliceEigvals:
     """``f(slice) = eigvals(slice)``."""
 
 
+class SliceDet:
+    """``f(slice) = det(slice)``."""
+
+
 class SliceMatmul:
     """``f(slices...) = a * b`` (Julia's matrix product, Python's ``@``): each operand a slice tracer or a host array."""
+
+    def __init__(self, a, b):
+        self.a, self.b = a, b
+
+
+class SliceLdiv:
+    """``f(slices...) = a \\ b`` (Julia's left division, ``dab.ldiv``): each operand a slice tracer or a host array."""
 
     def __init__(self, a, b):
         self.a, self.b = a, b
@@ -126,6 +138,28 @@ def matmul_of_slices(a, b):
     if not tracing():
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "a matrix product of a traced expression is only served inside ppeval")
     return SliceMatmul(a, b)
+
+
+def det(A):
+    """``det`` of a square slice: ``ppeval(det, D)`` or ``mapslices(det, D, dims=(d1, d2))``.  There is no distributed determinant;
+    anywhere else this raises.  A triangular slice gives the product of its diagonal, any other the product of its LU factor's diagonal
+    with the sign of the row swaps (exactly +0.0 for a zero pivot); det never raises for singular or non-finite input."""
+    if isinstance(A, Expr) and tracing():
+        if not _is_slice(A):
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "det of an expression of the slice is not served")
+        return SliceDet()
+    raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "det is served for the slices of a DArray only: ppeval(det, D) or "
+                                "mapslices(det, D, dims=(d1, d2))")
+
+
+def ldiv(a, b):
+    """Julia's ``a \\ b`` of slices (Python has no ``\\``): ``ppeval(ldiv, A, B)``, either operand possibly a broadcast host array.  A
+    diagonal slice gives ``b ./ d``, a triangular one is solved by substitution, any other through its pivoted LU factorization;
+    ``SingularException(i)`` for a zero diagonal entry or pivot, ``ArgumentError`` for a NaN / Inf in a slice that needs the LU path.
+    Anywhere else this raises."""
+    if tracing() and (isinstance(a, Expr) or isinstance(b, Expr)):
+        return SliceLdiv(a, b)
+    raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, "ldiv is served for the slices of a DArray only: ppeval(ldiv, A, B)")
 
 
 # ---- the rules of Base.mapslices ----------------------------------------------------------------------------------------------------
@@ -209,7 +243,7 @@ class _Plan:
             return (min(sl),)
         if self.kind == "eigvals":
             return (sl[0],)
-        if self.kind == "reduce":
+        if self.kind in ("reduce", "det"):
             return ()
         return tuple(self.const.shape)
 
@@ -228,7 +262,7 @@ def _classify(f, D: DArray, dims: Tuple[int, ...]) -> _Plan:
         raise
     except Exception as e:  # noqa: BLE001 - anything f does with the tracer that is not a served form
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"mapslices: {getattr(f, '__name__', f)!r} is not a served slice function "
-                                    f"({type(e).__name__}: {e}); served: sort, svdvals, sum/prod/maximum/minimum of an elementwise "
+                                    f"({type(e).__name__}: {e}); served: sort, svdvals, eigvals, det, sum/prod/maximum/minimum of an elementwise "
                                     "expression of the slice, elementwise expressions, constant results") from None
     finally:
         SLICE_TRACING[0] -= 1
@@ -240,6 +274,14 @@ def plan_of(r, dims: Tuple[int, ...], dt: np.dtype, what: str = "mapslices") -> 
     from ._mapreduce import _result_dtype, classify_map
     if isinstance(r, SliceMatmul):
         raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what}: matrix products of slices are served by ppeval(*, A, B) only")
+    if isinstance(r, SliceLdiv):
+        raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what}: ldiv (a \\ b) of slices is served by ppeval(ldiv, A, B) only")
+    if isinstance(r, SliceDet):
+        if len(dims) != 2:
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what}(det) is served for matrix slices (two slice dimensions), got dims {dims}")
+        if dt not in _SORT_DTYPES:
+            raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what}(det): eltype {dt} (served: Float32 Float64 Int32 Int64)")
+        return _Plan("det", dims, dt if dt.kind == "f" else np.dtype(np.float64))
     if isinstance(r, SliceEigvals):
         if len(dims) != 2:
             raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what}(eigvals) is served for matrix slices (two slice dimensions), got "
@@ -290,18 +332,21 @@ def _sort_chunk(rt, plan: _Plan, ch: B200Array, out: B200Array):
 
 
 def _packed_chunk(rt, plan: _Plan, ch: B200Array, out: B200Array, status_ptr: int, temps: List[B200Array]):
-    """svdvals / eigvals: the slices packed as (m, n, batch), one batched kernel, the (k, batch) values scattered into the chunk."""
+    """svdvals / eigvals / det: the slices packed as (m, n, batch), one batched kernel, the (k, batch) values scattered into the chunk."""
     d1, d2 = plan.dims
     s = ch.shape
     m, n = s[d1 - 1], s[d2 - 1]
-    k = min(m, n)
+    k = 1 if plan.kind == "det" else min(m, n)
     wdt = plan.dtype
+    if plan.kind == "det" and n == 0:                              # det of a 0 x 0 matrix is one(T): no kernel
+        out.copy_from_host(np.ones(out.shape, dtype=wdt))
+        return
     src = ch
     if ch.dtype != wdt:                                            # svdvals / eigvals(::Matrix{Int}) work on Float64
         src = B200Array.empty(rt, s, wdt, temp=True)
         temps.append(src)
         run_local(rt, convert(Expr("arg", (), tag_of(ch.dtype), 0), tag_of(wdt)), src, [LocalArg(ch, None, tag_of(ch.dtype))])
-    batch = ch.size // (m * n)
+    batch = int(np.prod([s[j] for j in range(len(s)) if j not in (d1 - 1, d2 - 1)]))
     packed = B200Array.empty(rt, (m * n * batch,), wdt, temp=True)
     S = B200Array.empty(rt, (k * batch,), wdt, temp=True)
     temps += [packed, S]
@@ -321,6 +366,8 @@ def _packed_chunk(rt, plan: _Plan, ch: B200Array, out: B200Array, status_ptr: in
     _gather(rt, es, packed.ptr, pstr, src.ptr, _dense_strides(s), s)                 # slices -> (m, n, batch)
     if plan.kind == "svdvals":
         _lib.call("dab_svdvals_batched", rt.ctx, dab_dtype(wdt), C.c_void_p(packed.ptr), m, n, batch, C.c_void_p(S.ptr), C.c_void_p(status_ptr))
+    elif plan.kind == "det":
+        _lib.call("dab_det_batched", rt.ctx, dab_dtype(wdt), n, C.c_void_p(packed.ptr), n * n, C.c_void_p(S.ptr), batch)
     else:
         _lib.call("dab_eigvals_sym_batched", rt.ctx, dab_dtype(wdt), C.c_void_p(packed.ptr), n, batch, C.c_void_p(S.ptr), C.c_void_p(status_ptr))
     _gather(rt, es, out.ptr, _dense_strides(out.shape), S.ptr, sstr, out.shape)      # (k, 1, batch) -> the result chunk
@@ -355,7 +402,7 @@ def _const_chunk(rt, plan: _Plan, cdev: B200Array, out: B200Array):
 
 def check_limits(plan: _Plan, shapes, what: str = "mapslices"):
     """The kernels' limits on the slices of chunks of ``shapes``, checked before anything is launched."""
-    if plan.kind not in ("svdvals", "eigvals"):
+    if plan.kind not in ("svdvals", "eigvals", "det"):
         return
     d1, d2 = plan.dims
     for s in shapes:
@@ -363,18 +410,29 @@ def check_limits(plan: _Plan, shapes, what: str = "mapslices"):
         if plan.kind == "svdvals" and (min(m, n) > _lib.SVDVALS_MAX_K or m * n > _lib.SVDVALS_MAX_ELEMS):
             raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what}(svdvals): slices of {m}x{n}; served: min(m,n) <= "
                                         f"{_lib.SVDVALS_MAX_K} and m*n <= {_lib.SVDVALS_MAX_ELEMS}")
-        if plan.kind == "eigvals":
+        if plan.kind in ("eigvals", "det"):
             if m != n:                                             # LinearAlgebra.checksquare
                 raise _lib.DimensionMismatch(_lib.ERR_DIM_MISMATCH, f"matrix is not square: dimensions are ({m}, {n})")
-            if n > _lib.EIGVALS_SYM_MAX_N:
-                raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what}(eigvals): slices of {m}x{n}; served: n <= {_lib.EIGVALS_SYM_MAX_N}")
+            lim = _lib.EIGVALS_SYM_MAX_N if plan.kind == "eigvals" else _lib.LU_MAX_N
+            if n > lim:
+                raise _lib.UnsupportedError(_lib.ERR_UNSUPPORTED, f"{what}({plan.kind}): slices of {m}x{n}; served: n <= {lim}")
 
 
-def raise_on_status(rt, flags: int):
-    """The status words of dab_svdvals_batched / dab_eigvals_sym_batched, ORed over this rank's chunks: every rank raises, or none."""
-    if rt.world > 1:                                               # the ranks stay in step
-        for f in rt.allgather_object(flags):
+def raise_on_status(rt, flags: int, first=None):
+    """The status words of dab_svdvals_batched / dab_eigvals_sym_batched, ORed over this rank's chunks, and ``first``, this rank's first
+    failing ``ldiv`` slice as ``(order, info)`` (``info`` 0 for a NaN / Inf on the LU path) or None: every rank raises the same
+    exception, or none.  ``order`` sorts the slices as the result's last dimension does, so the failure raised is the lowest of all ranks'."""
+    if rt.world > 1:                                               # the ranks stay in step: one gather of both
+        firsts = []
+        for f, fi in rt.allgather_object((flags, first)):
             flags |= int(f)
+            if fi is not None:
+                firsts.append(tuple(fi))
+        first = min(firsts) if firsts else None
+    if first is not None:
+        if first[-1] == 0:
+            raise _lib.ArgumentError(_lib.ERR_ARG, "ArgumentError: matrix contains Infs or NaNs")
+        raise _lib.SingularException(first[-1])
     if flags & 1:
         raise _lib.ArgumentError(_lib.ERR_ARG, "ArgumentError: matrix contains Infs or NaNs")
     if flags & 2:
@@ -386,7 +444,7 @@ def run_chunk(rt, plan: _Plan, ch: B200Array, out: B200Array, status_ptr: int, c
     """One chunk of a mapslices plan: ``out`` (already of the result shape) from ``ch``."""
     if plan.kind == "sort":
         _sort_chunk(rt, plan, ch, out)
-    elif plan.kind in ("svdvals", "eigvals"):
+    elif plan.kind in ("svdvals", "eigvals", "det"):
         _packed_chunk(rt, plan, ch, out, status_ptr, temps)
     elif plan.kind == "reduce":
         _reduce_chunk(rt, plan, ch, out, temps)

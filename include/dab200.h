@@ -567,6 +567,26 @@ int32_t dab_matmul_batched(dab_ctx* ctx, int32_t dtype, size_t m, size_t n, size
  * matrix to the general, complex eigenvalue problem, so the host runtime raises on either once it has read status. */
 int32_t dab_eigvals_sym_batched(dab_ctx* ctx, int32_t dtype, const void* A, size_t n, size_t batch, void* W, int32_t* status);
 
+/* Largest n dab_ldiv_batched / dab_det_batched serve (one fp64 matrix of a CTA's shared memory). */
+#define DAB_LU_MAX_N 64
+/* X_b = A_b \ B_b for b < batch: A_b n x n, B_b and X_b n x nrhs, dense column-major; strides in elements, 0 broadcasts that operand to
+ * every b; X_b is stored at X + b*n*nrhs and must not overlap A or B, which are only read.  ppeval(\, A, B) once the slices are packed.
+ * Julia's dispatch of `\` on a square matrix: a diagonal slice gives b ./ d (bit-exact), a lower or upper triangular one is solved by
+ * substitution, any other is factored with partial pivoting (LAPACK's idamax rule) and solved with the factors.  fp64 throughout, Float32
+ * rounded once.  status: a device uint64 set to all ones by the call; a failing slice b lowers it (atomicMin) to (b << 8) | low, with low =
+ * info (1-based) for an exactly-zero diagonal entry or pivot (Julia's SingularException(info); not raised by a diagonal slice when nrhs == 0)
+ * or 0x80 for a NaN / Inf anywhere in a slice on the LU path (ArgumentError from getrf!'s chkfinite; on the other paths NaN / Inf flow
+ * through).  The word ends as the lowest failing b; X is unspecified for failing slices.  dtypes F32 F64 and n <= DAB_LU_MAX_N, otherwise
+ * DAB_ERR_UNSUPPORTED before anything is launched.  n == 0 or batch == 0 launches nothing. */
+int32_t dab_ldiv_batched(dab_ctx* ctx, int32_t dtype, size_t n, size_t nrhs, const void* A, size_t strideA, const void* B, size_t strideB,
+                         void* X, size_t batch, void* status);
+/* D[b] = det(A_b) for b < batch, A_b n x n dense column-major at A + b*strideA (0 broadcasts): ppeval(det, D) / mapslices(det, lp,
+ * dims=(d1, d2)) once the slices are packed.  A triangular slice gives the product of its diagonal in index order; any other is factored
+ * with partial pivoting and gives the product of U's diagonal in index order, negated for an odd number of row swaps, or +0.0 when a pivot
+ * is exactly zero.  No finiteness check, no status: det never fails.  fp64 throughout, Float32 rounded once; n == 0 gives 1.  dtypes F32
+ * F64 and n <= DAB_LU_MAX_N, otherwise DAB_ERR_UNSUPPORTED. */
+int32_t dab_det_batched(dab_ctx* ctx, int32_t dtype, size_t n, const void* A, size_t strideA, void* D, size_t batch);
+
 /* ==== cross-worker combine: NCCL over NVLink (replaces Distributed.remotecall_fetch on
  *      this path only; src/mapreduce.jl:30-34, 72-80; src/darray.jl:809-815) ============== */
 /* 128-byte ncclUniqueId; rank 0 creates it, the host runtime ships it to the other workers. */

@@ -26,6 +26,7 @@
 #   (Base.sortperm: scalar getindex)  sortperm(A; dims)                    Base.sortperm(::DArray; dims), unverified   dab_sortperm_slices
 #   src/mapreduce.jl:205 mapslices(f, localpart(y), dims) mapslices_sort / svdvals_batched       dab_sort_slices / dab_svdvals_batched
 #   src/mapreduce.jl:315 _ppeval(f, localparts...; dim)   matmul_batched / eigvals_sym_batched  dab_matmul_batched / dab_eigvals_sym_batched
+#                                                         ldiv_batched / det_batched            dab_ldiv_batched / dab_det_batched
 #   (no reference method)  accumulate!(op, lp, lp; dims)   Base.accumulate! (cumsum! / cumprod!)   dab_scan
 #   src/linalg.jl:95-97,141 localpart(A)*xj, SparseMatrixCSC chunks   Base.:* (SparseB200Chunk)   dab_spmv / dab_csc_to_csr
 #   (Base._findmax: scalar getindex)  findmax(f, d) / findmin(f, d)   (DArray methods below)   dab_findminmax / dab_combine_findminmax
@@ -493,6 +494,26 @@ function eigvals_sym_batched(a::B200Array{T,3}) where {T<:Union{Float32,Float64}
     flags & 1 == 0 || throw(ArgumentError("matrix contains Infs or NaNs"))
     flags & 2 == 0 || error("eigvals: a slice is not symmetric; complex eigenvalues are not served")
     W
+end
+
+# _ppeval(f, localparts...; dim) for f = \ and f = det (K27): `batch` packed column-major n x n slices, n <= 64, stride 0 broadcasts.
+# The status word names the lowest failing slice: (b << 8) | info, or | 0x80 for a NaN / Inf on the LU path.
+function ldiv_batched(A::B200Array{T}, sa::Int, B::B200Array{T}, sb::Int, n::Int, nrhs::Int, batch::Int) where {T<:Union{Float32,Float64}}
+    X = B200Array{T,3}(undef, (n, nrhs, batch)); st = B200Array{UInt64,1}(undef, (1,))
+    check(ccall((:dab_ldiv_batched, libdab), Int32,
+                (Ptr{Cvoid}, Int32, Csize_t, Csize_t, Ptr{Cvoid}, Csize_t, Ptr{Cvoid}, Csize_t, Ptr{Cvoid}, Csize_t, Ptr{Cvoid}),
+                ctx(), dab_dtype(T), n, nrhs, A.ptr, sa, B.ptr, sb, X.ptr, batch, st.ptr), ctx())
+    w = Array(st)[1]
+    w == typemax(UInt64) || (w & 0xff == 0x80 ? throw(ArgumentError("matrix contains Infs or NaNs")) : throw(SingularException(Int(w & 0xff))))
+    X
+end
+function det_batched(a::B200Array{T,3}) where {T<:Union{Float32,Float64}}
+    n, n2, batch = size(a)
+    n == n2 || throw(DimensionMismatch("matrix is not square: dimensions are ($n, $n2)"))
+    D = B200Array{T,1}(undef, (batch,))
+    check(ccall((:dab_det_batched, libdab), Int32, (Ptr{Cvoid}, Int32, Csize_t, Ptr{Cvoid}, Csize_t, Ptr{Cvoid}, Csize_t),
+                ctx(), dab_dtype(T), n, a.ptr, n * n, D.ptr, batch), ctx())
+    D
 end
 
 # localpart(A) * Bjk, transpose(localpart(A)) * Bjk inside _matmatmul!  (src/linalg.jl:218-226): K12, wgmma 3xTF32 for Float32
