@@ -11,7 +11,9 @@ dimension (``sortperm(A; dims, by)``: 1-based global linear indices per fibre, s
 elementwise and constant slice functions), ``ppeval`` (batched slice products ``ppeval(operator.matmul, A, B)``, ``eigvals`` of symmetric
 slices, solves ``ppeval(ldiv, A, B)`` (Julia's ``A \\ B``) and determinants ``ppeval(det, A)`` / ``mapslices(det, D, dims)``, and every
 ``mapslices`` slice function), ``cumsum`` / ``cumprod`` / ``accumulate`` and their ``!`` forms
-(``cumsum_`` ...), ``Array(d)`` (``to_array``), range ``getindex``, ``d[I]`` with ``I`` a DArray of Int32 / Int64 (a gather on the GPU:
+(``cumsum_`` ...), ``Array(d)`` (``to_array``), range ``getindex``, ``permutedims(A, perm)`` /
+``permutedims(A)`` / ``permutedims_(dest, src, perm)`` (Julia's ``permutedims!``; 1-based ``perm``, N-d, a tiled permutation on the GPU),
+``d[I]`` with ``I`` a DArray of Int32 / Int64 (a gather on the GPU:
 ``v[sortperm(v)]``, ``A[findmax(A; dims)[2]]``; a DArray key holds Julia's 1-based linear indices, host Python indices stay 0-based),
 logical indexing ``d[mask]`` with a Bool DArray of ``d``'s dims, ``findall(mask)`` / ``findall(f, d)`` (1-based linear indices as a
 ``DArray{Int64}``) and ``filter(f, d)`` (stream compaction on the GPU; results are DVectors in column-major order); ``d[key] = v`` for
@@ -50,6 +52,7 @@ from ._sort import sort, sort_with_boundaries, sortperm
 from ._scan import accumulate, accumulate_, cumprod, cumprod_, cumsum, cumsum_
 from ._slices import det, eigvals, ldiv, mapslices, svdvals
 from ._ppeval import ppeval
+from ._permute import permutedims, permutedims_
 from ._sparse import SparseChunk, SparseDArray
 from .runtime import Runtime, init, myid, nworkers, runtime, workers
 

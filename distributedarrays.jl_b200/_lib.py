@@ -125,6 +125,7 @@ _SIGS = {
     "dab_scan_carrier_dtype": (_i32, [_i32, _i32, _i32, C.POINTER(_i32)]),
     "dab_copy_box": (_i32, [_vp, _i32, _vp, C.POINTER(_sz), C.POINTER(_sz), _vp, C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz)]),
     "dab_gather_box": (_i32, [_vp, _i32, _i32, _vp, C.POINTER(C.c_longlong), _pvp, _vp, C.POINTER(C.c_longlong), _pvp, C.POINTER(_sz)]),
+    "dab_permute_box": (_i32, [_vp, _i32, _i32, _vp, C.POINTER(C.c_longlong), _vp, C.POINTER(C.c_longlong), C.POINTER(_sz)]),
     "dab_index_gather": (_i32, [_vp, _i32, _vp, _vp, _i32, _sz, _i32, C.POINTER(_sz), C.POINTER(_i32), C.POINTER(_sz), _pvp, _vp]),
     "dab_compact_count": (_i32, [_vp, _vp, _sz, _sz, _vp]),
     "dab_compact": (_i32, [_vp, _i32, _vp, _vp, _sz, _sz, _vp, _vp, _i32, C.POINTER(_sz), _pvp]),

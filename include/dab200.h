@@ -346,6 +346,19 @@ int32_t dab_copy_box(dab_ctx* ctx, int32_t elem_bytes, void* dst, const size_t d
 int32_t dab_gather_box(dab_ctx* ctx, int32_t elem_bytes, int32_t ndim, void* dst, const long long* dst_strides, const void* const* dst_index,
                        const void* src, const long long* src_strides, const void* const* src_index, const size_t* extent);
 
+/* ==== dimension permutation K28 (row f18) ===================================================
+ * dst[sum_k t_k * dst_strides[k]] = src[sum_k t_k * src_strides[k]] for every coordinate t < extent: one piece of permutedims(A, perm)
+ * / permutedims!(dest, src, perm), which Base computes with one scalar getindex (one remotecall_fetch) per element on a DArray.  This
+ * is the affine part of dab_gather_box's contract, restricted to boxes where dimension 0 is contiguous in the destination
+ * (dst_strides[0] == 1) and exactly one other dimension q is contiguous in the source (src_strides[q] == 1); it replaces
+ * dab_gather_box on those pieces, whose warps would read or write with a stride.  Each CTA moves one tile of the (0, q) plane through
+ * shared memory, the other dimensions being a batch; 16-byte global accesses on both sides when dst, src, the strides outside the
+ * plane and both plane extents allow it.  ndim 2..8, elem_bytes 1, 2, 4, 8 or 16 (bytes are moved: NaN payloads and -0.0 kept);
+ * strides in elements, may be negative.  src may be a peer mapping.  Anything else returns DAB_ERR_ARG and touches nothing; a zero
+ * extent launches nothing.  One launch per call, asynchronous on the ctx stream. */
+int32_t dab_permute_box(dab_ctx* ctx, int32_t elem_bytes, int32_t ndim, void* dst, const long long* dst_strides, const void* src,
+                        const long long* src_strides, const size_t* extent);
+
 /* ==== indexed gather K22 (row f12) ==========================================================
  * out[k] = d[idx[k]] for k < n: one localpart of R = d[I::DArray{<:Integer}], which Base's generic getindex computes as
  * similar(d, axes(I)) (src/darray.jl:238) filled by scalar reads.  idx holds the matching block of I: 1-based column-major LINEAR

@@ -34,6 +34,8 @@
 #                                                         Base.getindex(::DArray, ::DArray{<:Integer})   dab_index_gather
 #   (Base getindex(A, I::AbstractArray{Bool}) / findall: scalar iteration)  d[m::DArray{Bool}], findall(m)
 #                                                         Base.getindex(::DArray, ::DArray{Bool}), Base.findall   dab_compact_count / dab_compact
+#   (Base.permutedims / permutedims!: scalar getindex)  permutedims(A, perm), permutedims!(dest, src, perm), unverified
+#                                                         Base.permutedims / Base.permutedims!   dab_permute_box / dab_gather_box
 module DArrayB200
 
 using Distributed, DistributedArrays, LinearAlgebra
@@ -748,6 +750,68 @@ function Base.setindex!(d::DArray{T,N,B200Array{T,N}}, x::Number, m::DArray{Bool
     end
     d
 end
+
+# permutedims(A, perm) / permutedims!(dest, src, perm) (row f18; Base's generic methods read a DArray with one scalar getindex per
+# element): every worker of dest fills its localpart from the pieces of src its preimage box meets (local or CUDA-IPC peer loads), one
+# launch per piece: dab_permute_box (K28), or dab_gather_box when dest's dim 1 is also contiguous in src (a batch of contiguous runs)
+# or the plane of the two contiguous dims is below the measured size.
+# Per piece the extent-1 dims are dropped and dest-adjacent dims contiguous on both sides merged, as permute_plan does in the Python
+# runtime.  A matrix with perm (2, 1) is copy(transpose(A)).  Unverified: no Julia run on a GPU yet.
+const PERMUTE_MIN_PLANE = Dict(1 => 1536, 2 => 512, 4 => 1024, 8 => 512, 16 => 512)   # below it a K28 tile is mostly idle (_permute.py)
+function permute_collapse(ext, ds, ss)
+    out = [[e, d, s] for (e, d, s) in zip(ext, ds, ss) if e != 1]
+    isempty(out) && return ([1], [1], [1])
+    merged = [out[1]]
+    for (e, d, s) in out[2:end]
+        pe, pd, ps = merged[end]
+        d == pd * pe && s == ps * pe ? (merged[end][1] = pe * e) : push!(merged, [e, d, s])
+    end
+    (getindex.(merged, 1), getindex.(merged, 2), getindex.(merged, 3))
+end
+function Base.permutedims!(dest::DArray{T,N,B200Array{T,N}}, src::DArray{T,N,B200Array{T,N}}, perm) where {T,N}
+    length(perm) == N || throw(ArgumentError("expected permutation of size $N, but length(perm)=$(length(perm))"))
+    isperm(perm) || throw(ArgumentError("input is not a permutation"))
+    all(size(dest, k) == size(src, perm[k]) for k in 1:N) || throw(DimensionMismatch("destination tensor of incorrect size"))
+    dest === src && throw(ArgumentError("permutedims!: dest and src share storage (the result would be unspecified)"))
+    owners = vec(src.pids)
+    handles = Dict(p => remotecall_fetch(() -> ipc_handle(localpart(src)), p) for p in owners)
+    asyncmap(procs(dest)) do p
+        remotecall_fetch(p) do
+            I = localindices(dest)
+            any(isempty, I) && return nothing
+            J = Vector{UnitRange{Int}}(undef, N)
+            for k in 1:N
+                J[perm[k]] = I[k]                                             # the preimage box in src
+            end
+            dstr = cumprod((1, map(length, I)[1:end-1]...))
+            for (c, q) in enumerate(owners)
+                K = src.indices[c]
+                box = map(intersect, J, K)
+                any(isempty, box) && continue
+                sstr = cumprod((1, map(length, K)[1:end-1]...))
+                sp = (q == myid() ? localpart(src).ptr : ipc_open(handles[q])) + sum((first(box[j]) - first(K[j])) * sstr[j] for j in 1:N) * sizeof(T)
+                dp = localpart(dest).ptr + sum((first(box[perm[k]]) - first(J[perm[k]])) * dstr[k] for k in 1:N) * sizeof(T)
+                e, ds, ss = permute_collapse([length(box[perm[k]]) for k in 1:N], collect(dstr), [sstr[perm[k]] for k in 1:N])
+                n = length(e)
+                q = n >= 2 && ds[1] == 1 && count(==(1), ss[2:end]) == 1 ? findlast(==(1), ss) : 0
+                if q > 0 && e[1] * e[q] >= PERMUTE_MIN_PLANE[sizeof(T)] && min(e[1], e[q]) * sizeof(T) >= 16
+                    check(ccall((:dab_permute_box, libdab), Int32, (Ptr{Cvoid}, Int32, Int32, Ptr{Cvoid}, Ptr{Clonglong}, Ptr{Cvoid}, Ptr{Clonglong},
+                                Ptr{Csize_t}), ctx(), sizeof(T), n, dp, Clonglong[ds...], sp, Clonglong[ss...], Csize_t[e...]), ctx())
+                else
+                    check(ccall((:dab_gather_box, libdab), Int32, (Ptr{Cvoid}, Int32, Int32, Ptr{Cvoid}, Ptr{Clonglong}, Ptr{Ptr{Cvoid}}, Ptr{Cvoid},
+                                Ptr{Clonglong}, Ptr{Ptr{Cvoid}}, Ptr{Csize_t}), ctx(), sizeof(T), n, dp, Clonglong[ds...], C_NULL, sp,
+                                Clonglong[ss...], C_NULL, Csize_t[e...]), ctx())
+                end
+            end
+            check(ccall((:dab_sync, libdab), Int32, (Ptr{Cvoid},), ctx()), ctx())       # the peer reads end before the owners move on
+            nothing
+        end
+    end
+    dest
+end
+Base.permutedims(A::DArray{T,N,B200Array{T,N}}, perm) where {T,N} =
+    N == 2 && Tuple(perm) == (2, 1) ? copy(transpose(A)) :
+    permutedims!(DArray(I -> B200Array{T,N}(undef, map(length, I)), ntuple(k -> size(A, perm[k]), N), procs(A)), A, perm)
 
 # user code is then unchanged:
 #   d = DArray(I -> B200Array(rand(Float32, map(length, I))), (8 * 2^30,))
