@@ -420,6 +420,13 @@ class HostMemABI:
     # -- K11
     def dab_sort(self, ctx, dtype, inp, out, tmp, n):
         n, u = int(n), _utype(dtype)
+        src, dst, t = _addr(inp), _addr(out), _addr(tmp)
+        if n and n <= 1024 and src == dst and not t:
+            return 2                                               # DAB_ERR_ARG: the in-place rank sort needs tmp
+        if n > 1024 and (not t or t == src or t == dst):
+            return 2                                               # DAB_ERR_ARG: tmp must be a distinct buffer
+        if n >= 0xFFFFF000:
+            return 6                                               # DAB_ERR_UNSUPPORTED
         if n:
             raw = _view(inp, n, u).copy()
             _view(out, n, u)[:] = radix_dec(np.sort(radix_enc(raw, dtype), kind="stable"), dtype)
@@ -435,6 +442,8 @@ class HostMemABI:
         n = int(n)
         if n == 0:
             return 0
+        if n >= 0xFFFFF000:
+            return 6                                            # DAB_ERR_UNSUPPORTED
         need = C.c_size_t()
         self.dab_sort_by_key_scratch_bytes(key_dtype, n, C.byref(need))
         assert int(scratch_bytes) >= need.value and _addr(scratch) % 16 == 0 and _addr(vals) != _addr(vals_out)

@@ -384,14 +384,14 @@ def test_last_session_gpu_tests_dry_run_on_the_host_memory_abi(hostmem, dab):
 
 def test_gpu_test_modules_against_the_host_memory_abi():
     """Host-runtime regression net: the ``-m gpu`` modules (hot path, widening, views, linalg host flows, sort, the last-session module,
-    the exact reductions, the scalar semantics, the data-movement kernels, the fused map-reduce kernel) executed in a subprocess with ``DAB_HOSTMEM=1`` -- the C ABI emulated over host memory (tests/hostmem_abi.py), everything above it
+    the exact reductions, the scalar semantics, the data-movement kernels, the fused map-reduce kernel, the sort's dispatch paths) executed in a subprocess with ``DAB_HOSTMEM=1`` -- the C ABI emulated over host memory (tests/hostmem_abi.py), everything above it
     real.  Left out: the full-size tests (GiB-sized arrays), the tests that only make sense on the device (TMA variant, pinned H2D rates,
     the GEMM kernel module, multi-GPU).  A failure here is a regression in the HOST logic; the kernels are the ``-m gpu`` tier's job."""
     import subprocess
     env = dict(os.environ, DAB_HOSTMEM="1")
     mods = ["tests/test_gpu_hotpath.py", "tests/test_gpu_widen.py", "tests/test_gpu_views.py", "tests/test_gpu_linalg.py", "tests/test_gpu_sort.py",
             "tests/test_gpu_zz_last_session.py", "tests/test_gpu_reduce_exact.py", "tests/test_gpu_scalar_semantics.py",
-            "tests/test_gpu_data_movement.py", "tests/test_gpu_mapreduce_expr.py"]
+            "tests/test_gpu_data_movement.py", "tests/test_gpu_mapreduce_expr.py", "tests/test_gpu_sort_paths.py"]
     r = subprocess.run([sys.executable, "-m", "pytest", *mods, "-m", "gpu", "-q", "-x", "-p", "no:cacheprovider", "--timeout", "600",
                         "-k", "not full_size and not tma_variant and not pinned_large and not bandwidth_shape and not transpose_large"
                               " and not copy_box_index_64"],

@@ -252,3 +252,97 @@ def test_host_sort_flow_by_with_nan_values_and_nan_keys(hostmem, dab):
                         assert np.array_equal(gb, wb, equal_nan=True) and got.layout.indices == want.indices
                         assert np.array_equal(dab.to_array(got).view(np.uint8), orc.to_array(want).view(np.uint8)), (nw, T, n)
                 d.close()
+
+
+# ---- tests/test_gpu_sort_paths.py: its digit-set data, its model and its tile-shape premise, checked without a GPU ---------------
+
+def test_sort_paths_digit_set_generator():
+    """Every named case of the onesweep path tests has exactly its intended non-constant digits, for every dtype, keys only and pairs;
+    for pairs of floats only the NaN case holds NaNs (several payloads, both signs), and those are exactly the keys that collapse to the
+    top radix key.  The outliers differ from the rest in one key, and one-digit-per-tile data is constant in digit 0 inside every tile."""
+    import test_gpu_sort_paths as sp
+    rng = np.random.default_rng(31)
+    for T in map(np.dtype, sp.DTYPES):
+        w, U = T.itemsize, sp.UINT[T.itemsize]
+        sets = sp.digit_sets(w)
+        assert sets["odd"][0] > 0 and sets["odd"][-1] < w - 1 and len(sets["odd"]) % 2 == 1
+        assert sets["even"][0] > 0 and sets["even"][-1] < w - 1 and len(sets["even"]) % 2 == 0
+        for pairs in (False, True):
+            tile = (sp.PAIRS_TILE if pairs else sp.KEYS_TILE)[w]
+            for n in (1025, 3 * tile + 1):
+                for name in sp.SMALL_NAMES:
+                    a, act, outl = sp.make_case(T, name, n, tile, rng, pairs)
+                    assert a.dtype == T and a.size == n
+                    sp.check_premise(a, act, outl, pairs)
+                    if name in sets:
+                        assert act == sets[name]
+                    r = sp.pairs_radix(a) if pairs else sp.keys_radix(a)
+                    if outl is not None:                                    # one key differs from the n - 1 others
+                        assert sorted(np.unique(r, return_counts=True)[1]) == [1, n - 1]
+                    if name == "tile_digit":
+                        d0 = (r & U(0xFF)).astype(np.int64)
+                        t = np.arange(n) // tile
+                        assert np.array_equal(d0, t * 97 % 256)
+                    if pairs and T.kind == "f":
+                        nan = np.isnan(a)
+                        assert np.array_equal(nan, r == ~U(0))
+                        if name == "all_nan":
+                            raw = a.view(U)
+                            assert nan.any() and np.unique(raw[nan]).size > 10 and np.unique(raw[nan] >> U(8 * w - 1)).size == 2
+                        else:
+                            assert not nan.any()
+    # the premise check itself: a digit with one odd key out is non-constant, a constant one is not
+    k = np.full(5000, 0x11223344, dtype=np.uint32)
+    assert sp.active_digits(k) == ()
+    k[4999] = 0x11223345
+    assert sp.active_digits(k) == (0,) and sp.largest_bin(k, 0) == 4999
+
+
+def test_sort_paths_model_matches_oracle():
+    """The model of the path tests against the oracle: dec(sort(enc)) is Julia's sort on NaN-free data (signed zeros, infinities, ties),
+    and the stable argsort of the collapsed key is Julia's stable sortperm (NaNs equal to each other) with or without NaNs."""
+    import hostmem_abi as hm
+    import test_gpu_sort_paths as sp
+    rng = np.random.default_rng(32)
+    for T in map(np.dtype, sp.DTYPES):
+        for name in ("all", "odd", "low_top", "outlier_first", "tile_digit"):
+            a, _, _ = sp.make_case(T, name, 20000, sp.PAIRS_TILE[T.itemsize], rng, pairs=True)     # NaN-free
+            a = a.copy()
+            a[rng.integers(0, a.size, 2000)] = a[rng.integers(0, a.size, 2000)]                   # ties
+            if T.kind == "f":
+                a[rng.integers(0, a.size, 300)] = rng.choice(np.array([0.0, -0.0, np.inf, -np.inf], dtype=T), 300)
+            U = sp.UINT[T.itemsize]
+            assert np.array_equal(sp.model_sort(a), orc.jl_sort(a).view(U)), (T, name)
+            perm, ek = sp.model_pairs(a)
+            assert np.array_equal(perm, orc.jl_sortperm_stable(a)), (T, name)
+            assert np.array_equal(hm.radix_dec(ek, sp.CODE[T]), orc.jl_sort(a).view(U))
+        if T.kind == "f":
+            a, _, _ = sp.make_case(T, "all_nan", 20000, sp.PAIRS_TILE[T.itemsize], rng, pairs=True)
+            assert np.isnan(a).any()
+            assert np.array_equal(sp.model_pairs(a)[0], orc.jl_sortperm_stable(a))
+
+
+def test_sort_paths_tile_shapes_match_the_kernel():
+    """The tile sizes and residency the path tests build their size classes from are the ones dab_sort.cu instantiates: keys only 256 x 32
+    (4-byte keys) and 256 x 16 (8-byte), pairs 256 x 16 and 256 x 10, each at most 3 CTAs per SM by its shared memory (228 KiB per H100
+    SM, 1 KiB of it reserved per CTA), so that the persistent class really gives every resident CTA 4 or more tiles."""
+    import os
+    import re
+
+    import test_gpu_sort_paths as sp
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    src = open(os.path.join(root, "distributedarrays.jl_b200", "csrc", "dab_sort.cu")).read()
+    body = src[src.index("int32_t sort_t("):]
+    body = body[:body.index("\n}\n")]
+    pairs_part = body[body.index("if constexpr (!std::is_void<P>::value)"):body.index("} else if constexpr (sizeof(U) == 8)")]
+    keys_part = body[body.index("} else if constexpr (sizeof(U) == 8)"):]
+    inst = r"sort_passes<T, P, (\d+), (\d+), (\d+)>"
+    smem_line = ("constexpr size_t smem = 2 * (size_t)TILE * (sizeof(U) + (PAIRS ? 4 : 0)) + (size_t)(THREADS / 32) * 1024 + 1024 + 32;")
+    assert smem_line in src
+    for part, tiles, pair_bytes in ((pairs_part, sp.PAIRS_TILE, 4), (keys_part, sp.KEYS_TILE, 0)):
+        got = [tuple(map(int, m)) for m in re.findall(inst, part)]
+        assert len(got) == 2, got
+        for (threads, kpt, minb), width in zip(got, (8, 4)):                # the 8-byte branch comes first in both
+            assert threads * kpt == tiles[width] and minb == sp.CTAS_PER_SM
+            smem = 2 * threads * kpt * (width + pair_bytes) + threads // 32 * 1024 + 1024 + 32
+            assert smem <= 227 * 1024 and (228 * 1024) // (smem + 1024) <= sp.CTAS_PER_SM, (width, pair_bytes, smem)
