@@ -58,6 +58,8 @@ __host__ __device__ __forceinline__ FmKey<T> order_key(T v) {
     }
 }
 
+// Strict in the index: of two entries with equal key and index (index inputs that carry one index twice) the accumulator keeps the one
+// it holds, so a walk or fold in position order keeps the earlier one.
 template <typename U>
 __host__ __device__ __forceinline__ bool fm_better(U ka, unsigned long long ia, U kb, unsigned long long ib) {
     return ka > kb || (ka == kb && ia < ib);

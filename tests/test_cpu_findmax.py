@@ -135,6 +135,101 @@ def test_gpu_findmax_module_against_the_host_memory_abi():
     assert m and int(m.group(1)) >= 30, tail
 
 
+def test_gpu_findmax_paths_module_against_the_host_memory_abi():
+    """tests/test_gpu_findmax_paths.py with the C ABI emulated over host memory: its case designs, premises, guard bands and refusal
+    statuses against the same model (the 2 GiB cases skip)."""
+    env = dict(os.environ, DAB_HOSTMEM="1")
+    r = subprocess.run([sys.executable, "-m", "pytest", "tests/test_gpu_findmax_paths.py", "-m", "gpu", "-q", "-x", "-p", "no:cacheprovider"],
+                       cwd=ROOT, env=env, capture_output=True, text=True, timeout=1500)
+    tail = "\n".join((r.stdout + r.stderr).splitlines()[-25:])
+    assert r.returncode == 0, tail
+    m = re.search(r"(\d+) passed", r.stdout)
+    assert m and int(m.group(1)) >= 130, tail
+
+
+@pytest.mark.parametrize("sm_count", [132, 114, 16, fo.MIN_SM_COUNT])
+def test_case_table_reaches_every_label_from_the_minimum_sm_count(sm_count):
+    """The launch model reaches every label from the case table of tests/test_gpu_findmax_paths.py at the SM counts of the H100 SXM (132)
+    and PCIe (114), of a 16-SM partition and at the table's minimum; each case reaches the label it is named for, and Bool never takes the
+    16-byte kernel."""
+    seen = set()
+    for case in fo.case_table(sm_count):
+        for dt in (np.float32, np.float64, np.int32, np.int64, np.bool_):
+            labels = fo.case_labels(case, dt, sm_count)
+            want = "bool_vec_shape" if dt == np.bool_ and case[1] in ("vec", "vec_split") else case[1]
+            assert want in labels, (case[0], np.dtype(dt).name, labels)
+            assert dt != np.bool_ or not any(l.startswith("vec") for l in labels)
+            seen |= labels
+    assert seen == fo.ALL_LABELS, fo.ALL_LABELS ^ seen
+
+
+def test_no_pass_leaves_a_split_empty_below_the_minimum_sm_count():
+    """Below fo.MIN_SM_COUNT SMs a pass gets at most 256 splits of at least 256 elements, so none is empty: the case table refuses to be
+    built there, rather than claim a label it cannot reach."""
+    sm = fo.MIN_SM_COUNT - 1
+    with pytest.raises(ValueError):
+        fo.case_table(sm)
+    for inner in (1, 2, 5, 300):
+        for red in list(range(256, 256 * 300, 37)) + [256 * 256 + k for k in range(-3, 4)]:
+            assert not fo.fmdim_plan(np.float32, inner, red, 1, 0, False, sm)["empty"], (inner, red)
+    assert fo.fmdim_plan(np.float32, 2, 256 * 288 + 1, 1, 0, False, fo.MIN_SM_COUNT)["empty"]
+
+
+def test_launch_model_on_literal_plans():
+    """fmdim_plan on hand-worked plans: the split count and bounds, an empty split, the launch count and the grid that loops."""
+    p = fo.fmdim_plan(np.float32, 2, 306200, 1, 0, False, 132)        # 1024 splits of 300: the last three are empty
+    assert p["kernel"] == "strided" and p["nsplit"] == 1024 and p["bounds"][1020] == (306000, 306200) and p["empty"]
+    assert [hi <= lo for lo, hi in p["bounds"]].count(True) == 3 and p["launches"] == 2
+    p = fo.fmdim_plan(np.float32, 1, 12293, 3, 0, False, 132)          # lead32: 6 splits of 2049, the last 2048
+    assert (p["kernel"], p["G"], p["nsplit"], p["bounds"][-1]) == ("lead", 32, 6, (10245, 12293))
+    assert fo.fmdim_plan(np.float32, 1, 65536, 1, 0, False, 132)["launches"] == 2
+    assert fo.fmdim_plan(np.float32, 1, 65536, 1, 0, True, 132)["kernel"] == "lead"   # never the whole-chunk kernel with an index input
+    assert fo.fmdim_plan(np.float64, 16384, 3, 1, 0, False, 132)["vec"]
+    assert not fo.fmdim_plan(np.float64, 16384, 3, 1, 8, False, 132)["vec"]          # one element off 16 bytes
+    assert fo.fmdim_plan(np.int32, 1, 5, 132 * 8 * 64 + 1, 0, False, 132)["loops"]
+    assert not fo.fmdim_plan(np.int32, 1, 5, 132 * 8 * 64, 0, False, 132)["loops"]
+    g = fo.flat_grid(np.float32, 8, 2 + 3 * 4096 + 5 * 4 + 3)
+    assert (g["head"], g["tiles"], g["grid"], g["tiles_per_cta"], g["rem_vecs"], g["tail"]) == (2, 3, 2, 2, 5, 3)
+
+
+def test_emulated_index_input_pass_is_the_sequential_loop():
+    """The emulated dab_findminmax_dim with an index input (a later pass, or the fold on the owner) against ``seq_find`` over the whole
+    original run: the earlier pass's (value, 1-based index) of random groups of positions, in random order, with "no element" entries (-1)
+    mixed in, for every dtype and both functions."""
+    import ctypes as C
+    import hostmem_abi as hm
+    rng = np.random.default_rng(31)
+    emu = hm.HostMemABI()
+    codes = {np.float32: hm.F32, np.float64: hm.F64, np.int32: hm.I32, np.int64: hm.I64, np.bool_: hm.U8}
+    for trial in range(300):
+        dtype = list(codes)[trial % 5]
+        which = (fo.FINDMAX, fo.FINDMIN)[(trial // 5) % 2]
+        inner, n = int(rng.integers(1, 4)), int(rng.integers(1, 30))
+        ngroups = int(rng.integers(1, n + 1))
+        red = ngroups + int(rng.integers(0, 3))
+        X = np.empty((inner, red, 1), dtype=dtype)
+        II = np.full((inner, red, 1), -1, dtype=np.int64)
+        wants = []
+        for i in range(inner):
+            A = _specials(rng, dtype, n)
+            g = rng.integers(0, ngroups, n)
+            g[:ngroups] = np.arange(ngroups)                     # no group is empty
+            slots = rng.permutation(red)[:ngroups]               # the pass's entries in an order of their own; the rest are -1
+            X[i, :, 0] = A[0]
+            for k in range(ngroups):
+                members = np.nonzero(g == k)[0]
+                v, j = fo.seq_find(which, A[members])
+                X[i, slots[k], 0], II[i, slots[k], 0] = v, members[j] + 1
+            wants.append(fo.seq_find(which, A))
+        ov, oi = np.zeros(inner, dtype=dtype), np.zeros(inner, dtype=np.int64)
+        vp = lambda a: C.c_void_p(a.ctypes.data)
+        xs, iis = np.asfortranarray(X), np.asfortranarray(II)
+        st = fo.dab_findminmax_dim(emu, None, codes[dtype], which, 0, vp(xs), vp(iis), inner, red, 1, 0, None, None, None, vp(ov), vp(oi))
+        assert st == 0
+        for i, (v, j) in enumerate(wants):
+            assert fo.same_bits(ov[i:i + 1], np.asarray([v])) and oi[i] == j + 1, (trial, i, ov[i], oi[i], v, j)
+
+
 def test_dab_findminmax_compiles_without_stack_or_spills():
     """``nvcc -Xptxas -v`` of dab_findminmax.cu for sm_90a: no entry function uses a stack frame or spills."""
     import shutil
